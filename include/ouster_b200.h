@@ -50,7 +50,8 @@ typedef struct ob_decoder ob_decoder; /* device-resident PacketFormat decode tab
 /* ---- library ---- */
 int ob_abi_version(void);
 /* sizeof() of a public struct by name ("ob_cloud_io", "ob_field_desc", "ob_packet_layout",
- * "ob_decode_io", "ob_decode_batch", "ob_dewarp_frame_io", "ob_normals_io", "ob_encode_io", "ob_dewarp_frames_io"); 0 for unknown names.  Lets FFI bindings verify their layout. */
+ * "ob_decode_io", "ob_decode_batch", "ob_dewarp_frame_io", "ob_normals_io", "ob_encode_io", "ob_dewarp_frames_io",
+ * "ob_voxel_io"); 0 for unknown names.  Lets FFI bindings verify their layout. */
 size_t ob_abi_sizeof(const char* struct_name);
 const char* ob_last_error(void);
 /* number of visible CUDA devices (0 without a driver/GPU); never fails */
@@ -58,7 +59,7 @@ int ob_device_count(void);
 /* kernels launched by this library since load (all threads); the bench's gpu_launches claim */
 uint64_t ob_kernel_launch_count(void);
 /* launches of one named kernel family since load: "decode_pipe" (pipelined K2), "decode" (K2, any
- * kernel), "cloud" (K1); 0 for unknown names.  Lets tests assert which code path ran. */
+ * kernel), "cloud" (K1), "normals", "voxel"; 0 for unknown names.  Lets tests assert which code path ran. */
 uint64_t ob_kernel_launch_count_of(const char* name);
 /* tuning hook (launch geometry and code-path selection only, never results): cloud_tw, cloud_stages,
  * cloud_threads (compute threads; a copy warp is added), cloud_ctas_per_sm, cloud_store_lag,
@@ -226,6 +227,54 @@ typedef struct ob_normals_io {
     double* vertical_subtent_out;      /* optional, n_frames doubles: the per-pixel vertical subtent used */
 } ob_normals_io;
 ob_status ob_normals(ob_dtype dtype, const ob_normals_io* io, ob_stream* s);
+
+/* ---- voxel-grid downsampling (SURVEY 8f-2, the prefilter beside normals) ----
+ * replaces core::voxel_downsample(frame, voxel_size)      ouster_core/src/voxel_hash_map.cpp:262-310   (SHUFFLE_FIRST)
+ *          core::voxel_downsample_3d / _xd(frame, ...)     ouster_core/src/voxel_hash_map.cpp:312-393   (FIRST_N_POINT,
+ *                                                          AVERAGE_POINT, RANDOM; voxel_hash_map.h:287-334, 587-635)
+ *          algorithm::voxel_downsample_with_normals        ouster_algorithm/src/voxel_downsample.cpp:21-57 (POINT_NORMAL;
+ *                                                          PointNormalBucket, voxel_hash_map.h:142-185)
+ * Voxel of a row: floor(p * (1.0 / voxel_size)) on columns 0-2, cast to int32 with NaN / out-of-range -> INT32_MIN
+ * (x86 cvttsd2si, what the reference compiles to).  float32 inputs are widened exactly; outputs are float64.
+ * Output order: SHUFFLE_FIRST is the reference's order exactly (points_out / indices_out); the other modes emit
+ * voxels in the order of their first row in the input (the reference: tsl::robin_map iteration order), inside a
+ * voxel in the bucket's slot order.  indices_out (optional) = source row of every output row (for AVERAGE_POINT
+ * and POINT_NORMAL: the voxel's first row).  Every mode except POINT_NORMAL returns an empty result for an empty
+ * input before any check; POINT_NORMAL skips rows with a non-finite point or normal or a normal of norm <= 1e-12.
+ * Row count: n (host) or, when n_device is set, a device word read in stream order (values above `capacity` are
+ * clamped; work is launched for `capacity` rows, parameters are checked whenever capacity > 0).  n_out may be
+ * host memory (the call synchronises once and host outputs are final on return) or device memory (nothing waits;
+ * all outputs must then be device memory).  Output buffers hold `capacity` (or n) rows.
+ * errors (OB_INVALID_ARGUMENT, the reference's std::invalid_argument texts): "max_points_per_voxel must be greater
+ * than 0" (checked first), "voxel_size must be greater than 0", "voxel_downsample_xd: frame must have at least 3
+ * columns", "voxel_downsample_with_normals expects Nx3 inputs", "voxel_downsample_with_normals voxel_size must be > 0".
+ */
+typedef enum ob_voxel_mode {
+    OB_VOXEL_FIRST_N_POINT = 0, /* VoxelDownsampleStrategy::FIRST_N_POINT */
+    OB_VOXEL_AVERAGE_POINT = 1, /* VoxelDownsampleStrategy::AVERAGE_POINT */
+    OB_VOXEL_RANDOM = 2,        /* VoxelDownsampleStrategy::RANDOM */
+    OB_VOXEL_SHUFFLE_FIRST = 3, /* core::voxel_downsample */
+    OB_VOXEL_POINT_NORMAL = 4   /* algorithm::voxel_downsample_with_normals */
+} ob_voxel_mode;
+
+typedef struct ob_voxel_io {
+    int32_t mode;                /* ob_voxel_mode */
+    int32_t dtype;               /* ob_dtype of points / normals */
+    const void* points;          /* rows x cols */
+    size_t cols;                 /* >= 3 (3 for SHUFFLE_FIRST and POINT_NORMAL); columns 0-2 are x, y, z */
+    const void* normals;         /* POINT_NORMAL: rows x 3 */
+    size_t n;                    /* row count when n_device is NULL */
+    const size_t* n_device;      /* optional device-resident row count (e.g. ob_dewarp_frames' n_points) */
+    size_t capacity;             /* rows the input buffers hold; used with n_device */
+    double voxel_size;
+    size_t max_points_per_voxel; /* FIRST_N_POINT, RANDOM (reference default 1) */
+    size_t min_pts_threshold;    /* AVERAGE_POINT (reference default 1) */
+    double* points_out;          /* rows x cols float64 (POINT_NORMAL: x 3) */
+    double* normals_out;         /* POINT_NORMAL, optional: rows x 3 float64 unit normals */
+    uint32_t* indices_out;       /* optional: rows */
+    size_t* n_out;               /* rows written; host or device memory */
+} ob_voxel_io;
+ob_status ob_voxel_downsample(const ob_voxel_io* io, ob_stream* s);
 
 /* ---- fused range -> (XYZ, destaggered range, destaggered XYZ), batched over frames ----
  * One launch performs, for every frame f and return r of the batch, what the reference does as

@@ -46,6 +46,16 @@ class NormalsIO(C.Structure):
                 ("vertical_subtent_rad", C.c_double), ("vertical_subtent_out", vp)]
 
 
+class VoxelIO(C.Structure):
+    _fields_ = [("mode", C.c_int32), ("dtype", C.c_int32), ("points", vp), ("cols", sz), ("normals", vp),
+                ("n", sz), ("n_device", vp), ("capacity", sz), ("voxel_size", C.c_double),
+                ("max_points_per_voxel", sz), ("min_pts_threshold", sz), ("points_out", vp), ("normals_out", vp),
+                ("indices_out", vp), ("n_out", vp)]
+
+
+OB_VOXEL_FIRST_N_POINT, OB_VOXEL_AVERAGE_POINT, OB_VOXEL_RANDOM, OB_VOXEL_SHUFFLE_FIRST, OB_VOXEL_POINT_NORMAL = range(5)
+
+
 class DewarpFramesIO(C.Structure):
     _fields_ = [("lut", vp), ("range", vp), ("poses", vp), ("status", vp), ("timestamps", vp)]
 
@@ -125,6 +135,7 @@ _sig("ob_dewarp", i32, i32, vp, vp, sz, sz, vp, vp)
 _sig("ob_scan_to_cloud", i32, vp, vp, sz, C.POINTER(CloudIO), vp)
 _sig("ob_dewarp_frame", i32, vp, C.POINTER(DewarpFrameIO), C.POINTER(sz), vp)
 _sig("ob_normals", i32, i32, C.POINTER(NormalsIO), vp)
+_sig("ob_voxel_downsample", i32, C.POINTER(VoxelIO), vp)
 _sig("ob_dewarp_frames", i32, C.POINTER(DewarpFramesIO), sz, C.c_double, C.c_double, vp, sz, vp, vp, vp,
      C.POINTER(sz), C.POINTER(sz), vp)
 if hasattr(lib, "ob_decoder_create"):

@@ -469,6 +469,87 @@ def normals(xyz, rng, *args, sensor_origins_xyz=None, pixel_search_range=1,
     return (res, float(sub[0])) if return_subtent else res
 
 
+VOXEL_MODES = {"first_n": _capi.OB_VOXEL_FIRST_N_POINT, "average": _capi.OB_VOXEL_AVERAGE_POINT,
+               "random": _capi.OB_VOXEL_RANDOM, "shuffle_first": _capi.OB_VOXEL_SHUFFLE_FIRST,
+               "point_normal": _capi.OB_VOXEL_POINT_NORMAL}
+
+
+def voxel_downsample(points, voxel_size, mode="shuffle_first", normals=None, max_points_per_voxel=1,
+                     min_pts_threshold=1, n=None, stream=None, device=0):
+    """Voxel-grid downsampling on the GPU (ob_voxel_downsample), one of VOXEL_MODES:
+      "shuffle_first"  core::voxel_downsample(frame, voxel_size) (voxel_hash_map.cpp:262-310), the reference's
+                       output order and indices exactly;
+      "first_n" / "average" / "random"  core::voxel_downsample_xd with that VoxelDownsampleStrategy (:312-393);
+      "point_normal"   algorithm::voxel_downsample_with_normals (voxel_downsample.cpp:21-57), `normals` [n, 3].
+    points: [n, cols] float32 / float64 (voxel from columns 0-2), numpy or torch (CUDA tensors stay on the device).
+    Returns (points [m, cols] float64, indices [m] uint32 -- int32 on the device), with the normals [m, 3] between
+    them for "point_normal".  Voxels come out in the order of their first input row (DESIGN 9).
+    n: optional device-resident row count (CUDA integer tensor of one int64, e.g. dewarp_frame's out_count); then
+    `points` is a buffer of `capacity` rows, nothing waits for the GPU, and the result is capacity-row buffers plus
+    a CUDA int64 [1] count of the valid rows, appended to the tuple.  ValueError texts of the reference."""
+    from ._capi import VoxelIO
+    m = VOXEL_MODES[mode]
+    on_dev = _is_torch(points) and points.is_cuda
+
+    def prep(a):
+        if _is_torch(a):
+            import torch
+            return (a if a.dtype in (torch.float32, torch.float64) else a.double()).contiguous()
+        a = np.ascontiguousarray(a)
+        return a if a.dtype in (np.float32, np.float64) else a.astype(np.float64)
+
+    points = prep(points)
+    if len(points.shape) != 2:
+        raise ValueError("points must be [n, cols]")
+    rows, cols = int(points.shape[0]), int(points.shape[1])
+    dt = _np_dtype(points)
+    nrm = None
+    if m == _capi.OB_VOXEL_POINT_NORMAL:
+        if normals is None:
+            raise ValueError("point_normal needs normals")
+        nrm = prep(normals)
+        if _np_dtype(nrm) != dt:
+            nrm = nrm.to(points.dtype) if _is_torch(nrm) else nrm.astype(dt)
+        if tuple(nrm.shape) != (rows, 3) or cols != 3:
+            raise ValueError("voxel_downsample_with_normals expects Nx3 inputs" if cols != 3 or nrm.shape[-1] != 3
+                             else "voxel_downsample_with_normals points/normals size mismatch")
+    out_cols = 3 if m == _capi.OB_VOXEL_POINT_NORMAL else cols
+    if on_dev:
+        import torch
+        dev = points.device
+        st = stream or Stream(dev.index, cuda_stream=torch.cuda.current_stream(dev).cuda_stream)
+        out = torch.empty((rows, out_cols), dtype=torch.float64, device=dev)
+        out_n = torch.empty((rows, 3), dtype=torch.float64, device=dev) if nrm is not None else None
+        idx = torch.empty(rows, dtype=torch.int32, device=dev)
+    else:
+        if n is not None:
+            raise ValueError("a device-side row count needs device inputs")
+        st = _stream(stream, device)
+        out = np.empty((rows, out_cols), np.float64)
+        out_n = np.empty((rows, 3), np.float64) if nrm is not None else None
+        idx = np.empty(rows, np.uint32)
+    io = VoxelIO()
+    io.mode, io.dtype = m, _capi.OB_F64 if dt == np.float64 else _capi.OB_F32
+    io.points, io.cols, io.normals = _ptr(points), cols, _ptr(nrm)
+    io.voxel_size = float(voxel_size)
+    io.max_points_per_voxel, io.min_pts_threshold = int(max_points_per_voxel), int(min_pts_threshold)
+    io.points_out, io.normals_out, io.indices_out = _ptr(out), _ptr(out_n), _ptr(idx)
+    head = (out, out_n, idx) if nrm is not None else (out, idx)
+    if n is not None:
+        import torch
+        if not (_is_torch(n) and n.is_cuda and n.dtype == torch.int64 and n.numel() == 1):
+            raise ValueError("n must be a CUDA int64 tensor with one element")
+        count = torch.zeros(1, dtype=torch.int64, device=points.device)
+        io.n_device, io.capacity, io.n_out = n.data_ptr(), rows, count.data_ptr()
+        check(lib.ob_voxel_downsample(C.byref(io), st.h))
+        return head + (count,)
+    cnt = C.c_size_t(0)
+    io.n, io.n_out = rows, C.addressof(cnt)
+    check(lib.ob_voxel_downsample(C.byref(io), st.h))
+    k = cnt.value
+    return tuple(a[:k] for a in head)
+
+
 def dewarp_frames(frames, min_range=0.0, max_range=float("inf"), provenance=False, stream=None):
     """dewarp(frame_set, xyzluts, min_range, max_range) (pose_util.h:475, impl/dewarp_impl.h:84-117):
     `frames` is a list with one entry per slot of the set -- None for an empty slot, else a dict

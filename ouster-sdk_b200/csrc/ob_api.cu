@@ -16,12 +16,12 @@ namespace ob {
 static thread_local std::string g_last_error;
 static std::atomic<uint64_t> g_launches{0};
 
-static std::atomic<uint64_t> g_family[4];
-static const char* const kFamilies[4] = {"decode_pipe", "decode", "cloud", "normals"};
+static std::atomic<uint64_t> g_family[5];
+static const char* const kFamilies[5] = {"decode_pipe", "decode", "cloud", "normals", "voxel"};
 
 void count_launch(uint64_t n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 void count_launch_of(int family, uint64_t n) {
-    if (family >= 0 && family < 4) g_family[family].fetch_add(n, std::memory_order_relaxed);
+    if (family >= 0 && family < 5) g_family[family].fetch_add(n, std::memory_order_relaxed);
 }
 
 ob_status fail(ob_status st, const std::string& msg) {
@@ -323,6 +323,7 @@ size_t ob_abi_sizeof(const char* name) {
     if (n == "ob_normals_io") return sizeof(ob_normals_io);
     if (n == "ob_encode_io") return sizeof(ob_encode_io);
     if (n == "ob_dewarp_frames_io") return sizeof(ob_dewarp_frames_io);
+    if (n == "ob_voxel_io") return sizeof(ob_voxel_io);
     return 0;
 }
 
@@ -341,7 +342,7 @@ uint64_t ob_kernel_launch_count(void) { return g_launches.load(std::memory_order
 
 uint64_t ob_kernel_launch_count_of(const char* name) {
     if (!name) return 0;
-    for (int i = 0; i < 4; ++i)
+    for (int i = 0; i < 5; ++i)
         if (std::string(name) == kFamilies[i]) return g_family[i].load(std::memory_order_relaxed);
     return 0;
 }

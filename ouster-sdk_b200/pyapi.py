@@ -5,6 +5,8 @@ error behaviour as the nanobind binding (python/src/cpp/client/processing.cpp:34
     xyz = core.XYZLut(info)(scan)                 # (H, W, 3) float64, staggered
     img = core.destagger(info, scan.field("RANGE"))
 """
+import enum
+
 import numpy as np
 
 from . import core as _c
@@ -173,6 +175,69 @@ def normals(xyz, range, *args, **kwargs):
                                                        device=t.device)
     st = _c.Stream(t.device.index, cuda_stream=torch.cuda.current_stream(t.device).cuda_stream)
     return _c.normals(t.contiguous(), _dev(range), *conv, stream=st, device=t.device.index, **kwargs)
+
+
+class VoxelDownsampleStrategy(enum.IntEnum):
+    """core.VoxelDownsampleStrategy (voxel_hash_map.h:697-701, processing.cpp:959-962)."""
+    FIRST_N_POINT = 0
+    AVERAGE_POINT = 1
+    RANDOM = 2
+
+
+_STRATEGY_MODE = {VoxelDownsampleStrategy.FIRST_N_POINT: "first_n", VoxelDownsampleStrategy.AVERAGE_POINT: "average",
+                  VoxelDownsampleStrategy.RANDOM: "random"}
+
+
+def _voxel_xd(frame, voxel_size, max_points_per_voxel, min_pts_threshold, strategy, name, shape_ok, shape_msg):
+    t = _dev(frame)
+    f = t.contiguous() if t is not None else np.ascontiguousarray(frame, np.float64)
+    if len(f.shape) != 2 or not shape_ok(int(f.shape[1])):
+        raise ValueError(shape_msg)
+    if f.shape[0] == 0:   # empty frame: returned before any other check (voxel_hash_map.cpp:317, 355)
+        return f[:0].double() if t is not None else np.empty((0, f.shape[1]), np.float64)
+    try:
+        mode = _STRATEGY_MODE[VoxelDownsampleStrategy(strategy)]
+    except ValueError:
+        raise ValueError(f"{name}: unknown strategy") from None
+    return _c.voxel_downsample(f, voxel_size, mode, max_points_per_voxel=max_points_per_voxel,
+                               min_pts_threshold=min_pts_threshold)[0]
+
+
+def voxel_downsample_3d(frame, voxel_size, max_points_per_voxel=1, min_pts_threshold=1,
+                        strategy=VoxelDownsampleStrategy.RANDOM):
+    """core.voxel_downsample_3d (processing.cpp:511-523, 964-980): Nx3 in, Mx3 float64 out.  Device tensors
+    give device tensors.  Voxels come out in first-appearance order (the reference: hash-map order)."""
+    return _voxel_xd(frame, voxel_size, max_points_per_voxel, min_pts_threshold, strategy, "voxel_downsample_3d",
+                     lambda c: c == 3, "voxel_downsample_3d: frame must be Nx3")
+
+
+def voxel_downsample_xd(frame, voxel_size, max_points_per_voxel=1, min_pts_threshold=1,
+                        strategy=VoxelDownsampleStrategy.RANDOM):
+    """core.voxel_downsample_xd (processing.cpp:496-509, 982-990): NxD (D >= 3, columns 0-2 are x, y, z, the
+    rest attributes carried along) in, MxD float64 out."""
+    return _voxel_xd(frame, voxel_size, max_points_per_voxel, min_pts_threshold, strategy, "voxel_downsample_xd",
+                     lambda c: c >= 3, "voxel_downsample_xd: frame must be Nx>=3 (x,y,z + optional attributes)")
+
+
+voxel_downsample = voxel_downsample_xd   # python/src/ouster/sdk/core/__init__.py:76-78
+
+
+def voxel_downsample_with_normals(points, normals, voxel_size):
+    """algorithm.voxel_downsample_with_normals(points, normals, voxel_size) (voxel_downsample.cpp:21-57):
+    per voxel the mean position and the renormalised sum of the unit normals, as (points, normals) float64."""
+    tp = _dev(points)
+    if tp is not None:
+        tn = _dev(normals)
+        tn = tn if tn is not None else _torch().as_tensor(np.ascontiguousarray(normals), device=tp.device)
+        p, q = tp, tn
+    else:
+        p, q = np.ascontiguousarray(points, np.float64), np.ascontiguousarray(normals, np.float64)
+    if len(p.shape) != 2 or len(q.shape) != 2 or p.shape[1] != 3 or q.shape[1] != 3:
+        raise ValueError("voxel_downsample_with_normals expects Nx3 inputs")
+    if p.shape[0] != q.shape[0]:
+        raise ValueError("voxel_downsample_with_normals points/normals size mismatch")
+    out_p, out_n, _ = _c.voxel_downsample(p, voxel_size, "point_normal", normals=q)
+    return out_p, out_n
 
 
 class DeviceLidarScan:

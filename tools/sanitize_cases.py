@@ -7,6 +7,7 @@ import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import __graft_entry__ as graft
 from oracle import oracle as orc
+from oracle import voxel as orv
 from tests.helpers import (col_map_from_packets, decoder_desc_from_oracle, oracle_pf, random_frame,
                            random_lut, random_range)
 
@@ -268,4 +269,16 @@ for i, (hh, ww) in enumerate(((16, 64), (24, 96))):
     want.append(orc.dewarp_frame(rg, d, o, poses, stt, tsn, 0.5, 40.0)[0])
 assert np.array_equal(ob.dewarp_frames(frames, 0.5, 40.0), np.concatenate(want))
 print("batched K3 ok")
+vp = np.random.default_rng(12).random((3000, 4)) * 3
+for code, name in ((orv.FIRST_N_POINT, "first_n"), (orv.AVERAGE_POINT, "average"), (orv.RANDOM, "random")):
+    got, gi = ob.voxel_downsample(vp, 0.5, name, max_points_per_voxel=3, min_pts_threshold=2)
+    want, wi = orv.voxel_downsample_xd(vp, 0.5, 3, 2, code, with_indices=True)
+    assert np.array_equal(got, want) and np.array_equal(gi, wi), name
+got, gi = ob.voxel_downsample(vp[:, :3].copy(), 0.5)
+assert np.array_equal(gi, orv.voxel_downsample(vp[:, :3], 0.5)[1])
+vn = vp[:, 1:] - 1.5
+gp, gn, _ = ob.voxel_downsample(vp[:, :3].copy(), 0.5, "point_normal", normals=vn)
+wp, wn = orv.voxel_downsample_with_normals(vp[:, :3], vn, 0.5)
+assert np.array_equal(gp, wp) and np.array_equal(gn, wn)
+print("voxel ok")
 print("SANITIZE CASES OK")
