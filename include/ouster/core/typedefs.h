@@ -124,6 +124,28 @@ struct mat4d {
     bool operator==(const mat4d& o) const { return m == o.m; }
 };
 
+/// Row-major 4x4 pose (stand-in for Eigen::Matrix<double, 4, 4, RowMajor>, typedefs.h Matrix4dR).
+using Matrix4dR = mat4d;
+
+/// 3-vector of doubles (stand-in for Eigen::Vector3d): three contiguous doubles, so a std::vector<Vector3d> is an
+/// n x 3 row-major array.
+struct Vector3d {
+    double v[3] = {0.0, 0.0, 0.0};
+    Vector3d() = default;
+    Vector3d(double x, double y, double z) : v{x, y, z} {}
+    double& operator[](int i) { return v[i]; }
+    const double& operator[](int i) const { return v[i]; }
+    double& operator()(int i) { return v[i]; }
+    const double& operator()(int i) const { return v[i]; }
+    double x() const { return v[0]; }
+    double y() const { return v[1]; }
+    double z() const { return v[2]; }
+    double* data() { return v; }
+    const double* data() const { return v; }
+    bool operator==(const Vector3d& o) const { return v[0] == o.v[0] && v[1] == o.v[1] && v[2] == o.v[2]; }
+};
+static_assert(sizeof(Vector3d) == 3 * sizeof(double), "Vector3d must be three packed doubles");
+
 }  // namespace core
 }  // namespace sdk
 }  // namespace ouster

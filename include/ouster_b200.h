@@ -51,7 +51,8 @@ typedef struct ob_decoder ob_decoder; /* device-resident PacketFormat decode tab
 int ob_abi_version(void);
 /* sizeof() of a public struct by name ("ob_cloud_io", "ob_field_desc", "ob_packet_layout",
  * "ob_decode_io", "ob_decode_batch", "ob_dewarp_frame_io", "ob_normals_io", "ob_encode_io", "ob_dewarp_frames_io",
- * "ob_voxel_io"); 0 for unknown names.  Lets FFI bindings verify their layout. */
+ * "ob_voxel_io", "ob_point_rows", "ob_voxel_map_cull_io", "ob_voxel_query_io", "ob_icp_io", "ob_icp_system_io");
+ * 0 for unknown names.  Lets FFI bindings verify their layout. */
 size_t ob_abi_sizeof(const char* struct_name);
 const char* ob_last_error(void);
 /* number of visible CUDA devices (0 without a driver/GPU); never fails */
@@ -59,7 +60,7 @@ int ob_device_count(void);
 /* kernels launched by this library since load (all threads); the bench's gpu_launches claim */
 uint64_t ob_kernel_launch_count(void);
 /* launches of one named kernel family since load: "decode_pipe" (pipelined K2), "decode" (K2, any
- * kernel), "cloud" (K1), "normals", "voxel"; 0 for unknown names.  Lets tests assert which code path ran. */
+ * kernel), "cloud" (K1), "normals", "voxel", "voxel_map", "icp"; 0 for unknown names.  Lets tests assert which code path ran. */
 uint64_t ob_kernel_launch_count_of(const char* name);
 /* tuning hook (launch geometry and code-path selection only, never results): cloud_tw, cloud_stages,
  * cloud_threads (compute threads; a copy warp is added), cloud_ctas_per_sm, cloud_store_lag,
@@ -275,6 +276,106 @@ typedef struct ob_voxel_io {
     size_t* n_out;               /* rows written; host or device memory */
 } ob_voxel_io;
 ob_status ob_voxel_downsample(const ob_voxel_io* io, ob_stream* s);
+
+/* ---- frame-to-map registration: device-resident VoxelHashMap3d and ICP (DESIGN f-6) ----
+ * Rows of x, y, z: `dtype` (OB_F32 / OB_F64) rows x 3, n rows, or a device-resident row count (n_device, clamped to
+ * `capacity`, e.g. the n_out of ob_voxel_downsample).  Outputs are float64.  Buffers may be host or device memory. */
+typedef struct ob_point_rows {
+    int32_t dtype;
+    const void* points;     /* rows x 3 */
+    size_t n;               /* row count when n_device is NULL */
+    const size_t* n_device; /* optional device-resident row count */
+    size_t capacity;        /* rows the buffer holds; used with n_device */
+} ob_point_rows;
+
+typedef struct ob_voxel_map ob_voxel_map; /* VoxelHashMap3d: open-addressing table in device memory */
+
+/* replaces VoxelHashMap3d(voxel_size, max_distance, max_points_per_voxel, min_pts_threshold)
+ *          ouster_core/src/voxel_hash_map.cpp:14-41 (min_pts_threshold is stored and unused, as there)
+ * errors (OB_INVALID_ARGUMENT, checked in this order): "max_points_per_voxel must be greater than 0",
+ * "voxel_size must be greater than 0", "max_distance must be greater than 0"; then OB_NO_DEVICE without a GPU. */
+ob_status ob_voxel_map_create(double voxel_size, double max_distance, size_t max_points_per_voxel,
+                              size_t min_pts_threshold, int device, ob_voxel_map** out);
+ob_status ob_voxel_map_destroy(ob_voxel_map* m);
+/* replaces VoxelHashMap::clear                      voxel_hash_map.h:387-389 */
+ob_status ob_voxel_map_clear(ob_voxel_map* m, ob_stream* s);
+/* replaces VoxelHashMap::add_points / add_point     voxel_hash_map.cpp:85-107, first_n_point voxel_hash_map.h:287-301
+ * The result equals inserting the rows one at a time.  Asynchronous unless a host-side bound (occupied slots plus
+ * the batch's row capacity, or `capacity` with n_device) passes half the table: then the call synchronises once to
+ * read the counters and the batch's distinct-voxel count, and grows the table to the next power of two >=
+ * 4 x (live + new voxels) slots (DESIGN 4, f-6).  Growth frees the old table, so a CUDA graph that captured
+ * ob_icp_align or ob_voxel_map_closest_neighbors on this map must be captured again.  error (OB_RUNTIME_ERROR):
+ * "voxel map: a table of N slots (B bytes) does not fit in free device memory"; on any error the map is unchanged
+ * and nothing of the batch is inserted. */
+ob_status ob_voxel_map_add_points(ob_voxel_map* m, const ob_point_rows* rows, ob_stream* s);
+
+/* replaces remove_voxels_far_from_location / extract_voxels_far_from_location   voxel_hash_map.cpp:109-154
+ * origin: 3 doubles, host or device (so a device-resident pose can feed it).  Voxels with
+ * |v - v_origin|^2 >= (ceil(max_distance / voxel_size) + 1)^2, in wrapping int32 arithmetic as the reference runs on
+ * x86, are erased.  n_extracted != NULL also emits their points (creation order, then slot order) into `extracted`
+ * (capacity rows x 3 float64; give it at least the map's point count, ob_voxel_map_size): with a host n_extracted the
+ * call synchronises once, with a device one nothing waits.  error: "output capacity too small" (the voxels are
+ * erased regardless). */
+typedef struct ob_voxel_map_cull_io {
+    const double* origin;
+    double* extracted;
+    size_t capacity;
+    size_t* n_extracted;
+} ob_voxel_map_cull_io;
+ob_status ob_voxel_map_remove_far(ob_voxel_map* m, const ob_voxel_map_cull_io* io, ob_stream* s);
+
+/* replaces VoxelHashMap::pointcloud / pointcloud_vector   voxel_hash_map.cpp:43-76
+ * Voxels in creation order (the reference: tsl::robin_map order, DESIGN 9), inside a voxel in slot order.
+ * points: capacity x 3 float64 (NULL: count only); n_out host (one synchronisation) or device (none). */
+ob_status ob_voxel_map_point_cloud(const ob_voxel_map* m, double* points, size_t capacity, size_t* n_out,
+                                   ob_stream* s);
+/* live voxels and stored points (VoxelHashMap::empty is voxels == 0); synchronises the stream */
+ob_status ob_voxel_map_size(const ob_voxel_map* m, size_t* voxels, size_t* points, ob_stream* s);
+
+/* replaces VoxelHashMap::get_closest_neighbor(query, max_distance_sq), one query per row   voxel_hash_map.cpp:194-247
+ * The 27 voxels in VOXEL_SHIFTS order, each pruned by its AABB lower bound, the first strictly smaller squared
+ * distance kept; (0, 0, 0) and max_distance_sq when nothing qualifies.  neighbors: rows x 3 float64;
+ * distances_sq (optional): rows float64. */
+typedef struct ob_voxel_query_io {
+    ob_point_rows queries;
+    double max_distance_sq; /* the reference's default is DBL_MAX */
+    double* neighbors;
+    double* distances_sq;
+} ob_voxel_query_io;
+ob_status ob_voxel_map_closest_neighbors(const ob_voxel_map* m, const ob_voxel_query_io* io, ob_stream* s);
+
+/* replaces ICPRegistration::align_points_to_map(frame, VoxelHashMap3d, max_distance, kernel_scale)
+ *          ouster_mapping/src/icp_registration.cpp (align_points_to_map_impl, data_association, build_linear_system)
+ * Every iteration runs on the stream: association fused with applying the previous increment to the source,
+ * order-preserving compaction, the linear system in parallel_deterministic_reduce's tree, and one kernel for the
+ * LDLT solve, SE3::exp, t_icp = estimation * t_icp and the stop test (|dx|^2 < convergence_criterion^2).
+ * pose: 16 doubles, row-major 4x4 (t_icp.matrix()); iterations (optional): iterations run, 0 for an empty map
+ * (which gives the identity).  Device pose and iterations: nothing waits for the GPU; otherwise one synchronisation. */
+typedef struct ob_icp_io {
+    ob_point_rows source;
+    double max_distance;          /* max correspondence distance */
+    double kernel_scale;          /* Geman-McClure scale */
+    int32_t max_num_iterations;   /* ICPRegistration::max_num_iterations_ (reference default 50) */
+    double convergence_criterion; /* ICPRegistration::convergence_criterion_ (reference default 1e-4) */
+    double* pose;
+    int32_t* iterations;
+} ob_icp_io;
+ob_status ob_icp_align(const ob_voxel_map* m, const ob_icp_io* io, ob_stream* s);
+
+/* replaces build_linear_system(correspondences, kernel_scale)   ouster_mapping/src/icp_registration.cpp
+ * source / target: n x 3 float64 pairs (n or a device count clamped to capacity); jtj: 36 doubles row-major (lower
+ * triangle filled, the rest 0, as the reference leaves it), jtr: 6 doubles.  Same summation tree as the reference. */
+typedef struct ob_icp_system_io {
+    const double* source;
+    const double* target;
+    size_t n;
+    const size_t* n_device;
+    size_t capacity;
+    double kernel_scale;
+    double* jtj;
+    double* jtr;
+} ob_icp_system_io;
+ob_status ob_icp_linear_system(const ob_icp_system_io* io, ob_stream* s);
 
 /* ---- fused range -> (XYZ, destaggered range, destaggered XYZ), batched over frames ----
  * One launch performs, for every frame f and return r of the batch, what the reference does as

@@ -56,6 +56,29 @@ class VoxelIO(C.Structure):
 OB_VOXEL_FIRST_N_POINT, OB_VOXEL_AVERAGE_POINT, OB_VOXEL_RANDOM, OB_VOXEL_SHUFFLE_FIRST, OB_VOXEL_POINT_NORMAL = range(5)
 
 
+class PointRows(C.Structure):
+    _fields_ = [("dtype", C.c_int32), ("points", vp), ("n", sz), ("n_device", vp), ("capacity", sz)]
+
+
+class VoxelMapCullIO(C.Structure):
+    _fields_ = [("origin", vp), ("extracted", vp), ("capacity", sz), ("n_extracted", vp)]
+
+
+class VoxelQueryIO(C.Structure):
+    _fields_ = [("queries", PointRows), ("max_distance_sq", C.c_double), ("neighbors", vp), ("distances_sq", vp)]
+
+
+class IcpIO(C.Structure):
+    _fields_ = [("source", PointRows), ("max_distance", C.c_double), ("kernel_scale", C.c_double),
+                ("max_num_iterations", C.c_int32), ("convergence_criterion", C.c_double), ("pose", vp),
+                ("iterations", vp)]
+
+
+class IcpSystemIO(C.Structure):
+    _fields_ = [("source", vp), ("target", vp), ("n", sz), ("n_device", vp), ("capacity", sz),
+                ("kernel_scale", C.c_double), ("jtj", vp), ("jtr", vp)]
+
+
 class DewarpFramesIO(C.Structure):
     _fields_ = [("lut", vp), ("range", vp), ("poses", vp), ("status", vp), ("timestamps", vp)]
 
@@ -136,6 +159,16 @@ _sig("ob_scan_to_cloud", i32, vp, vp, sz, C.POINTER(CloudIO), vp)
 _sig("ob_dewarp_frame", i32, vp, C.POINTER(DewarpFrameIO), C.POINTER(sz), vp)
 _sig("ob_normals", i32, i32, C.POINTER(NormalsIO), vp)
 _sig("ob_voxel_downsample", i32, C.POINTER(VoxelIO), vp)
+_sig("ob_voxel_map_create", i32, C.c_double, C.c_double, sz, sz, i32, C.POINTER(vp))
+_sig("ob_voxel_map_destroy", i32, vp)
+_sig("ob_voxel_map_clear", i32, vp, vp)
+_sig("ob_voxel_map_add_points", i32, vp, C.POINTER(PointRows), vp)
+_sig("ob_voxel_map_remove_far", i32, vp, C.POINTER(VoxelMapCullIO), vp)
+_sig("ob_voxel_map_point_cloud", i32, vp, vp, sz, vp, vp)
+_sig("ob_voxel_map_size", i32, vp, C.POINTER(sz), C.POINTER(sz), vp)
+_sig("ob_voxel_map_closest_neighbors", i32, vp, C.POINTER(VoxelQueryIO), vp)
+_sig("ob_icp_align", i32, vp, C.POINTER(IcpIO), vp)
+_sig("ob_icp_linear_system", i32, C.POINTER(IcpSystemIO), vp)
 _sig("ob_dewarp_frames", i32, C.POINTER(DewarpFramesIO), sz, C.c_double, C.c_double, vp, sz, vp, vp, vp,
      C.POINTER(sz), C.POINTER(sz), vp)
 if hasattr(lib, "ob_decoder_create"):

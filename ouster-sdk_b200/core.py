@@ -550,6 +550,185 @@ def voxel_downsample(points, voxel_size, mode="shuffle_first", normals=None, max
     return tuple(a[:k] for a in head)
 
 
+DBL_MAX = float(np.finfo(np.float64).max)
+
+
+def _torch_stream(x, stream):
+    import torch
+    return stream or Stream(x.device.index, cuda_stream=torch.cuda.current_stream(x.device).cuda_stream)
+
+
+def _point_rows(points, n=None, what="add_points expects an Nx3 array"):
+    """(PointRows, kept array) for [rows, 3] float32 / float64 points (numpy or torch); n: optional CUDA int64 [1]
+    device-resident row count, then `points` holds `capacity` rows."""
+    from ._capi import PointRows
+    if _is_torch(points):
+        import torch
+        if points.dtype not in (torch.float32, torch.float64):
+            points = points.double()
+        points = points.contiguous()
+    else:
+        points = np.ascontiguousarray(points)
+        if points.dtype not in (np.float32, np.float64):
+            points = points.astype(np.float64)
+    if len(points.shape) != 2 or points.shape[1] != 3:
+        raise ValueError(what)
+    r = PointRows()
+    r.dtype = _capi.OB_F64 if _np_dtype(points) == np.float64 else _capi.OB_F32
+    r.points = _ptr(points)
+    if n is None:
+        r.n = int(points.shape[0])
+    else:
+        import torch
+        if not (_is_torch(n) and n.is_cuda and n.dtype == torch.int64 and n.numel() == 1):
+            raise ValueError("n must be a CUDA int64 tensor with one element")
+        if not (_is_torch(points) and points.is_cuda):
+            raise ValueError("a device-side row count needs device inputs")
+        r.n_device, r.capacity = n.data_ptr(), int(points.shape[0])
+    return r, points
+
+
+class VoxelMap:
+    """Device-resident VoxelHashMap3d (ob_voxel_map, voxel_hash_map.cpp:14-247) with first_n_point insertion.
+    Points may be numpy arrays or torch tensors (CUDA tensors stay on the device); results are float64.
+    point_cloud() and the extracted rows list voxels in creation order (DESIGN 9)."""
+
+    def __init__(self, voxel_size, max_distance=100.0, max_points_per_voxel=20, min_pts_threshold=1, device=0):
+        h = C.c_void_p()
+        check(lib.ob_voxel_map_create(float(voxel_size), float(max_distance), int(max_points_per_voxel),
+                                      int(min_pts_threshold), device, C.byref(h)))
+        self._h, self.device = h, device
+        self.voxel_size, self.max_distance = float(voxel_size), float(max_distance)
+        self.max_points_per_voxel, self.min_pts_threshold = int(max_points_per_voxel), int(min_pts_threshold)
+
+    def __del__(self):
+        if getattr(self, "_h", None) and lib is not None:
+            try:
+                lib.ob_voxel_map_destroy(self._h)
+            except Exception:
+                pass
+            self._h = None
+
+    def _st(self, x, stream):
+        return _torch_stream(x, stream) if _is_torch(x) and x.is_cuda else _stream(stream, self.device)
+
+    def clear(self, stream=None):
+        check(lib.ob_voxel_map_clear(self._h, _stream(stream, self.device).h))
+
+    def size(self, stream=None):
+        """(live voxels, stored points); waits for the stream."""
+        v, p = C.c_size_t(0), C.c_size_t(0)
+        check(lib.ob_voxel_map_size(self._h, C.byref(v), C.byref(p), _stream(stream, self.device).h))
+        return v.value, p.value
+
+    def add_points(self, points, n=None, stream=None):
+        r, keep = _point_rows(points, n)
+        st = self._st(keep, stream)  # held: a wrapped stream is destroyed with its Python object
+        check(lib.ob_voxel_map_add_points(self._h, C.byref(r), st.h))
+
+    def remove_far(self, origin, extract=False, stream=None):
+        """remove_voxels_far_from_location(origin); extract=True returns the erased points (numpy [m, 3])."""
+        from ._capi import VoxelMapCullIO
+        if _is_torch(origin):
+            org = origin.double().contiguous().reshape(3)
+            st = _torch_stream(org, stream) if org.is_cuda else _stream(stream, self.device)
+        else:
+            org = np.ascontiguousarray(origin, np.float64).reshape(3)
+            st = _stream(stream, self.device)
+        io = VoxelMapCullIO()
+        io.origin = _ptr(org)
+        if not extract:
+            check(lib.ob_voxel_map_remove_far(self._h, C.byref(io), st.h))
+            return None
+        cap = self.size(stream=st)[1]
+        out = np.empty((cap, 3), np.float64)
+        cnt = C.c_size_t(0)
+        io.extracted, io.capacity, io.n_extracted = _ptr(out), cap, C.addressof(cnt)
+        check(lib.ob_voxel_map_remove_far(self._h, C.byref(io), st.h))
+        return out[:cnt.value]
+
+    def point_cloud(self, device=False, stream=None):
+        """pointcloud(): [m, 3] float64 numpy array, or a CUDA tensor with device=True."""
+        st = _stream(stream, self.device)
+        cap = self.size(stream=st)[1]
+        cnt = C.c_size_t(0)
+        if device:
+            import torch
+            out = torch.empty((cap, 3), dtype=torch.float64, device=torch.device("cuda", self.device))
+        else:
+            out = np.empty((cap, 3), np.float64)
+        check(lib.ob_voxel_map_point_cloud(self._h, _ptr(out), cap, C.addressof(cnt), st.h))
+        if device:
+            st.sync()
+        return out[:cnt.value]
+
+    def closest_neighbors(self, points, max_distance_sq=DBL_MAX, n=None, stream=None):
+        """get_closest_neighbor for every row: (neighbors [rows, 3], squared distances [rows]) float64, torch on the
+        device for CUDA inputs (asynchronous), numpy otherwise."""
+        from ._capi import VoxelQueryIO
+        r, keep = _point_rows(points, n, "VoxelHashMap method expects a 3-element point")
+        rows = int(keep.shape[0])
+        if _is_torch(keep) and keep.is_cuda:
+            import torch
+            nb = torch.zeros((rows, 3), dtype=torch.float64, device=keep.device)
+            d2 = torch.empty(rows, dtype=torch.float64, device=keep.device)
+        else:
+            nb, d2 = np.zeros((rows, 3), np.float64), np.empty(rows, np.float64)
+        io = VoxelQueryIO()
+        io.queries, io.max_distance_sq, io.neighbors, io.distances_sq = r, float(max_distance_sq), _ptr(nb), _ptr(d2)
+        st = self._st(keep, stream)
+        check(lib.ob_voxel_map_closest_neighbors(self._h, C.byref(io), st.h))
+        if not _is_torch(nb):
+            st.sync()
+        return nb, d2
+
+
+def icp_align(voxel_map, source, max_distance, kernel_scale, max_num_iterations=50, convergence_criterion=1e-4,
+              n=None, stream=None):
+    """ICPRegistration::align_points_to_map on the GPU (ob_icp_align): (pose [4, 4] float64, iterations run).
+    A CUDA-tensor source gives CUDA tensors (pose float64 [4, 4], iterations int32 [1]) and nothing waits for the
+    GPU; n: optional device-resident source row count (e.g. voxel_downsample's count)."""
+    from ._capi import IcpIO
+    r, keep = _point_rows(source, n)
+    io = IcpIO()
+    io.source, io.max_distance, io.kernel_scale = r, float(max_distance), float(kernel_scale)
+    io.max_num_iterations, io.convergence_criterion = int(max_num_iterations), float(convergence_criterion)
+    if _is_torch(keep) and keep.is_cuda:
+        import torch
+        pose = torch.empty((4, 4), dtype=torch.float64, device=keep.device)
+        it = torch.empty(1, dtype=torch.int32, device=keep.device)
+        io.pose, io.iterations = pose.data_ptr(), it.data_ptr()
+        st = _torch_stream(keep, stream)
+        check(lib.ob_icp_align(voxel_map._h, C.byref(io), st.h))
+        return pose, it
+    pose = np.empty((4, 4), np.float64)
+    it = C.c_int32(0)
+    io.pose, io.iterations = pose.ctypes.data, C.addressof(it)
+    check(lib.ob_icp_align(voxel_map._h, C.byref(io), _stream(stream, voxel_map.device).h))
+    return pose, it.value
+
+
+def icp_linear_system(source, target, kernel_scale, stream=None, device=0):
+    """build_linear_system(correspondences, kernel_scale) (icp_registration.cpp) on the GPU with the reference's
+    deterministic-reduce tree: (jtj [6, 6], lower triangle, jtr [6]) float64 numpy arrays."""
+    from ._capi import IcpSystemIO
+    def f64(a):  # the C ABI reads dense float64 rows
+        return a.double().contiguous() if _is_torch(a) else np.ascontiguousarray(a, np.float64)
+
+    s, t = f64(source), f64(target)
+    if tuple(s.shape) != tuple(t.shape) or len(s.shape) != 2 or s.shape[1] != 3:
+        raise ValueError("source and target must both be [n, 3]")
+    if _is_torch(s) != _is_torch(t) or (_is_torch(s) and s.device != t.device):
+        raise ValueError("source and target must live in the same memory")
+    jtj, jtr = np.empty((6, 6), np.float64), np.empty(6, np.float64)
+    io = IcpSystemIO()
+    io.source, io.target, io.n, io.kernel_scale = _ptr(s), _ptr(t), int(s.shape[0]), float(kernel_scale)
+    io.jtj, io.jtr = jtj.ctypes.data, jtr.ctypes.data
+    st = _torch_stream(s, stream) if _is_torch(s) and s.is_cuda else _stream(stream, device)
+    check(lib.ob_icp_linear_system(C.byref(io), st.h))
+    return jtj, jtr
+
+
 def dewarp_frames(frames, min_range=0.0, max_range=float("inf"), provenance=False, stream=None):
     """dewarp(frame_set, xyzluts, min_range, max_range) (pose_util.h:475, impl/dewarp_impl.h:84-117):
     `frames` is a list with one entry per slot of the set -- None for an empty slot, else a dict

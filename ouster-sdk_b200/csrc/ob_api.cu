@@ -16,12 +16,13 @@ namespace ob {
 static thread_local std::string g_last_error;
 static std::atomic<uint64_t> g_launches{0};
 
-static std::atomic<uint64_t> g_family[5];
-static const char* const kFamilies[5] = {"decode_pipe", "decode", "cloud", "normals", "voxel"};
+static std::atomic<uint64_t> g_family[OB_FAM_COUNT];
+static const char* const kFamilies[OB_FAM_COUNT] = {"decode_pipe", "decode", "cloud", "normals", "voxel",
+                                                    "voxel_map", "icp"};
 
 void count_launch(uint64_t n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 void count_launch_of(int family, uint64_t n) {
-    if (family >= 0 && family < 5) g_family[family].fetch_add(n, std::memory_order_relaxed);
+    if (family >= 0 && family < OB_FAM_COUNT) g_family[family].fetch_add(n, std::memory_order_relaxed);
 }
 
 ob_status fail(ob_status st, const std::string& msg) {
@@ -324,6 +325,11 @@ size_t ob_abi_sizeof(const char* name) {
     if (n == "ob_encode_io") return sizeof(ob_encode_io);
     if (n == "ob_dewarp_frames_io") return sizeof(ob_dewarp_frames_io);
     if (n == "ob_voxel_io") return sizeof(ob_voxel_io);
+    if (n == "ob_point_rows") return sizeof(ob_point_rows);
+    if (n == "ob_voxel_map_cull_io") return sizeof(ob_voxel_map_cull_io);
+    if (n == "ob_voxel_query_io") return sizeof(ob_voxel_query_io);
+    if (n == "ob_icp_io") return sizeof(ob_icp_io);
+    if (n == "ob_icp_system_io") return sizeof(ob_icp_system_io);
     return 0;
 }
 
@@ -342,7 +348,7 @@ uint64_t ob_kernel_launch_count(void) { return g_launches.load(std::memory_order
 
 uint64_t ob_kernel_launch_count_of(const char* name) {
     if (!name) return 0;
-    for (int i = 0; i < 5; ++i)
+    for (int i = 0; i < OB_FAM_COUNT; ++i)
         if (std::string(name) == kFamilies[i]) return g_family[i].load(std::memory_order_relaxed);
     return 0;
 }

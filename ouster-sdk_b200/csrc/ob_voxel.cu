@@ -24,13 +24,12 @@
 // one slot per voxel.
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
-#include <cuda/std/tuple>
 
 #include <algorithm>
-#include <climits>
 #include <type_traits>
 
 #include "ob_api_common.h"
+#include "ob_voxel_common.cuh"
 
 namespace ob {
 
@@ -80,36 +79,6 @@ __device__ uint32_t xs_state_after(unsigned long long steps) {
     return v;
 }
 
-// ---- keys ----
-struct VKey {
-    uint32_t pad;  // 1: not a point (slot >= n, or a row POINT_NORMAL skips); sorts after every voxel
-    int32_t x, y, z;
-};
-struct VKeyDecomposer {
-    __host__ __device__ ::cuda::std::tuple<uint32_t&, int32_t&, int32_t&, int32_t&> operator()(VKey& k) const {
-        return {k.pad, k.x, k.y, k.z};
-    }
-};
-constexpr int kKeyBits = 97;  // x, y, z and the low bit of pad
-
-__device__ __forceinline__ bool same_key(const VKey& a, const VKey& b) {
-    return a.pad == b.pad && a.x == b.x && a.y == b.y && a.z == b.z;
-}
-
-// static_cast<int>(std::floor(v)) as x86 cvttsd2si evaluates it: NaN and out-of-range give INT_MIN
-// (the device conversion would saturate instead)
-__device__ __forceinline__ int32_t voxel_coord(double v) {
-    const double f = floor(v);
-    if (!(f >= -2147483648.0 && f < 2147483648.0)) return INT_MIN;
-    return static_cast<int32_t>(f);
-}
-
-__device__ __forceinline__ double mul(double a, double b) { return __dmul_rn(a, b); }
-__device__ __forceinline__ double add(double a, double b) { return __dadd_rn(a, b); }
-__device__ __forceinline__ double sub(double a, double b) { return __dsub_rn(a, b); }
-// squaredNorm of a 3-vector, (x0*x0 + x1*x1) + x2*x2 as in ob_normals.cu (DESIGN 2)
-__device__ __forceinline__ double sqn3(double a, double b, double c) { return add(add(mul(a, a), mul(b, b)), mul(c, c)); }
-
 struct VoxelParams {
     const void* points;   // capacity x cols of T
     const void* normals;  // POINT_NORMAL: capacity x 3 of T
@@ -129,8 +98,6 @@ __device__ __forceinline__ unsigned n_of(const VoxelParams& p) {
     const unsigned long long n = *p.n_dev;
     return n < p.cap ? static_cast<unsigned>(n) : p.cap;
 }
-
-__device__ __forceinline__ unsigned tid_global() { return blockIdx.x * blockDim.x + threadIdx.x; }
 
 template <typename T>
 __device__ __forceinline__ double ld(const void* base, size_t i) {
@@ -219,46 +186,11 @@ __global__ void vx_key_kernel(VoxelParams p, VKey* keys, uint32_t* seq) {
     seq[t] = t;
 }
 
-// ---- 3. segments ----
-__global__ void vx_head_kernel(unsigned cap, const VKey* sk, const uint32_t* sseq, uint32_t* opens) {
-    const unsigned q = tid_global();
-    if (q >= cap) return;
-    const VKey k = sk[q];
-    opens[sseq[q]] = (k.pad == 0u && (q == 0 || !same_key(k, sk[q - 1]))) ? 1u : 0u;
-}
-
-__global__ void vx_seg_kernel(unsigned cap, const VKey* sk, const uint32_t* sseq, const uint32_t* vrank, uint32_t* seg_start) {
-    const unsigned q = tid_global();
-    if (q >= cap) return;
-    const VKey k = sk[q];
-    if (k.pad == 0u && (q == 0 || !same_key(k, sk[q - 1]))) seg_start[vrank[sseq[q]] - 1] = q;
-}
-
+// ---- 3. segments (vx_head_kernel, vx_seg_kernel, segment_end: ob_voxel_common.cuh) ----
 struct Seg {
     unsigned start, len;
 };
-// Equal keys are contiguous after the sort, so "sk[q] == k" is true on [start, end) and false after it: the
-// end is found by galloping then bisecting, O(log len) probes instead of a walk over a dense voxel.
-__device__ __forceinline__ unsigned segment_end(unsigned start, unsigned cap, const VKey* sk) {
-    const VKey k = sk[start];
-    unsigned last = start, step = 1, hi = cap;
-    for (;;) {
-        const unsigned probe = last + step;
-        if (probe >= cap || !same_key(sk[probe], k)) {
-            hi = min(probe, cap);
-            break;
-        }
-        last = probe;
-        step <<= 1;
-    }
-    while (hi - last > 1) {
-        const unsigned mid = last + (hi - last) / 2;
-        if (same_key(sk[mid], k)) last = mid;
-        else hi = mid;
-    }
-    return hi;
-}
-// the same search backwards: the first sorted position of the voxel that holds position q
+// the same search as segment_end, backwards: the first sorted position of the voxel that holds position q
 __device__ __forceinline__ unsigned segment_begin(unsigned q, const VKey* sk) {
     const VKey k = sk[q];
     unsigned first = q, step = 1;
@@ -408,8 +340,8 @@ __global__ void vx_reduce_first_kernel(VoxelParams p, Work w) {
             bool near = false;
             for (unsigned k = 0; k < fill && !near; ++k) {
                 const size_t o = static_cast<size_t>(b[k]) * p.cols;
-                near = sqn3(sub(ld<T>(p.points, o), v[i][0]), sub(ld<T>(p.points, o + 1), v[i][1]),
-                            sub(ld<T>(p.points, o + 2), v[i][2])) < p.res_sq;
+                near = within_resolution(ld<T>(p.points, o), ld<T>(p.points, o + 1), ld<T>(p.points, o + 2), v[i][0],
+                                         v[i][1], v[i][2], p.res_sq);
             }
             if (!near) b[fill++] = rows[i];
         }
@@ -487,8 +419,6 @@ __global__ void vx_emit_kernel(VoxelParams p, Work w, const uint32_t* coff, doub
         if (out_idx) out_idx[base + k] = static_cast<uint32_t>(row);
     }
 }
-
-inline unsigned blocks_for(unsigned n) { return (n + 255u) / 256u; }
 
 }  // namespace
 

@@ -1,0 +1,1277 @@
+// ob_voxel_map.cu -- frame-to-map registration (DESIGN f-6): a device-resident VoxelHashMap3d and
+// ICPRegistration::align_points_to_map / build_linear_system.
+//
+// What it replaces (reference paths relative to the reference tree, ouster-sdk 1.0.1):
+//   VoxelHashMap3d (first_n_point, DefaultVoxelBucket)  ouster_core/include/ouster/core/voxel_hash_map.h:287-301, 352-510
+//                                                        ouster_core/src/voxel_hash_map.cpp:14-247
+//   ICPRegistration, build_linear_system               ouster_mapping/src/icp_registration.cpp
+//   Sophus SO3::expAndTheta / leftJacobian, SE3::exp, composition, matrix()
+//                                                        thirdparty/sophus/sophus/{so3,se3}.hpp
+//   Eigen LDLT (diagonal pivoting) and its solve        jtj.ldlt().solve(-jtr)
+//
+// The map is an open-addressing hash table in HBM (linear probing, power-of-two capacity).  A slot holds an int32
+// voxel key, a state (empty / live / tombstone / being claimed), a 64-bit creation stamp, a fill count and
+// max_points_per_voxel double3 points.  Erased voxels become tombstones: queries and inserts probe past them, and
+// they are dropped when the table is rebuilt (DESIGN 9).
+//
+// add_points keys and stable-sorts the batch by voxel (the downsampling pipeline's keys, sort and first-appearance
+// numbering, ob_voxel_common.cuh), then one thread per distinct voxel finds or claims its slot and runs the
+// first_n_point gate over the voxel's rows in input order, seeded with the points the bucket already holds -- the
+// result of inserting the rows one at a time.  A new voxel's stamp is the map's stamp counter plus its
+// first-appearance rank in the batch, so voxels are emitted in creation order.
+//
+// The host keeps an upper bound of the occupied slots (live + tombstones).  Only when that bound plus the batch's
+// row capacity could exceed half the table does it read the device counters and the batch's distinct-voxel count
+// (one stream synchronisation) and, if needed, rebuild the table for 4 x (live + new voxels) slots, dropping the
+// tombstones.  The rebuilt table replaces the old one only after every step succeeded (see reserve()).
+//
+// align_points_to_map runs its iterations as four kernels each, all on the stream; the convergence flag lives on the
+// device and later iterations return at once.
+#include <cub/block/block_reduce.cuh>
+#include <cub/block/block_scan.cuh>
+#include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
+
+#include <algorithm>
+#include <cfloat>
+#include <cmath>
+#include <type_traits>
+
+#include "ob_api_common.h"
+#include "ob_voxel_common.cuh"
+
+struct ob_voxel_map {
+    int device;
+    double voxel_size, max_distance, inv, res_sq;
+    size_t max_pts, min_pts;
+    unsigned cap;                // slots (power of two), 0 before the first insertion
+    int32_t* key;                // cap x 3
+    uint32_t* state;             // cap
+    unsigned long long* stamp;   // cap
+    uint32_t* cnt;               // cap
+    double* pts;                 // cap x max_pts x 3
+    unsigned long long* ctr;     // device counters, see Ctr
+    size_t occupied_bound;       // host upper bound of live + tombstone slots
+};
+
+namespace ob {
+namespace {
+
+enum : uint32_t { kEmpty = 0, kLive = 1, kTomb = 2, kClaimed = 3 };
+// device counters (ob_voxel_map::ctr)
+enum { C_STAMP = 0, C_LIVE = 1, C_POINTS = 2, C_OCCUPIED = 3, C_FULL = 4, C_WORDS = 5 };
+
+struct Table {
+    unsigned cap;
+    int32_t* key;
+    uint32_t* state;
+    unsigned long long* stamp;
+    uint32_t* cnt;
+    double* pts;
+    unsigned max_pts;
+};
+
+Table table_of(const ob_voxel_map* m) {
+    return Table{m->cap, m->key, m->state, m->stamp, m->cnt, m->pts, static_cast<unsigned>(m->max_pts)};
+}
+
+__device__ __forceinline__ unsigned slot_hash(int32_t x, int32_t y, int32_t z, unsigned mask) {
+    unsigned long long h = static_cast<unsigned long long>(static_cast<uint32_t>(x)) * 0x9E3779B97F4A7C15ull;
+    h ^= static_cast<unsigned long long>(static_cast<uint32_t>(y)) * 0xC2B2AE3D27D4EB4Full;
+    h ^= static_cast<unsigned long long>(static_cast<uint32_t>(z)) * 0x165667B19E3779F9ull;
+    h ^= h >> 32;
+    h *= 0xD6E8FEB86659FD93ull;
+    h ^= h >> 32;
+    return static_cast<unsigned>(h) & mask;
+}
+
+__device__ __forceinline__ uint32_t load_state(const uint32_t* s) { return *reinterpret_cast<const volatile uint32_t*>(s); }
+
+// slot of a live voxel, or -1
+__device__ __forceinline__ int find_slot(const Table& t, int32_t x, int32_t y, int32_t z) {
+    if (t.cap == 0) return -1;
+    const unsigned mask = t.cap - 1;
+    unsigned i = slot_hash(x, y, z, mask);
+    for (unsigned probes = 0; probes < t.cap; ++probes, i = (i + 1) & mask) {
+        const uint32_t s = load_state(t.state + i);
+        if (s == kEmpty) return -1;
+        if (s == kLive && t.key[3 * i] == x && t.key[3 * i + 1] == y && t.key[3 * i + 2] == z) return static_cast<int>(i);
+    }
+    return -1;
+}
+
+// Find the voxel or claim the first empty slot of its probe chain.  Keys are unique inside a batch, so a slot
+// another thread claims concurrently never holds this key, and the chain before the first empty slot (all from
+// earlier batches) is stable.  Returns the slot; *fresh = 1 for a claimed one (still kClaimed).
+__device__ int find_or_claim(const Table& t, int32_t x, int32_t y, int32_t z, unsigned long long* ctr, int* fresh) {
+    const unsigned mask = t.cap - 1;
+    unsigned i = slot_hash(x, y, z, mask);
+    for (unsigned probes = 0; probes < t.cap; ++probes, i = (i + 1) & mask) {
+        uint32_t s = load_state(t.state + i);
+        if (s == kEmpty) {
+            s = atomicCAS(t.state + i, kEmpty, kClaimed);
+            if (s == kEmpty) {
+                *fresh = 1;
+                return static_cast<int>(i);
+            }
+        }
+        if (s == kLive) {
+            __threadfence();
+            if (t.key[3 * i] == x && t.key[3 * i + 1] == y && t.key[3 * i + 2] == z) {
+                *fresh = 0;
+                return static_cast<int>(i);
+            }
+        }
+    }
+    atomicAdd(ctr + C_FULL, 1ull);  // cannot happen while the host keeps the load at or below one half
+    return -1;
+}
+
+// rows of an input: n on the host, or a device word clamped to the capacity
+struct Rows {
+    const void* p;
+    const unsigned long long* n_dev;
+    unsigned long long n_host;
+    unsigned cap;
+};
+__device__ __forceinline__ unsigned rows_n(const Rows& r) {
+    if (r.n_dev == nullptr) return static_cast<unsigned>(r.n_host);
+    const unsigned long long n = *r.n_dev;
+    return n < r.cap ? static_cast<unsigned>(n) : r.cap;
+}
+template <typename T>
+__device__ __forceinline__ void load3(const void* base, size_t row, double* v) {
+    const T* p = static_cast<const T*>(base) + row * 3;
+    v[0] = static_cast<double>(p[0]);
+    v[1] = static_cast<double>(p[1]);
+    v[2] = static_cast<double>(p[2]);
+}
+
+// ---- add_points ----
+template <typename T>
+__global__ void vm_key_kernel(Rows r, double inv, VKey* keys, uint32_t* seq) {
+    const unsigned t = tid_global();
+    if (t >= r.cap) return;
+    VKey k{1u, 0, 0, 0};
+    if (t < rows_n(r)) {
+        double v[3];
+        load3<T>(r.p, t, v);
+        k = VKey{0u, voxel_coord(mul(v[0], inv)), voxel_coord(mul(v[1], inv)), voxel_coord(mul(v[2], inv))};
+    }
+    keys[t] = k;
+    seq[t] = t;
+}
+
+// one thread per distinct voxel of the batch (first-appearance rank r)
+template <typename T>
+__global__ void vm_insert_kernel(Rows r, Table t, unsigned long long* ctr, const VKey* sk, const uint32_t* sseq,
+                                 const uint32_t* vrank, const uint32_t* seg_start, double res_sq) {
+    const unsigned rank = tid_global();
+    if (rank >= r.cap || rank >= vrank[r.cap - 1]) return;
+    const unsigned start = seg_start[rank];
+    const unsigned end = segment_end(start, r.cap, sk);
+    const VKey k = sk[start];
+    int fresh = 0;
+    const int slot = find_or_claim(t, k.x, k.y, k.z, ctr, &fresh);
+    if (slot < 0) return;
+    if (fresh) {
+        t.key[3 * slot] = k.x;
+        t.key[3 * slot + 1] = k.y;
+        t.key[3 * slot + 2] = k.z;
+        t.stamp[slot] = ctr[C_STAMP] + rank;
+        t.cnt[slot] = 0;
+        __threadfence();
+        atomicExch(t.state + slot, kLive);
+        atomicAdd(ctr + C_LIVE, 1ull);
+        atomicAdd(ctr + C_OCCUPIED, 1ull);
+    }
+    double* b = t.pts + static_cast<size_t>(slot) * t.max_pts * 3;
+    const unsigned before = t.cnt[slot];
+    unsigned fill = before;
+    for (unsigned q = start; q < end && fill < t.max_pts; ++q) {  // first_n_point, voxel_hash_map.h:287-301
+        double v[3];
+        load3<T>(r.p, sseq[q], v);
+        bool near = false;
+        for (unsigned j = 0; j < fill && !near; ++j)
+            near = within_resolution(b[3 * j], b[3 * j + 1], b[3 * j + 2], v[0], v[1], v[2], res_sq);
+        if (!near) {
+            b[3 * fill] = v[0];
+            b[3 * fill + 1] = v[1];
+            b[3 * fill + 2] = v[2];
+            ++fill;
+        }
+    }
+    t.cnt[slot] = fill;
+    if (fill != before) atomicAdd(ctr + C_POINTS, static_cast<unsigned long long>(fill - before));
+}
+
+__global__ void vm_advance_stamp_kernel(unsigned cap, const uint32_t* vrank, unsigned long long* ctr) {
+    ctr[C_STAMP] += vrank[cap - 1];
+}
+
+// move the live voxels of `o` into the empty table `t`
+__global__ void vm_rehash_kernel(Table o, Table t) {
+    const unsigned i = tid_global();
+    if (i >= o.cap || o.state[i] != kLive) return;
+    const int32_t x = o.key[3 * i], y = o.key[3 * i + 1], z = o.key[3 * i + 2];
+    const unsigned mask = t.cap - 1;
+    unsigned j = slot_hash(x, y, z, mask);
+    while (atomicCAS(t.state + j, kEmpty, kClaimed) != kEmpty) j = (j + 1) & mask;
+    t.key[3 * j] = x;
+    t.key[3 * j + 1] = y;
+    t.key[3 * j + 2] = z;
+    t.stamp[j] = o.stamp[i];
+    t.cnt[j] = o.cnt[i];
+    const size_t w = static_cast<size_t>(o.max_pts) * 3;
+    for (size_t c = 0; c < static_cast<size_t>(o.cnt[i]) * 3; ++c) t.pts[j * w + c] = o.pts[i * w + c];
+    t.state[j] = kLive;
+}
+
+// ---- remove_voxels_far_from_location (voxel_hash_map.cpp:109-125) ----
+// (voxel - origin_voxel).squaredNorm() >= max_voxel_dist_sq in int32 arithmetic, wrapping as x86 does
+__global__ void vm_cull_kernel(Table t, unsigned long long* ctr, const double* origin, double inv, int32_t thr,
+                               uint32_t* removed) {
+    const unsigned i = tid_global();
+    if (i >= t.cap) return;
+    uint32_t out = 0;
+    if (t.state[i] == kLive) {
+        const uint32_t ox = static_cast<uint32_t>(voxel_coord(mul(origin[0], inv)));
+        const uint32_t oy = static_cast<uint32_t>(voxel_coord(mul(origin[1], inv)));
+        const uint32_t oz = static_cast<uint32_t>(voxel_coord(mul(origin[2], inv)));
+        const uint32_t dx = static_cast<uint32_t>(t.key[3 * i]) - ox, dy = static_cast<uint32_t>(t.key[3 * i + 1]) - oy,
+                       dz = static_cast<uint32_t>(t.key[3 * i + 2]) - oz;
+        const int32_t d2 = static_cast<int32_t>((dx * dx + dy * dy) + dz * dz);
+        if (d2 >= thr) {
+            t.state[i] = kTomb;
+            atomicAdd(ctr + C_LIVE, ~0ull);
+            atomicAdd(ctr + C_POINTS, 0ull - t.cnt[i]);
+            out = 1;
+        }
+    }
+    if (removed) removed[i] = out;
+}
+
+// ---- emission in creation order: pointcloud() and the extracted rows ----
+__global__ void vm_emit_keys_kernel(Table t, const uint32_t* sel, unsigned long long* keys, uint32_t* slots) {
+    const unsigned i = tid_global();
+    if (i >= t.cap) return;
+    const bool on = sel ? sel[i] != 0 : t.state[i] == kLive;
+    keys[i] = on ? t.stamp[i] : ~0ull;
+    slots[i] = i;
+}
+__global__ void vm_emit_counts_kernel(Table t, const unsigned long long* skeys, const uint32_t* sslots, uint32_t* c) {
+    const unsigned p = tid_global();
+    if (p >= t.cap) return;
+    c[p] = skeys[p] != ~0ull ? t.cnt[sslots[p]] : 0u;
+}
+__global__ void vm_emit_kernel(Table t, const unsigned long long* skeys, const uint32_t* sslots, const uint32_t* off,
+                               double* out, unsigned long long capacity, unsigned long long* n_out) {
+    const unsigned p = tid_global();
+    if (p >= t.cap) return;
+    if (p == t.cap - 1) *n_out = off[p];
+    if (skeys[p] == ~0ull) return;
+    const unsigned s = sslots[p];
+    const unsigned c = t.cnt[s];
+    const unsigned long long base = off[p] - c;
+    const double* b = t.pts + static_cast<size_t>(s) * t.max_pts * 3;
+    for (unsigned k = 0; k < c && base + k < capacity; ++k)
+        for (int d = 0; d < 3; ++d) out[(base + k) * 3 + d] = b[3 * k + d];
+}
+
+// ---- get_closest_neighbor (voxel_hash_map.cpp:194-247) ----
+__constant__ int8_t kShift[27][3] = {
+    {0, 0, 0},   {1, 0, 0},   {-1, 0, 0},  {0, 1, 0},   {0, -1, 0},   {0, 0, 1},  {0, 0, -1},  {1, 1, 0},   {1, -1, 0},
+    {-1, 1, 0},  {-1, -1, 0}, {1, 0, 1},   {1, 0, -1},  {-1, 0, 1},   {-1, 0, -1}, {0, 1, 1},  {0, 1, -1},  {0, -1, 1},
+    {0, -1, -1}, {1, 1, 1},   {1, 1, -1},  {1, -1, 1},  {1, -1, -1},  {-1, 1, 1}, {-1, 1, -1}, {-1, -1, 1}, {-1, -1, -1},
+};
+
+// nearest point to q with squared distance < max_d2, visiting the 27 voxels in VOXEL_SHIFTS order and pruning each by
+// its AABB lower bound; (0,0,0) and max_d2 when nothing qualifies
+__device__ double closest(const Table& t, double inv, double vs, const double* q, double max_d2, double* nb) {
+    const int32_t v[3] = {voxel_coord(mul(q[0], inv)), voxel_coord(mul(q[1], inv)), voxel_coord(mul(q[2], inv))};
+    double best = max_d2;
+    nb[0] = nb[1] = nb[2] = 0.0;
+    for (int s = 0; s < 27; ++s) {
+        int32_t w[3];
+        double lb = 0.0;
+        for (int d = 0; d < 3; ++d) {
+            w[d] = static_cast<int32_t>(static_cast<uint32_t>(v[d]) + static_cast<uint32_t>(kShift[s][d]));
+            const double lo = mul(static_cast<double>(w[d]), vs);
+            const double hi = add(lo, vs);
+            if (q[d] < lo) {
+                const double delta = sub(lo, q[d]);
+                lb = add(lb, mul(delta, delta));
+            } else if (q[d] > hi) {
+                const double delta = sub(q[d], hi);
+                lb = add(lb, mul(delta, delta));
+            }
+        }
+        if (lb >= best) continue;
+        const int slot = find_slot(t, w[0], w[1], w[2]);
+        if (slot < 0) continue;
+        const double* b = t.pts + static_cast<size_t>(slot) * t.max_pts * 3;
+        const unsigned c = t.cnt[slot];
+        for (unsigned k = 0; k < c; ++k) {
+            const double d2 = sqn3(sub(b[3 * k], q[0]), sub(b[3 * k + 1], q[1]), sub(b[3 * k + 2], q[2]));
+            if (d2 < best) {
+                best = d2;
+                nb[0] = b[3 * k];
+                nb[1] = b[3 * k + 1];
+                nb[2] = b[3 * k + 2];
+            }
+        }
+    }
+    return best;
+}
+
+template <typename T>
+__global__ void vm_closest_kernel(Rows r, Table t, double inv, double vs, double max_d2, double* nb, double* d2) {
+    const unsigned i = tid_global();
+    if (i >= r.cap || i >= rows_n(r)) return;
+    double q[3], p[3];
+    load3<T>(r.p, i, q);
+    const double best = closest(t, inv, vs, q, max_d2, p);
+    nb[3 * i] = p[0];
+    nb[3 * i + 1] = p[1];
+    nb[3 * i + 2] = p[2];
+    if (d2) d2[i] = best;
+}
+
+// ---- build_linear_system in parallel_deterministic_reduce's tree (icp_registration.cpp) ----
+// blocked_range(begin, end, 128) splits at mid = b + (e - b) / 2 while it holds more than 128 pairs; a leaf sums
+// its pairs sequentially from zero; a parent is left + right.  Only the 15 entries of the lower triangle of JtJ
+// that a pair touches and the 6 of Jtr are stored: every other entry is +0.0 + +0.0 at every node.
+constexpr unsigned kGrain = 128;
+constexpr int kSys = 21;
+// JtJ (row, col) of the stored entries 0..14; Jtr is 15..20
+__constant__ uint8_t kJtjRC[15][2] = {{0, 0}, {1, 1}, {2, 2}, {3, 1}, {3, 2}, {4, 0}, {4, 2}, {5, 0},
+                                      {5, 1}, {3, 3}, {4, 3}, {4, 4}, {5, 3}, {5, 4}, {5, 5}};
+
+__host__ __device__ inline unsigned tree_depth(unsigned long long n) {
+    unsigned d = 0;
+    while (n > kGrain) {
+        n = (n + 1) / 2;
+        ++d;
+    }
+    return d;
+}
+// range of node (k, i) (i's k bits, most significant first, choose the child); false when an ancestor is a leaf
+__device__ inline bool tree_node(unsigned long long n, unsigned k, unsigned i, unsigned long long* b, unsigned long long* e) {
+    unsigned long long lo = 0, hi = n;
+    for (unsigned l = 0; l < k; ++l) {
+        if (hi - lo <= kGrain) return false;
+        const unsigned long long mid = lo + (hi - lo) / 2;
+        if ((i >> (k - 1 - l)) & 1u) lo = mid;
+        else hi = mid;
+    }
+    *b = lo;
+    *e = hi;
+    return true;
+}
+
+// the leaf body: pairs [b, e) summed from zero in order
+__device__ void leaf_sum(const double* src, const double* tgt, unsigned long long b, unsigned long long e, double ks,
+                         double* acc) {
+    for (int j = 0; j < kSys; ++j) acc[j] = 0.0;
+    const double k2 = mul(ks, ks);
+    for (unsigned long long i = b; i < e; ++i) {
+        const double sx = src[3 * i], sy = src[3 * i + 1], sz = src[3 * i + 2];
+        const double rx = sub(sx, tgt[3 * i]), ry = sub(sy, tgt[3 * i + 1]), rz = sub(sz, tgt[3 * i + 2]);
+        const double kr = add(ks, sqn3(rx, ry, rz));
+        const double w = k2 / mul(kr, kr);
+        const double wsx = mul(w, sx), wsy = mul(w, sy), wsz = mul(w, sz);
+        acc[0] = add(acc[0], w);
+        acc[1] = add(acc[1], w);
+        acc[2] = add(acc[2], w);
+        acc[3] = sub(acc[3], wsz);
+        acc[4] = add(acc[4], wsy);
+        acc[5] = add(acc[5], wsz);
+        acc[6] = sub(acc[6], wsx);
+        acc[7] = sub(acc[7], wsy);
+        acc[8] = add(acc[8], wsx);
+        const double wsx2 = mul(wsx, sx), wsy2 = mul(wsy, sy), wsz2 = mul(wsz, sz);
+        acc[9] = add(acc[9], add(wsy2, wsz2));
+        acc[10] = sub(acc[10], mul(wsx, sy));
+        acc[11] = add(acc[11], add(wsx2, wsz2));
+        acc[12] = sub(acc[12], mul(wsx, sz));
+        acc[13] = sub(acc[13], mul(wsy, sz));
+        acc[14] = add(acc[14], add(wsx2, wsy2));
+        acc[15] = add(acc[15], mul(w, rx));
+        acc[16] = add(acc[16], mul(w, ry));
+        acc[17] = add(acc[17], mul(w, rz));
+        const double cx = sub(mul(sy, rz), mul(sz, ry)), cy = sub(mul(sz, rx), mul(sx, rz)), cz = sub(mul(sx, ry), mul(sy, rx));
+        acc[18] = add(acc[18], mul(w, cx));
+        acc[19] = add(acc[19], mul(w, cy));
+        acc[20] = add(acc[20], mul(w, cz));
+    }
+}
+
+// one thread per slot of the deepest level; the thread whose path ends at a leaf with all remaining bits zero owns it
+__global__ void icp_leaf_kernel(const double* src, const double* tgt, const unsigned long long* n_pairs,
+                                unsigned long long max_n, double ks, const int* done, unsigned slots, double* val) {
+    if (done && *done) return;
+    const unsigned t = tid_global();
+    const unsigned long long n = n_pairs ? min(*n_pairs, max_n) : max_n;
+    const unsigned D = tree_depth(n);
+    if (t >= slots || t >= (1u << D)) return;
+    unsigned long long lo = 0, hi = n;
+    unsigned l = 0;
+    for (; l < D && hi - lo > kGrain; ++l) {
+        const unsigned long long mid = lo + (hi - lo) / 2;
+        if ((t >> (D - 1 - l)) & 1u) lo = mid;
+        else hi = mid;
+    }
+    if (t & ((1u << (D - l)) - 1u)) return;
+    double acc[kSys];
+    leaf_sum(src, tgt, lo, hi, ks, acc);
+    for (int j = 0; j < kSys; ++j) val[static_cast<size_t>(t) * kSys + j] = acc[j];
+}
+
+// parents bottom-up (one block): node (k, i) lives in slot i << (D - k), its right child in (2i + 1) << (D - k - 1)
+__device__ void tree_reduce(unsigned long long n, double* val) {
+    const unsigned D = tree_depth(n);
+    for (int k = static_cast<int>(D) - 1; k >= 0; --k) {
+        for (unsigned i = threadIdx.x; i < (1u << k); i += blockDim.x) {
+            unsigned long long b, e;
+            if (!tree_node(n, static_cast<unsigned>(k), i, &b, &e) || e - b <= kGrain) continue;
+            double* l = val + (static_cast<size_t>(i) << (D - k)) * kSys;
+            const double* r = val + (static_cast<size_t>(2 * i + 1) << (D - k - 1)) * kSys;
+            for (int j = 0; j < kSys; ++j) l[j] = add(l[j], r[j]);
+        }
+        __syncthreads();
+    }
+}
+
+// unpack the root: JtJ (6x6 row-major, lower triangle; the rest +0.0) and Jtr
+__device__ void unpack_system(const double* v, double* jtj, double* jtr) {
+    for (int j = 0; j < 36; ++j) jtj[j] = 0.0;
+    for (int j = 0; j < 15; ++j) jtj[kJtjRC[j][0] * 6 + kJtjRC[j][1]] = v[j];
+    for (int j = 0; j < 6; ++j) jtr[j] = v[15 + j];
+}
+
+// ---- Eigen LDLT (ldlt_inplace<Lower>::unblocked) and LDLT::_solve_impl, inner products in index order ----
+__device__ void ldlt_solve6(const double* A, const double* rhs, double* x) {
+    double m[6][6];
+    int tr[6];
+    for (int i = 0; i < 6; ++i)
+        for (int j = 0; j < 6; ++j) m[i][j] = j <= i ? A[i * 6 + j] : 0.0;
+    bool zero_diag = false;
+    for (int k = 0; k < 6 && !zero_diag; ++k) {
+        int big = k;
+        double bv = fabs(m[k][k]);
+        for (int i = k + 1; i < 6; ++i)
+            if (fabs(m[i][i]) > bv) {
+                bv = fabs(m[i][i]);
+                big = i;
+            }
+        tr[k] = big;
+        if (k != big) {
+            for (int j = 0; j < k; ++j) {
+                const double s = m[k][j];
+                m[k][j] = m[big][j];
+                m[big][j] = s;
+            }
+            for (int i = big + 1; i < 6; ++i) {
+                const double s = m[i][k];
+                m[i][k] = m[i][big];
+                m[i][big] = s;
+            }
+            const double s = m[k][k];
+            m[k][k] = m[big][big];
+            m[big][big] = s;
+            for (int i = k + 1; i < big; ++i) {
+                const double u = m[i][k];
+                m[i][k] = m[big][i];
+                m[big][i] = u;
+            }
+        }
+        if (k > 0) {
+            double temp[6];
+            for (int j = 0; j < k; ++j) temp[j] = mul(m[j][j], m[k][j]);
+            double dot = mul(m[k][0], temp[0]);
+            for (int j = 1; j < k; ++j) dot = add(dot, mul(m[k][j], temp[j]));
+            m[k][k] = sub(m[k][k], dot);
+            for (int i = k + 1; i < 6; ++i) {
+                double s = mul(m[i][0], temp[0]);
+                for (int j = 1; j < k; ++j) s = add(s, mul(m[i][j], temp[j]));
+                m[i][k] = sub(m[i][k], s);
+            }
+        }
+        const double akk = m[k][k];
+        const bool valid = fabs(akk) > 0.0;
+        if (k == 0 && !valid) {  // the whole diagonal is zero
+            for (int j = 0; j < 6; ++j) {
+                tr[j] = j;
+                for (int i = j + 1; i < 6; ++i) m[i][j] = 0.0;
+            }
+            zero_diag = true;
+            break;
+        }
+        if (valid)
+            for (int i = k + 1; i < 6; ++i) m[i][k] = m[i][k] / akk;
+    }
+    for (int i = 0; i < 6; ++i) x[i] = rhs[i];
+    for (int k = 0; k < 6; ++k) {
+        const double s = x[k];
+        x[k] = x[tr[k]];
+        x[tr[k]] = s;
+    }
+    for (int j = 0; j < 6; ++j)
+        for (int i = j + 1; i < 6; ++i) x[i] = sub(x[i], mul(x[j], m[i][j]));
+    for (int i = 0; i < 6; ++i) x[i] = fabs(m[i][i]) > DBL_MIN ? x[i] / m[i][i] : 0.0;
+    for (int i = 4; i >= 0; --i) {
+        double s = mul(m[i + 1][i], x[i + 1]);
+        for (int j = i + 2; j < 6; ++j) s = add(s, mul(m[j][i], x[j]));
+        x[i] = sub(x[i], s);
+    }
+    for (int k = 5; k >= 0; --k) {
+        const double s = x[k];
+        x[k] = x[tr[k]];
+        x[tr[k]] = s;
+    }
+}
+
+// ---- Sophus (quaternion x, y, z, w; translation) ----
+struct SE3 {
+    double q[4];  // x, y, z, w
+    double t[3];
+};
+
+__device__ void cross3(const double* a, const double* b, double* c) {
+    c[0] = sub(mul(a[1], b[2]), mul(a[2], b[1]));
+    c[1] = sub(mul(a[2], b[0]), mul(a[0], b[2]));
+    c[2] = sub(mul(a[0], b[1]), mul(a[1], b[0]));
+}
+// SO3 * p (so3.hpp:388-397): uv = q.vec() x p; uv += uv; p + w * uv + q.vec() x uv
+__device__ void rotate(const double* q, const double* p, double* out) {
+    double uv[3], c[3];
+    cross3(q, p, uv);
+    for (int d = 0; d < 3; ++d) uv[d] = add(uv[d], uv[d]);
+    cross3(q, uv, c);
+    for (int d = 0; d < 3; ++d) out[d] = add(add(p[d], mul(q[3], uv[d])), c[d]);
+}
+// SE3 * p (se3.hpp:319-322)
+__device__ void se3_apply(const SE3& g, const double* p, double* out) {
+    double r[3];
+    rotate(g.q, p, r);
+    for (int d = 0; d < 3; ++d) out[d] = add(r[d], g.t[d]);
+}
+// a * b (se3.hpp:302-306, so3.hpp:344-369 with SO3's normalising constructor, so3.hpp:527-534)
+__device__ SE3 se3_mul(const SE3& a, const SE3& b) {
+    SE3 c;
+    const double ax = a.q[0], ay = a.q[1], az = a.q[2], aw = a.q[3];
+    const double bx = b.q[0], by = b.q[1], bz = b.q[2], bw = b.q[3];
+    c.q[3] = sub(sub(sub(mul(aw, bw), mul(ax, bx)), mul(ay, by)), mul(az, bz));
+    c.q[0] = sub(add(add(mul(aw, bx), mul(ax, bw)), mul(ay, bz)), mul(az, by));
+    c.q[1] = sub(add(add(mul(aw, by), mul(ay, bw)), mul(az, bx)), mul(ax, bz));
+    c.q[2] = sub(add(add(mul(aw, bz), mul(az, bw)), mul(ax, by)), mul(ay, bx));
+    // coeffs() (x, y, z, w).norm() as Eigen's two-lane reduction sums it
+    const double len = sqrt(add(add(mul(c.q[0], c.q[0]), mul(c.q[2], c.q[2])), add(mul(c.q[1], c.q[1]), mul(c.q[3], c.q[3]))));
+    for (int j = 0; j < 4; ++j) c.q[j] = c.q[j] / len;
+    double r[3];
+    rotate(a.q, b.t, r);
+    for (int d = 0; d < 3; ++d) c.t[d] = add(a.t[d], r[d]);
+    return c;
+}
+// SE3::exp (se3.hpp:852-861): SO3::expAndTheta (so3.hpp:694-731), SO3::leftJacobian(omega, theta) (so3.hpp:550-571)
+__device__ SE3 se3_exp(const double* a) {
+    const double eps = DBL_EPSILON;
+    const double* om = a + 3;
+    const double theta_sq = sqn3(om[0], om[1], om[2]);
+    double theta, imag, real;
+    if (theta_sq < mul(eps, eps)) {
+        theta = 0.0;
+        const double po4 = mul(theta_sq, theta_sq);
+        imag = add(sub(0.5, mul(1.0 / 48.0, theta_sq)), mul(1.0 / 3840.0, po4));
+        real = add(sub(1.0, mul(1.0 / 8.0, theta_sq)), mul(1.0 / 384.0, po4));
+    } else {
+        theta = sqrt(theta_sq);
+        const double half = mul(0.5, theta);
+        imag = sin(half) / theta;
+        real = cos(half);
+    }
+    SE3 g;
+    g.q[0] = mul(imag, om[0]);
+    g.q[1] = mul(imag, om[1]);
+    g.q[2] = mul(imag, om[2]);
+    g.q[3] = real;
+    const double O[3][3] = {{0.0, -om[2], om[1]}, {om[2], 0.0, -om[0]}, {-om[1], om[0], 0.0}};
+    double V[3][3];
+    const double tsq = mul(theta, theta);
+    if (tsq < mul(eps, eps)) {
+        for (int i = 0; i < 3; ++i)
+            for (int j = 0; j < 3; ++j) V[i][j] = add(i == j ? 1.0 : 0.0, mul(0.5, O[i][j]));
+    } else {
+        const double c1 = sub(1.0, cos(theta)) / tsq;
+        const double c2 = sub(theta, sin(theta)) / mul(tsq, theta);
+        for (int i = 0; i < 3; ++i)
+            for (int j = 0; j < 3; ++j) {
+                const double o2 = add(add(mul(O[i][0], O[0][j]), mul(O[i][1], O[1][j])), mul(O[i][2], O[2][j]));
+                V[i][j] = add(add(i == j ? 1.0 : 0.0, mul(c1, O[i][j])), mul(c2, o2));
+            }
+    }
+    for (int i = 0; i < 3; ++i) g.t[i] = add(add(mul(V[i][0], a[0]), mul(V[i][1], a[1])), mul(V[i][2], a[2]));
+    return g;
+}
+// SE3::matrix() (se3.hpp:273-289; Eigen Quaternion::toRotationMatrix), row-major 4x4
+__device__ void se3_matrix(const SE3& g, double* M) {
+    const double x = g.q[0], y = g.q[1], z = g.q[2], w = g.q[3];
+    const double tx = mul(2.0, x), ty = mul(2.0, y), tz = mul(2.0, z);
+    const double twx = mul(tx, w), twy = mul(ty, w), twz = mul(tz, w);
+    const double txx = mul(tx, x), txy = mul(ty, x), txz = mul(tz, x);
+    const double tyy = mul(ty, y), tyz = mul(tz, y), tzz = mul(tz, z);
+    const double R[9] = {sub(1.0, add(tyy, tzz)), sub(txy, twz),           add(txz, twy),
+                         add(txy, twz),           sub(1.0, add(txx, tzz)), sub(tyz, twx),
+                         sub(txz, twy),           add(tyz, twx),           sub(1.0, add(txx, tyy))};
+    for (int i = 0; i < 3; ++i) {
+        for (int j = 0; j < 3; ++j) M[i * 4 + j] = R[i * 3 + j];
+        M[i * 4 + 3] = g.t[i];
+    }
+    M[12] = M[13] = M[14] = 0.0;
+    M[15] = 1.0;
+}
+
+// ---- align_points_to_map (icp_registration.cpp) ----
+struct IcpState {
+    SE3 inc;         // the previous iteration's estimation, applied to the source by the next association
+    SE3 pose;        // t_icp
+    int has_inc;
+    int done;        // converged, or the map is empty
+    int iterations;
+    int pad;
+    unsigned long long n_pairs;
+};
+
+constexpr unsigned kAssocThreads = 256;
+
+template <typename T>
+__global__ void icp_init_kernel(Rows r, const unsigned long long* ctr, double* src, IcpState* s) {
+    const unsigned i = tid_global();
+    if (i == 0) {
+        IcpState z{};
+        z.pose.q[3] = 1.0;
+        z.inc.q[3] = 1.0;
+        z.done = ctr[C_LIVE] == 0 ? 1 : 0;  // an empty map returns the identity
+        *s = z;
+    }
+    if (i >= r.cap || i >= rows_n(r)) return;
+    load3<T>(r.p, i, src + 3 * i);
+}
+
+// association (icp_registration.cpp data_association), fused with applying the previous increment in place
+__global__ void icp_assoc_kernel(Rows r, Table t, double inv, double vs, double max_d2, double* src, double* tgt,
+                                 uint32_t* valid, uint32_t* block_count, IcpState* s) {
+    if (s->done) return;
+    const unsigned i = tid_global();
+    const unsigned n = rows_n(r);
+    bool ok = false;
+    if (i < n) {
+        double p[3] = {src[3 * i], src[3 * i + 1], src[3 * i + 2]};
+        if (s->has_inc) {
+            double q[3];
+            se3_apply(s->inc, p, q);
+            for (int d = 0; d < 3; ++d) src[3 * i + d] = p[d] = q[d];
+        }
+        double nb[3];
+        const double d2 = closest(t, inv, vs, p, max_d2, nb);
+        ok = d2 < max_d2;
+        if (ok)
+            for (int d = 0; d < 3; ++d) tgt[3 * i + d] = nb[d];
+    }
+    if (i < r.cap) valid[i] = ok ? 1u : 0u;
+    const int c = __syncthreads_count(ok);
+    if (threadIdx.x == 0) block_count[blockIdx.x] = static_cast<uint32_t>(c);
+}
+
+// order-preserving compaction of the valid pairs; the last block writes the pair count
+__global__ void icp_compact_kernel(unsigned cap, const double* src, const double* tgt, const uint32_t* valid,
+                                   const uint32_t* block_count, double* ps, double* pt, IcpState* s) {
+    if (s->done) return;
+    using BR = cub::BlockReduce<unsigned, kAssocThreads>;
+    using BS = cub::BlockScan<unsigned, kAssocThreads>;
+    __shared__ union {
+        typename BR::TempStorage r;
+        typename BS::TempStorage s;
+    } tmp;
+    __shared__ unsigned base;
+    unsigned part = 0;
+    for (unsigned b = threadIdx.x; b < blockIdx.x; b += blockDim.x) part += block_count[b];
+    const unsigned before = BR(tmp.r).Sum(part);
+    if (threadIdx.x == 0) base = before;
+    __syncthreads();
+    const unsigned i = tid_global();
+    const unsigned f = i < cap ? valid[i] : 0u;
+    unsigned pos, total;
+    BS(tmp.s).ExclusiveSum(f, pos, total);
+    if (f) {
+        const size_t o = static_cast<size_t>(base) + pos;
+        for (int d = 0; d < 3; ++d) {
+            ps[3 * o + d] = src[3 * static_cast<size_t>(i) + d];
+            pt[3 * o + d] = tgt[3 * static_cast<size_t>(i) + d];
+        }
+    }
+    if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) s->n_pairs = base + total;
+}
+
+// the tree's parents, then (thread 0) the LDLT solve, SE3::exp, t_icp = estimation * t_icp and the stop test
+constexpr unsigned kTreeThreads = 256;
+
+__global__ void __launch_bounds__(kTreeThreads, 1) icp_solve_kernel(double* val, double crit_sq, IcpState* s) {
+    if (s->done) return;
+    const unsigned long long n = s->n_pairs;
+    tree_reduce(n, val);
+    if (threadIdx.x != 0) return;
+    double jtj[36], jtr[6], rhs[6], dx[6];
+    unpack_system(val, jtj, jtr);
+    for (int j = 0; j < 6; ++j) rhs[j] = -jtr[j];
+    ldlt_solve6(jtj, rhs, dx);
+    const SE3 est = se3_exp(dx);
+    s->pose = se3_mul(est, s->pose);
+    s->inc = est;
+    s->has_inc = 1;
+    s->iterations += 1;
+    // Vector6d::squaredNorm in Eigen's two-lane order
+    const double l0 = add(mul(dx[0], dx[0]), add(mul(dx[2], dx[2]), mul(dx[4], dx[4])));
+    const double l1 = add(mul(dx[1], dx[1]), add(mul(dx[3], dx[3]), mul(dx[5], dx[5])));
+    if (add(l0, l1) < crit_sq) s->done = 1;
+}
+
+__global__ void icp_finish_kernel(const IcpState* s, double* pose, int32_t* iterations) {
+    se3_matrix(s->pose, pose);
+    if (iterations) *iterations = s->iterations;
+}
+
+// build_linear_system on its own: the root of the tree, unpacked
+__global__ void __launch_bounds__(kTreeThreads, 1) icp_system_kernel(const unsigned long long* n_pairs,
+                                                                    unsigned long long max_n, double* val, double* jtj,
+                                                                    double* jtr) {
+    const unsigned long long n = n_pairs ? min(*n_pairs, max_n) : max_n;
+    tree_reduce(n, val);
+    if (threadIdx.x == 0) unpack_system(val, jtj, jtr);
+}
+
+}  // namespace
+}  // namespace ob
+
+using namespace ob;
+
+namespace {
+
+bool dtype_ok(int32_t d) { return d == OB_F32 || d == OB_F64; }
+
+// validate an ob_point_rows and stage it: host rows go through scratch; the row capacity is returned
+ob_status stage_rows(const ob_point_rows* in, Staging& stg, Rows* r, const char* what) {
+    if (!dtype_ok(in->dtype)) return fail(OB_INVALID_ARGUMENT, "unknown dtype");
+    const bool dev_n = in->n_device != nullptr;
+    const size_t cap = dev_n ? in->capacity : in->n;
+    if (cap > 0x7fffffffu) return fail(OB_INVALID_ARGUMENT, "too many points in one call");
+    if (dev_n && !is_device_ptr(in->n_device)) return fail(OB_INVALID_ARGUMENT, "n_device must be device memory");
+    if (cap && !in->points) return fail(OB_INVALID_ARGUMENT, "null points buffer");
+    const void* d = nullptr;
+    cudaError_t e = stg.in(in->points, cap * 3 * (in->dtype == OB_F64 ? 8 : 4), &d);
+    if (e != cudaSuccess) return fail_cuda(e, what);
+    r->p = d;
+    r->n_dev = reinterpret_cast<const unsigned long long*>(in->n_device);
+    r->n_host = in->n;
+    r->cap = static_cast<unsigned>(cap);
+    return OB_OK;
+}
+
+template <typename P>
+cudaError_t scratch(Staging& stg, size_t bytes, P** p) {
+    void* d = nullptr;
+    cudaError_t e = stg.scratch(bytes, &d);
+    *p = static_cast<P*>(d);
+    return e;
+}
+
+void free_table(ob_voxel_map* m) {
+    cudaFree(m->key);
+    cudaFree(m->state);
+    cudaFree(m->stamp);
+    cudaFree(m->cnt);
+    cudaFree(m->pts);
+    m->key = nullptr;
+    m->state = nullptr;
+    m->stamp = nullptr;
+    m->cnt = nullptr;
+    m->pts = nullptr;
+    m->cap = 0;
+}
+
+size_t table_bytes(size_t cap, size_t max_pts) { return cap * (12 + 4 + 8 + 4 + 24 * max_pts); }
+
+// a new, empty table in `t` (only its arrays and cap); on failure everything allocated here is freed again
+cudaError_t alloc_table(ob_voxel_map* t, unsigned cap, cudaStream_t st) {
+    t->key = nullptr;
+    t->state = nullptr;
+    t->stamp = nullptr;
+    t->cnt = nullptr;
+    t->pts = nullptr;
+    t->cap = cap;
+    cudaError_t e = cudaMalloc(&t->key, cap * 12ull);
+    if (e == cudaSuccess) e = cudaMalloc(&t->state, cap * 4ull);
+    if (e == cudaSuccess) e = cudaMalloc(&t->stamp, cap * 8ull);
+    if (e == cudaSuccess) e = cudaMalloc(&t->cnt, cap * 4ull);
+    if (e == cudaSuccess) e = cudaMalloc(&t->pts, cap * t->max_pts * 24ull);
+    if (e == cudaSuccess) e = cudaMemsetAsync(t->state, 0, cap * 4ull, st);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        free_table(t);
+    }
+    return e;
+}
+
+constexpr unsigned kMinSlots = 1024;
+
+// Make room before a batch of at most `rows` rows whose distinct voxel count is the device word *nv_dev (the batch
+// is already sorted and numbered).  The map waits for the host only here, and only when the host bound of occupied
+// slots plus `rows` could pass half the table: then it reads the counters and nv, and grows to the next power of two
+// >= 4 (live + nv) slots if live + tombstones + nv would pass half.  The new table is built and filled on the side
+// and committed only when every step succeeded; any failure leaves the map as it was.  *added = what the batch can
+// add to the occupied slots (rows, or the exact nv once it was read).
+ob_status reserve(ob_voxel_map* m, size_t rows, const uint32_t* nv_dev, cudaStream_t st, size_t* added) {
+    *added = rows;
+    if (m->cap && m->occupied_bound + rows <= m->cap / 2) return OB_OK;
+    unsigned long long c[C_WORDS] = {};
+    uint32_t nv = 0;
+    cudaError_t e = cudaMemcpyAsync(c, m->ctr, sizeof(c), cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&nv, nv_dev, 4, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return fail_cuda(e, "voxel map counters");
+    *added = nv;
+    m->occupied_bound = static_cast<size_t>(c[C_OCCUPIED]);
+    if (m->cap && m->occupied_bound + nv <= m->cap / 2) return OB_OK;
+    const size_t live = static_cast<size_t>(c[C_LIVE]);
+    const size_t need = 4 * (live + nv);
+    size_t cap = kMinSlots;
+    while (cap < need) cap <<= 1;
+    size_t free_b = 0, total_b = 0;
+    e = cudaMemGetInfo(&free_b, &total_b);
+    if (e != cudaSuccess) return fail_cuda(e, "voxel map allocation");
+    if (cap > (1ull << 31) || table_bytes(cap, m->max_pts) > free_b)
+        return fail(OB_RUNTIME_ERROR, "voxel map: a table of " + std::to_string(cap) + " slots (" +
+                                          std::to_string(table_bytes(cap, m->max_pts)) +
+                                          " bytes) does not fit in free device memory");
+    ob_voxel_map nt = *m;
+    e = alloc_table(&nt, static_cast<unsigned>(cap), st);
+    if (e != cudaSuccess) return fail_cuda(e, "voxel map allocation");
+    if (m->cap) {
+        vm_rehash_kernel<<<blocks_for(m->cap), 256, 0, st>>>(table_of(m), table_of(&nt));
+        count_launch();
+        count_launch_of(OB_FAM_VOXEL_MAP);
+        e = cudaGetLastError();
+    }
+    const unsigned long long occ = live;
+    if (e == cudaSuccess) e = cudaMemcpyAsync(m->ctr + C_OCCUPIED, &occ, 8, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);  // the old table is freed below, `occ` is on this stack
+    if (e != cudaSuccess) {
+        free_table(&nt);
+        return fail_cuda(e, "voxel map rehash");
+    }
+    free_table(m);
+    m->cap = nt.cap;
+    m->key = nt.key;
+    m->state = nt.state;
+    m->stamp = nt.stamp;
+    m->cnt = nt.cnt;
+    m->pts = nt.pts;
+    m->occupied_bound = live;
+    return OB_OK;
+}
+
+// a batch keyed, sorted and numbered by voxel (the first half of add_points)
+struct AddBatch {
+    VKey* sk;
+    uint32_t *sseq, *vrank, *seg_start;
+};
+
+template <typename T>
+cudaError_t sort_batch(const ob_voxel_map* m, Rows r, Staging& stg, cudaStream_t st, AddBatch* b) {
+    const unsigned cap = r.cap;
+    const unsigned nb = blocks_for(cap);
+    VKey* keys;
+    uint32_t *seq, *opens;
+    cudaError_t e = scratch(stg, cap * sizeof(VKey), &keys);
+    if (e == cudaSuccess) e = scratch(stg, cap * sizeof(VKey), &b->sk);
+    if (e == cudaSuccess) e = scratch(stg, cap * 4ull, &seq);
+    if (e == cudaSuccess) e = scratch(stg, cap * 4ull, &b->sseq);
+    if (e == cudaSuccess) e = scratch(stg, cap * 4ull, &opens);
+    if (e == cudaSuccess) e = scratch(stg, cap * 4ull, &b->vrank);
+    if (e == cudaSuccess) e = scratch(stg, cap * 4ull, &b->seg_start);
+    if (e != cudaSuccess) return e;
+    size_t need = 0, tmp_bytes = 0;
+    e = cub::DeviceRadixSort::SortPairs(nullptr, need, keys, b->sk, seq, b->sseq, static_cast<int>(cap),
+                                        VKeyDecomposer{}, 0, kKeyBits, st);
+    tmp_bytes = need;
+    if (e == cudaSuccess) e = cub::DeviceScan::InclusiveSum(nullptr, need, opens, b->vrank, static_cast<int>(cap), st);
+    tmp_bytes = std::max(tmp_bytes, need);
+    void* tmp = nullptr;
+    if (e == cudaSuccess) e = stg.scratch(tmp_bytes, &tmp);
+    if (e != cudaSuccess) return e;
+    vm_key_kernel<T><<<nb, 256, 0, st>>>(r, m->inv, keys, seq);
+    e = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, b->sk, seq, b->sseq, static_cast<int>(cap),
+                                        VKeyDecomposer{}, 0, kKeyBits, st);
+    if (e != cudaSuccess) return e;
+    vx_head_kernel<<<nb, 256, 0, st>>>(cap, b->sk, b->sseq, opens);
+    e = cub::DeviceScan::InclusiveSum(tmp, tmp_bytes, opens, b->vrank, static_cast<int>(cap), st);
+    if (e != cudaSuccess) return e;
+    vx_seg_kernel<<<nb, 256, 0, st>>>(cap, b->sk, b->sseq, b->vrank, b->seg_start);
+    count_launch(3);
+    count_launch_of(OB_FAM_VOXEL_MAP, 3);
+    return cudaGetLastError();
+}
+
+// the second half: every distinct voxel of the batch into the table
+template <typename T>
+cudaError_t insert_batch(ob_voxel_map* m, Rows r, const AddBatch& b, cudaStream_t st) {
+    vm_insert_kernel<T><<<blocks_for(r.cap), 256, 0, st>>>(r, table_of(m), m->ctr, b.sk, b.sseq, b.vrank, b.seg_start,
+                                                            m->res_sq);
+    vm_advance_stamp_kernel<<<1, 1, 0, st>>>(r.cap, b.vrank, m->ctr);
+    count_launch(2);
+    count_launch_of(OB_FAM_VOXEL_MAP, 2);
+    return cudaGetLastError();
+}
+
+// rows of the selected voxels (sel == null: every live voxel) in creation order into out (capacity rows);
+// *n_dev = the number of rows selected
+cudaError_t run_emit(const ob_voxel_map* m, const uint32_t* sel, Staging& stg, cudaStream_t st, double* out,
+                     size_t capacity, unsigned long long* n_dev) {
+    const unsigned cap = m->cap;
+    if (cap == 0) return cudaMemsetAsync(n_dev, 0, 8, st);
+    unsigned long long *keys, *skeys;
+    uint32_t *slots, *sslots, *c, *off;
+    cudaError_t e = scratch(stg, cap * 8ull, &keys);
+    if (e == cudaSuccess) e = scratch(stg, cap * 8ull, &skeys);
+    if (e == cudaSuccess) e = scratch(stg, cap * 4ull, &slots);
+    if (e == cudaSuccess) e = scratch(stg, cap * 4ull, &sslots);
+    if (e == cudaSuccess) e = scratch(stg, cap * 4ull, &c);
+    if (e == cudaSuccess) e = scratch(stg, cap * 4ull, &off);
+    if (e != cudaSuccess) return e;
+    size_t need = 0, tmp_bytes = 0;
+    e = cub::DeviceRadixSort::SortPairs(nullptr, need, keys, skeys, slots, sslots, static_cast<int>(cap), 0, 64, st);
+    tmp_bytes = need;
+    if (e == cudaSuccess) e = cub::DeviceScan::InclusiveSum(nullptr, need, c, off, static_cast<int>(cap), st);
+    tmp_bytes = std::max(tmp_bytes, need);
+    void* tmp = nullptr;
+    if (e == cudaSuccess) e = stg.scratch(tmp_bytes, &tmp);
+    if (e != cudaSuccess) return e;
+    const Table t = table_of(m);
+    const unsigned nb = blocks_for(cap);
+    vm_emit_keys_kernel<<<nb, 256, 0, st>>>(t, sel, keys, slots);
+    e = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, skeys, slots, sslots, static_cast<int>(cap), 0, 64, st);
+    if (e != cudaSuccess) return e;
+    vm_emit_counts_kernel<<<nb, 256, 0, st>>>(t, skeys, sslots, c);
+    e = cub::DeviceScan::InclusiveSum(tmp, tmp_bytes, c, off, static_cast<int>(cap), st);
+    if (e != cudaSuccess) return e;
+    vm_emit_kernel<<<nb, 256, 0, st>>>(t, skeys, sslots, off, out, capacity, n_dev);
+    count_launch(3);
+    count_launch_of(OB_FAM_VOXEL_MAP, 3);
+    return cudaGetLastError();
+}
+
+// rows written to `out` (host or device) with the count to `n_out` (host: one synchronisation; device: none)
+ob_status emit_rows(const ob_voxel_map* m, const uint32_t* sel, Staging& stg, cudaStream_t st, double* out,
+                    size_t capacity, size_t* n_out, const char* what) {
+    const bool dev_count = is_device_ptr(n_out);
+    const bool host_out = out && !is_device_ptr(out);
+    if (dev_count && host_out) return fail(OB_INVALID_ARGUMENT, "a device-side count needs device outputs");
+    double* dout = out;
+    cudaError_t e = cudaSuccess;
+    if (host_out && capacity) e = scratch(stg, capacity * 24, &dout);
+    unsigned long long* dn = reinterpret_cast<unsigned long long*>(n_out);
+    if (e == cudaSuccess && !dev_count) e = scratch(stg, 8, &dn);
+    if (e == cudaSuccess) e = run_emit(m, sel, stg, st, dout, out ? capacity : 0, dn);
+    if (e != cudaSuccess) return fail_cuda(e, what);
+    if (dev_count) return OB_OK;
+    unsigned long long total = 0;
+    e = cudaMemcpyAsync(&total, dn, 8, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e == cudaSuccess && host_out && total)
+        e = cudaMemcpyAsync(out, dout, std::min<size_t>(total, capacity) * 24, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess && host_out) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return fail_cuda(e, what);
+    *n_out = static_cast<size_t>(total);
+    if (out && total > capacity) return fail(OB_INVALID_ARGUMENT, "output capacity too small");
+    return OB_OK;
+}
+
+// max_voxel_dist_sq of remove_voxels_far_from_location (voxel_hash_map.cpp:112-113) in x86 int32 arithmetic
+int32_t cull_threshold(double max_distance, double inv) {
+    const double c = std::ceil(max_distance * inv);
+    const uint32_t d = static_cast<uint32_t>(c >= -2147483648.0 && c < 2147483648.0 ? static_cast<int32_t>(c) : INT32_MIN) + 1u;
+    return static_cast<int32_t>(d * d);
+}
+
+// leaf values of the deterministic-reduce tree for up to `cap` pairs
+unsigned tree_slots(size_t cap) { return 1u << tree_depth(cap); }
+
+}  // namespace
+
+extern "C" {
+
+ob_status ob_voxel_map_create(double voxel_size, double max_distance, size_t max_points_per_voxel,
+                              size_t min_pts_threshold, int device, ob_voxel_map** out) {
+    if (!out) return fail(OB_INVALID_ARGUMENT, "null output pointer");
+    // the constructor's checks in its order (voxel_hash_map.cpp:23-31)
+    if (max_points_per_voxel == 0) return fail(OB_INVALID_ARGUMENT, "max_points_per_voxel must be greater than 0");
+    if (voxel_size <= 0) return fail(OB_INVALID_ARGUMENT, "voxel_size must be greater than 0");
+    if (max_distance <= 0) return fail(OB_INVALID_ARGUMENT, "max_distance must be greater than 0");
+    if (max_points_per_voxel > 0xffffu) return fail(OB_INVALID_ARGUMENT, "max_points_per_voxel too large");
+    ob_status rs = require_device(device);
+    if (rs != OB_OK) return rs;
+    ob_voxel_map* m = new ob_voxel_map{};
+    m->device = device;
+    m->voxel_size = voxel_size;
+    m->max_distance = max_distance;
+    m->max_pts = max_points_per_voxel;
+    m->min_pts = min_pts_threshold;
+    m->res_sq = voxel_size * voxel_size / static_cast<double>(max_points_per_voxel);  // :38
+    m->inv = 1.0 / voxel_size;                                                          // :39
+    cudaError_t e = cudaMalloc(&m->ctr, C_WORDS * 8);
+    if (e == cudaSuccess) e = cudaMemset(m->ctr, 0, C_WORDS * 8);
+    if (e != cudaSuccess) {
+        cudaFree(m->ctr);
+        delete m;
+        return fail_cuda(e, "voxel map allocation");
+    }
+    *out = m;
+    return OB_OK;
+}
+
+ob_status ob_voxel_map_destroy(ob_voxel_map* m) {
+    if (!m) return OB_OK;
+    cudaSetDevice(m->device);
+    free_table(m);
+    cudaFree(m->ctr);
+    delete m;
+    return OB_OK;
+}
+
+ob_status ob_voxel_map_clear(ob_voxel_map* m, ob_stream* s) {
+    if (!m || !s) return fail(OB_INVALID_ARGUMENT, "null pointer");
+    ob_status rs = require_device(m->device);
+    if (rs != OB_OK) return rs;
+    cudaStream_t st = stream_handle(s);
+    cudaError_t e = cudaSuccess;
+    if (m->cap) e = cudaMemsetAsync(m->state, 0, m->cap * 4ull, st);
+    // the stamp counter keeps running: creation order stays monotone across clears
+    if (e == cudaSuccess) e = cudaMemsetAsync(m->ctr + C_LIVE, 0, (C_WORDS - C_LIVE) * 8, st);
+    if (e != cudaSuccess) return fail_cuda(e, "voxel map clear");
+    m->occupied_bound = 0;
+    return OB_OK;
+}
+
+ob_status ob_voxel_map_add_points(ob_voxel_map* m, const ob_point_rows* rows, ob_stream* s) {
+    if (!m || !rows || !s) return fail(OB_INVALID_ARGUMENT, "null pointer");
+    ob_status rs = require_device(m->device);
+    if (rs != OB_OK) return rs;
+    cudaStream_t st = stream_handle(s);
+    Staging stg(st);
+    Rows r{};
+    rs = stage_rows(rows, stg, &r, "stage voxel map rows");
+    if (rs != OB_OK || r.cap == 0) return rs;
+    const bool f64 = rows->dtype == OB_F64;
+    AddBatch b{};
+    cudaError_t e = f64 ? sort_batch<double>(m, r, stg, st, &b) : sort_batch<float>(m, r, stg, st, &b);
+    if (e != cudaSuccess) return fail_cuda(e, "voxel map add_points");
+    size_t added = 0;
+    rs = reserve(m, r.cap, b.vrank + r.cap - 1, st, &added);
+    if (rs != OB_OK) return rs;  // nothing inserted; the map is as it was
+    e = f64 ? insert_batch<double>(m, r, b, st) : insert_batch<float>(m, r, b, st);
+    if (e != cudaSuccess) return fail_cuda(e, "voxel map add_points");
+    m->occupied_bound += added;
+    return OB_OK;
+}
+
+ob_status ob_voxel_map_remove_far(ob_voxel_map* m, const ob_voxel_map_cull_io* io, ob_stream* s) {
+    if (!m || !io || !s || !io->origin) return fail(OB_INVALID_ARGUMENT, "null pointer");
+    if (io->extracted && !io->n_extracted) return fail(OB_INVALID_ARGUMENT, "extraction needs n_extracted");
+    ob_status rs = require_device(m->device);
+    if (rs != OB_OK) return rs;
+    cudaStream_t st = stream_handle(s);
+    Staging stg(st);
+    const void* org = nullptr;
+    cudaError_t e = stg.in(io->origin, 24, &org);
+    if (e != cudaSuccess) return fail_cuda(e, "stage origin");
+    uint32_t* removed = nullptr;
+    const bool extract = io->n_extracted != nullptr;
+    if (extract && m->cap) {
+        e = scratch(stg, m->cap * 4ull, &removed);
+        if (e != cudaSuccess) return fail_cuda(e, "voxel map cull");
+    }
+    if (m->cap) {
+        vm_cull_kernel<<<blocks_for(m->cap), 256, 0, st>>>(table_of(m), m->ctr, static_cast<const double*>(org), m->inv,
+                                                            cull_threshold(m->max_distance, m->inv), removed);
+        count_launch();
+        count_launch_of(OB_FAM_VOXEL_MAP);
+        e = cudaGetLastError();
+        if (e != cudaSuccess) return fail_cuda(e, "voxel map cull");
+    }
+    if (!extract) return OB_OK;
+    if (!m->cap) {
+        if (is_device_ptr(io->n_extracted)) {
+            e = cudaMemsetAsync(io->n_extracted, 0, 8, st);
+            return e == cudaSuccess ? OB_OK : fail_cuda(e, "voxel map cull");
+        }
+        *io->n_extracted = 0;
+        return OB_OK;
+    }
+    return emit_rows(m, removed, stg, st, io->extracted, io->capacity, io->n_extracted, "voxel map extract");
+}
+
+ob_status ob_voxel_map_point_cloud(const ob_voxel_map* m, double* points, size_t capacity, size_t* n_out, ob_stream* s) {
+    if (!m || !s || !n_out) return fail(OB_INVALID_ARGUMENT, "null pointer");
+    ob_status rs = require_device(m->device);
+    if (rs != OB_OK) return rs;
+    cudaStream_t st = stream_handle(s);
+    Staging stg(st);
+    if (!m->cap) {
+        if (is_device_ptr(n_out)) {
+            cudaError_t e = cudaMemsetAsync(n_out, 0, 8, st);
+            return e == cudaSuccess ? OB_OK : fail_cuda(e, "voxel map point cloud");
+        }
+        *n_out = 0;
+        return OB_OK;
+    }
+    return emit_rows(m, nullptr, stg, st, points, capacity, n_out, "voxel map point cloud");
+}
+
+ob_status ob_voxel_map_size(const ob_voxel_map* m, size_t* voxels, size_t* points, ob_stream* s) {
+    if (!m || !s) return fail(OB_INVALID_ARGUMENT, "null pointer");
+    ob_status rs = require_device(m->device);
+    if (rs != OB_OK) return rs;
+    cudaStream_t st = stream_handle(s);
+    unsigned long long c[C_WORDS] = {};
+    cudaError_t e = cudaMemcpyAsync(c, m->ctr, sizeof(c), cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return fail_cuda(e, "voxel map size");
+    if (c[C_FULL]) return fail(OB_RUNTIME_ERROR, "voxel map table overflow");
+    if (voxels) *voxels = static_cast<size_t>(c[C_LIVE]);
+    if (points) *points = static_cast<size_t>(c[C_POINTS]);
+    return OB_OK;
+}
+
+ob_status ob_voxel_map_closest_neighbors(const ob_voxel_map* m, const ob_voxel_query_io* io, ob_stream* s) {
+    if (!m || !io || !s) return fail(OB_INVALID_ARGUMENT, "null pointer");
+    ob_status rs = require_device(m->device);
+    if (rs != OB_OK) return rs;
+    cudaStream_t st = stream_handle(s);
+    Staging stg(st);
+    Rows r{};
+    rs = stage_rows(&io->queries, stg, &r, "stage queries");
+    if (rs != OB_OK || r.cap == 0) return rs;
+    if (!io->neighbors) return fail(OB_INVALID_ARGUMENT, "null neighbors buffer");
+    void *nb = nullptr, *d2 = nullptr;
+    cudaError_t e = stg.out(io->neighbors, r.cap * 24ull, &nb);
+    if (e == cudaSuccess) e = stg.out(io->distances_sq, r.cap * 8ull, &d2);
+    if (e != cudaSuccess) return fail_cuda(e, "stage neighbors");
+    const Table t = table_of(m);
+    if (io->queries.dtype == OB_F64)
+        vm_closest_kernel<double><<<blocks_for(r.cap), 256, 0, st>>>(r, t, m->inv, m->voxel_size, io->max_distance_sq,
+                                                                      static_cast<double*>(nb), static_cast<double*>(d2));
+    else
+        vm_closest_kernel<float><<<blocks_for(r.cap), 256, 0, st>>>(r, t, m->inv, m->voxel_size, io->max_distance_sq,
+                                                                     static_cast<double*>(nb), static_cast<double*>(d2));
+    count_launch();
+    count_launch_of(OB_FAM_VOXEL_MAP);
+    e = cudaGetLastError();
+    if (e == cudaSuccess) e = stg.flush();
+    if (e != cudaSuccess) return fail_cuda(e, "voxel map closest neighbors");
+    return OB_OK;
+}
+
+ob_status ob_icp_linear_system(const ob_icp_system_io* io, ob_stream* s) {
+    if (!io || !s || !io->jtj || !io->jtr) return fail(OB_INVALID_ARGUMENT, "null pointer");
+    const int device = stream_device(s);
+    ob_status rs = require_device(device);
+    if (rs != OB_OK) return rs;
+    cudaStream_t st = stream_handle(s);
+    Staging stg(st);
+    const bool dev_n = io->n_device != nullptr;
+    const size_t cap = dev_n ? io->capacity : io->n;
+    if (cap > 0x7fffffffu) return fail(OB_INVALID_ARGUMENT, "too many pairs in one call");
+    if (dev_n && !is_device_ptr(io->n_device)) return fail(OB_INVALID_ARGUMENT, "n_device must be device memory");
+    if (cap && (!io->source || !io->target)) return fail(OB_INVALID_ARGUMENT, "null pairs buffer");
+    const void *src = nullptr, *tgt = nullptr;
+    void *jtj = nullptr, *jtr = nullptr;
+    cudaError_t e = stg.in(io->source, cap * 24, &src);
+    if (e == cudaSuccess) e = stg.in(io->target, cap * 24, &tgt);
+    if (e == cudaSuccess) e = stg.out(io->jtj, 36 * 8, &jtj);
+    if (e == cudaSuccess) e = stg.out(io->jtr, 6 * 8, &jtr);
+    // a host count travels by value as the clamp (cap == n), a device count is read by the kernels
+    const unsigned long long* n = reinterpret_cast<const unsigned long long*>(io->n_device);
+    const unsigned slots = tree_slots(cap);
+    double* val = nullptr;
+    if (e == cudaSuccess) e = scratch(stg, slots * kSys * 8ull, &val);
+    if (e != cudaSuccess) return fail_cuda(e, "stage linear system");
+    icp_leaf_kernel<<<blocks_for(slots), 256, 0, st>>>(static_cast<const double*>(src), static_cast<const double*>(tgt), n,
+                                                        cap, io->kernel_scale, nullptr, slots, val);
+    icp_system_kernel<<<1, kTreeThreads, 0, st>>>(n, cap, val, static_cast<double*>(jtj), static_cast<double*>(jtr));
+    count_launch(2);
+    count_launch_of(OB_FAM_ICP, 2);
+    e = cudaGetLastError();
+    if (e == cudaSuccess) e = stg.flush();
+    if (e == cudaSuccess && (!is_device_ptr(io->jtj) || !is_device_ptr(io->jtr))) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return fail_cuda(e, "icp linear system");
+    return OB_OK;
+}
+
+ob_status ob_icp_align(const ob_voxel_map* m, const ob_icp_io* io, ob_stream* s) {
+    if (!m || !io || !s || !io->pose) return fail(OB_INVALID_ARGUMENT, "null pointer");
+    ob_status rs = require_device(m->device);
+    if (rs != OB_OK) return rs;
+    cudaStream_t st = stream_handle(s);
+    Staging stg(st);
+    Rows r{};
+    rs = stage_rows(&io->source, stg, &r, "stage icp source");
+    if (rs != OB_OK) return rs;
+    const bool dev_pose = is_device_ptr(io->pose);
+    const bool dev_it = io->iterations == nullptr || is_device_ptr(io->iterations);
+    double* pose = io->pose;
+    int32_t* iters = io->iterations;
+    IcpState* state = nullptr;
+    cudaError_t e = scratch(stg, sizeof(IcpState), &state);
+    if (e == cudaSuccess && !dev_pose) e = scratch(stg, 16 * 8, &pose);
+    if (e == cudaSuccess && !dev_it) e = scratch(stg, 4, &iters);
+    const unsigned cap = std::max(r.cap, 1u);
+    const unsigned nb = (cap + kAssocThreads - 1) / kAssocThreads;
+    const unsigned slots = tree_slots(cap);
+    double *src = nullptr, *tgt = nullptr, *ps = nullptr, *pt = nullptr, *val = nullptr;
+    uint32_t *valid = nullptr, *bc = nullptr;
+    if (e == cudaSuccess) e = scratch(stg, cap * 24ull, &src);
+    if (e == cudaSuccess) e = scratch(stg, cap * 24ull, &tgt);
+    if (e == cudaSuccess) e = scratch(stg, cap * 24ull, &ps);
+    if (e == cudaSuccess) e = scratch(stg, cap * 24ull, &pt);
+    if (e == cudaSuccess) e = scratch(stg, cap * 4ull, &valid);
+    if (e == cudaSuccess) e = scratch(stg, nb * 4ull, &bc);
+    if (e == cudaSuccess) e = scratch(stg, slots * kSys * 8ull, &val);
+    if (e != cudaSuccess) return fail_cuda(e, "icp workspace");
+    const Table t = table_of(m);
+    const double md2 = io->max_distance * io->max_distance;  // square(max_correspondance_distance)
+    const double crit_sq = io->convergence_criterion * io->convergence_criterion;
+    if (io->source.dtype == OB_F64) icp_init_kernel<double><<<nb, kAssocThreads, 0, st>>>(r, m->ctr, src, state);
+    else icp_init_kernel<float><<<nb, kAssocThreads, 0, st>>>(r, m->ctr, src, state);
+    uint64_t launches = 2;
+    for (int it = 0; it < io->max_num_iterations; ++it) {
+        icp_assoc_kernel<<<nb, kAssocThreads, 0, st>>>(r, t, m->inv, m->voxel_size, md2, src, tgt, valid, bc, state);
+        icp_compact_kernel<<<nb, kAssocThreads, 0, st>>>(r.cap, src, tgt, valid, bc, ps, pt, state);
+        icp_leaf_kernel<<<blocks_for(slots), 256, 0, st>>>(ps, pt, &state->n_pairs, cap, io->kernel_scale, &state->done,
+                                                            slots, val);
+        icp_solve_kernel<<<1, kTreeThreads, 0, st>>>(val, crit_sq, state);
+        launches += 4;
+    }
+    icp_finish_kernel<<<1, 1, 0, st>>>(state, pose, iters);
+    count_launch(launches);
+    count_launch_of(OB_FAM_ICP, launches);
+    e = cudaGetLastError();
+    if (e != cudaSuccess) return fail_cuda(e, "icp launch");
+    if (dev_pose && dev_it) return OB_OK;  // nothing waits for the GPU
+    if (!dev_pose) e = cudaMemcpyAsync(io->pose, pose, 16 * 8, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess && !dev_it) e = cudaMemcpyAsync(io->iterations, iters, 4, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return fail_cuda(e, "icp result");
+    return OB_OK;
+}
+
+}  // extern "C"

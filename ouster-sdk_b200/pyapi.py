@@ -332,3 +332,145 @@ class DeviceScanBatcher:
 
     batched_packets = property(lambda self: self._b.batched_packets)
     dropped_packets = property(lambda self: self._b.dropped_packets)
+
+
+# ---- frame-to-map registration (DESIGN f-6) -----------------------------------------------------------
+# ouster.sdk.core.VoxelHashMap3d (processing.cpp:395-470, 1040-1055) and ouster.sdk.mapping.ICPRegistration /
+# AdaptiveThreshold (python/src/cpp/mapping/_mapping_registration.cpp).  numpy in and out as in the reference; torch
+# CUDA tensors are accepted as well and keep the work on the device.
+
+DBL_MAX = _c.DBL_MAX
+
+
+def _point3(point):
+    d = _dev(point)
+    p = d.double().reshape(-1) if d is not None else np.ascontiguousarray(point, np.float64).reshape(-1)
+    if p.shape[0] != 3:
+        raise ValueError("VoxelHashMap method expects a 3-element point")
+    return p
+
+
+def _rows3(points, msg="add_points expects an Nx3 array"):
+    d = _dev(points)
+    p = d if d is not None else np.ascontiguousarray(points, np.float64)
+    if len(p.shape) != 2 or p.shape[1] != 3:
+        raise ValueError(msg)
+    return p
+
+
+class VoxelHashMap3d:
+    """core.VoxelHashMap3d: first_n_point voxel map, held in device memory.  point_cloud() and
+    extract_voxels_far_from_location() list voxels in creation order (the reference: hash-map order, DESIGN 9)."""
+
+    def __init__(self, voxel_size=0.1, max_distance=100.0, max_points_per_voxel=20, min_pts_threshold=1):
+        self._m = _c.VoxelMap(voxel_size, max_distance, max_points_per_voxel, min_pts_threshold)
+
+    @property
+    def empty(self):
+        return self._m.size()[0] == 0
+
+    def max_points_per_voxel(self):
+        return self._m.max_points_per_voxel
+
+    def min_pts_threshold(self):
+        return self._m.min_pts_threshold
+
+    def clear(self):
+        self._m.clear()
+
+    def add_points(self, points):
+        self._m.add_points(_rows3(points))
+
+    def point_cloud(self):
+        return self._m.point_cloud()
+
+    def remove_voxels_far_from_location(self, point):
+        self._m.remove_far(_point3(point))
+
+    def extract_voxels_far_from_location(self, point):
+        return self._m.remove_far(_point3(point), extract=True)
+
+    def get_closest_neighbor(self, point, max_distance_sq=DBL_MAX):
+        """(closest point [3] float64, squared distance); ((0, 0, 0), max_distance_sq) when nothing qualifies."""
+        p = _point3(point)
+        nb, d2 = self._m.closest_neighbors(p.reshape(1, 3), max_distance_sq)
+        if _c._is_torch(nb):
+            nb, d2 = nb.cpu().numpy(), d2.cpu().numpy()
+        return nb[0], float(d2[0])
+
+    def get_closest_neighbors(self, points, max_distance_sq=DBL_MAX):
+        """Batched get_closest_neighbor: (points [n, 3], squared distances [n]); CUDA tensors in, CUDA tensors out."""
+        return self._m.closest_neighbors(_rows3(points, "VoxelHashMap method expects a 3-element point"),
+                                         max_distance_sq)
+
+
+class ICPRegistration:
+    """mapping.ICPRegistration(max_num_iterations=50, convergence_criterion=1e-4, max_num_threads=0).
+    max_num_threads has no effect on the GPU; like the reference it reads back as a positive number."""
+
+    def __init__(self, max_num_iterations=50, convergence_criterion=0.0001, max_num_threads=0):
+        import os
+        self.max_num_iterations = int(max_num_iterations)
+        self.convergence_criterion = float(convergence_criterion)
+        self.max_num_threads = int(max_num_threads) if max_num_threads > 0 else (os.cpu_count() or 1)
+
+    def align_points_to_map(self, frame, voxel_map, max_distance, kernel_scale):
+        """4x4 float64 correction that moves `frame` onto the map (a CUDA tensor for a CUDA-tensor frame)."""
+        m = voxel_map._m if isinstance(voxel_map, VoxelHashMap3d) else voxel_map
+        pose, _ = _c.icp_align(m, _rows3(frame), max_distance, kernel_scale, self.max_num_iterations,
+                               self.convergence_criterion)
+        return pose
+
+
+def build_linear_system(source, target, kernel_scale):
+    """mapping build_linear_system over the pairs (source[i], target[i]): (JtJ 6x6, lower triangle, Jtr [6])."""
+    return _c.icp_linear_system(source, target, kernel_scale)
+
+
+class AdaptiveThreshold:
+    """mapping.AdaptiveThreshold (adaptive_threshold.h, adaptive_threshold.cpp): host scalars."""
+
+    def __init__(self, max_range, initial_threshold=2.0, min_motion_threshold=0.01):
+        self.min_motion_threshold = float(min_motion_threshold)
+        self.max_range = float(max_range)
+        self.model_sse = float(initial_threshold) * float(initial_threshold)
+        self.num_samples = 1
+
+    @staticmethod
+    def _angle(r):
+        """Eigen::AngleAxisd(R).angle(): R -> quaternion (Quaternion.h, quaternionbase_assign_impl), then
+        2 atan2(|vec|, |w|)."""
+        t = r[0, 0] + r[1, 1] + r[2, 2]
+        if t > 0:
+            s = np.sqrt(t + 1.0)
+            w = 0.5 * s
+            s = 0.5 / s
+            v = np.array([(r[2, 1] - r[1, 2]) * s, (r[0, 2] - r[2, 0]) * s, (r[1, 0] - r[0, 1]) * s])
+        else:
+            i = 0
+            if r[1, 1] > r[0, 0]:
+                i = 1
+            if r[2, 2] > r[i, i]:
+                i = 2
+            j, k = (i + 1) % 3, (i + 2) % 3
+            s = np.sqrt(r[i, i] - r[j, j] - r[k, k] + 1.0)
+            v = np.zeros(3)
+            v[i] = 0.5 * s
+            s = 0.5 / s
+            w = (r[k, j] - r[j, k]) * s
+            v[j] = (r[j, i] + r[i, j]) * s
+            v[k] = (r[k, i] + r[i, k]) * s
+        n = float(np.linalg.norm(v))
+        return 0.0 if n < np.finfo(np.float64).eps else 2.0 * np.arctan2(n, abs(w))
+
+    def update_model_deviation(self, current_deviation):
+        m = np.asarray(current_deviation, np.float64).reshape(4, 4)
+        delta_rot = 2.0 * self.max_range * np.sin(self._angle(m[:3, :3]) / 2.0)
+        delta_trans = float(np.linalg.norm(m[:3, 3]))
+        model_error = delta_trans + delta_rot
+        if model_error > self.min_motion_threshold:
+            self.model_sse += model_error * model_error
+            self.num_samples += 1
+
+    def compute_threshold(self):
+        return float(np.sqrt(self.model_sse / self.num_samples))

@@ -281,4 +281,22 @@ gp, gn, _ = ob.voxel_downsample(vp[:, :3].copy(), 0.5, "point_normal", normals=v
 wp, wn = orv.voxel_downsample_with_normals(vp[:, :3], vn, 0.5)
 assert np.array_equal(gp, wp) and np.array_equal(gn, wn)
 print("voxel ok")
+# voxel map + ICP: add (f32 and f64), cull with extraction, point cloud, closest neighbours, linear system, align
+from oracle import icp as oi
+rs = np.random.default_rng(11)
+gm, om = ob.VoxelMap(0.5, 3.0, 3), oi.VoxelHashMap3d(0.5, 3.0, 3)
+for k in range(3):
+    vm_pts = rs.normal(k, 2.0, (600, 3))
+    gm.add_points(vm_pts.astype(np.float32) if k % 2 else vm_pts)
+    om.add_points(vm_pts.astype(np.float32).astype(np.float64) if k % 2 else vm_pts)
+    assert np.array_equal(gm.remove_far([k, 0, 0], extract=True), om.extract_voxels_far_from_location([k, 0, 0]))
+assert np.array_equal(gm.point_cloud(), om.point_cloud())
+vq = rs.normal(0, 2.0, (300, 3))
+assert all(np.array_equal(a, b) for a, b in zip(gm.closest_neighbors(vq, 1.0), om.get_closest_neighbors(vq, 1.0)))
+assert all(np.array_equal(a, b) for a, b in zip(ob.icp_linear_system(vq, vq + 0.01, 0.5),
+                                                  oi.build_linear_system(vq, vq + 0.01, 0.5)))
+vp, vit = ob.icp_align(gm, om.point_cloud() + 0.02, 1.0, 0.5, 10)
+wp, wit = oi.align_points_to_map(om.point_cloud() + 0.02, om, 1.0, 0.5, 10)
+assert vit == wit and np.abs(vp - wp).max() <= 1e-12
+print("voxel map / icp ok")
 print("SANITIZE CASES OK")
