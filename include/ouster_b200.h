@@ -51,7 +51,8 @@ typedef struct ob_decoder ob_decoder; /* device-resident PacketFormat decode tab
 int ob_abi_version(void);
 /* sizeof() of a public struct by name ("ob_cloud_io", "ob_field_desc", "ob_packet_layout",
  * "ob_decode_io", "ob_decode_batch", "ob_dewarp_frame_io", "ob_normals_io", "ob_encode_io", "ob_dewarp_frames_io",
- * "ob_voxel_io", "ob_point_rows", "ob_voxel_map_cull_io", "ob_voxel_query_io", "ob_icp_io", "ob_icp_system_io");
+ * "ob_voxel_io", "ob_point_rows", "ob_voxel_map_cull_io", "ob_voxel_query_io", "ob_icp_io", "ob_icp_system_io",
+ * "ob_cloud_align_io", "ob_cloud_nearest_io");
  * 0 for unknown names.  Lets FFI bindings verify their layout. */
 size_t ob_abi_sizeof(const char* struct_name);
 const char* ob_last_error(void);
@@ -60,7 +61,7 @@ int ob_device_count(void);
 /* kernels launched by this library since load (all threads); the bench's gpu_launches claim */
 uint64_t ob_kernel_launch_count(void);
 /* launches of one named kernel family since load: "decode_pipe" (pipelined K2), "decode" (K2, any
- * kernel), "cloud" (K1), "normals", "voxel", "voxel_map", "icp"; 0 for unknown names.  Lets tests assert which code path ran. */
+ * kernel), "cloud" (K1), "normals", "voxel", "voxel_map", "icp", "align"; 0 for unknown names.  Lets tests assert which code path ran. */
 uint64_t ob_kernel_launch_count_of(const char* name);
 /* tuning hook (launch geometry and code-path selection only, never results): cloud_tw, cloud_stages,
  * cloud_threads (compute threads; a copy warp is added), cloud_ctas_per_sm, cloud_store_lag,
@@ -376,6 +377,56 @@ typedef struct ob_icp_system_io {
     double* jtr;
 } ob_icp_system_io;
 ob_status ob_icp_linear_system(const ob_icp_system_io* io, ob_stream* s);
+
+/* ---- cloud-to-cloud ICP (DESIGN f-7) ---- */
+typedef enum ob_align_mode { OB_ALIGN_POINT_TO_POINT = 0, OB_ALIGN_POINT_TO_PLANE = 1 } ob_align_mode;
+
+/* replaces algorithm::point_to_point_align and algorithm::point_to_plane_align
+ *          ouster_algorithm/src/align_clouds.cpp:1590-1874 (declared in align_clouds.h:20-84), with the
+ *          SpatialHashGrid3D they search (align_clouds.cpp:146-235, impl/spatial_hash.h:73-101)
+ * source / target: rows of one dtype (a device count works as for ob_icp_align).  POINT_TO_PLANE also reads
+ * source_normals / target_normals (rows x 3 of that dtype; *_normal_rows is their row count, which must equal the
+ * points' rows: n, or capacity with n_device).  initial_guess: 16 doubles, row-major, host or device (NULL: the
+ * identity).  pose: 16 doubles out; iterations (optional): the iterations that reached the solve (the SVD or the
+ * LDLT).  At most 10 iterations; fewer than 20 rows in either cloud, or no iteration with 20 correspondences, give
+ * initial_guess back bit for bit.  Device pose and iterations: nothing waits for the GPU and the call can be
+ * captured in a CUDA graph; otherwise one synchronisation.
+ * errors (OB_INVALID_ARGUMENT, checked in this order, before the 20-row rule):
+ * "max_corr_dist must be finite and greater than zero", "max_normal_angle_deg must be finite and in [0, 180]",
+ * "source_points and source_normals must have the same number of rows",
+ * "target_points and target_normals must have the same number of rows"; then OB_NO_DEVICE without a GPU. */
+typedef struct ob_cloud_align_io {
+    int32_t mode; /* ob_align_mode */
+    ob_point_rows source;
+    ob_point_rows target;
+    const void* source_normals;
+    size_t source_normal_rows;
+    const void* target_normals;
+    size_t target_normal_rows;
+    const double* initial_guess;
+    double max_corr_dist;        /* reference default 0.25 */
+    double max_normal_angle_deg; /* POINT_TO_PLANE; reference default 20 */
+    double* pose;
+    int32_t* iterations;
+} ob_cloud_align_io;
+ob_status ob_cloud_align(const ob_cloud_align_io* io, ob_stream* s);
+
+/* replaces SpatialHashGrid3D(target[, target_normals], cell_size).nearest(target, query, max_dist_sq), one query
+ *          per row   align_clouds.cpp:170-235
+ * Cells are floor(p / cell_size) in int64 (NaN and out-of-range: INT64_MIN, as on x86); target rows that are not
+ * finite (or, with target_normals, whose normal is not finite or has norm <= 1e-12) are left out.  The 27 cells in
+ * dx, dy, dz order, a cell's rows in ascending index, the first strictly smaller squared distance below
+ * max_dist_sq kept.  indices: one int32 per query row, -1 for none (and for a non-finite query).  target and
+ * queries share a dtype; target_normals has target's. */
+typedef struct ob_cloud_nearest_io {
+    ob_point_rows target;
+    const void* target_normals; /* optional */
+    ob_point_rows queries;
+    double cell_size;
+    double max_dist_sq;
+    int32_t* indices;
+} ob_cloud_nearest_io;
+ob_status ob_cloud_nearest(const ob_cloud_nearest_io* io, ob_stream* s);
 
 /* ---- fused range -> (XYZ, destaggered range, destaggered XYZ), batched over frames ----
  * One launch performs, for every frame f and return r of the batch, what the reference does as

@@ -79,6 +79,21 @@ class IcpSystemIO(C.Structure):
                 ("kernel_scale", C.c_double), ("jtj", vp), ("jtr", vp)]
 
 
+OB_ALIGN_POINT_TO_POINT, OB_ALIGN_POINT_TO_PLANE = range(2)
+
+
+class CloudAlignIO(C.Structure):
+    _fields_ = [("mode", C.c_int32), ("source", PointRows), ("target", PointRows), ("source_normals", vp),
+                ("source_normal_rows", sz), ("target_normals", vp), ("target_normal_rows", sz),
+                ("initial_guess", vp), ("max_corr_dist", C.c_double), ("max_normal_angle_deg", C.c_double),
+                ("pose", vp), ("iterations", vp)]
+
+
+class CloudNearestIO(C.Structure):
+    _fields_ = [("target", PointRows), ("target_normals", vp), ("queries", PointRows), ("cell_size", C.c_double),
+                ("max_dist_sq", C.c_double), ("indices", vp)]
+
+
 class DewarpFramesIO(C.Structure):
     _fields_ = [("lut", vp), ("range", vp), ("poses", vp), ("status", vp), ("timestamps", vp)]
 
@@ -169,6 +184,8 @@ _sig("ob_voxel_map_size", i32, vp, C.POINTER(sz), C.POINTER(sz), vp)
 _sig("ob_voxel_map_closest_neighbors", i32, vp, C.POINTER(VoxelQueryIO), vp)
 _sig("ob_icp_align", i32, vp, C.POINTER(IcpIO), vp)
 _sig("ob_icp_linear_system", i32, C.POINTER(IcpSystemIO), vp)
+_sig("ob_cloud_align", i32, C.POINTER(CloudAlignIO), vp)
+_sig("ob_cloud_nearest", i32, C.POINTER(CloudNearestIO), vp)
 _sig("ob_dewarp_frames", i32, C.POINTER(DewarpFramesIO), sz, C.c_double, C.c_double, vp, sz, vp, vp, vp,
      C.POINTER(sz), C.POINTER(sz), vp)
 if hasattr(lib, "ob_decoder_create"):

@@ -8,6 +8,8 @@ in place (zero copy), host arrays are staged by the C library.
 """
 import ctypes as C
 
+import math
+
 import numpy as np
 
 from . import _capi
@@ -706,6 +708,122 @@ def icp_align(voxel_map, source, max_distance, kernel_scale, max_num_iterations=
     io.pose, io.iterations = pose.ctypes.data, C.addressof(it)
     check(lib.ob_icp_align(voxel_map._h, C.byref(io), _stream(stream, voxel_map.device).h))
     return pose, it.value
+
+
+def _align_arrays(points, normals, n, what):
+    """(PointRows, kept points, kept normals or None) with the normals converted to the points' dtype and memory."""
+    r, keep = _point_rows(points, n, f"{what} expects an Nx3 array")
+    if normals is None:
+        return r, keep, None
+    if _is_torch(keep):
+        import torch
+        nk = torch.as_tensor(normals, device=keep.device).to(keep.dtype).contiguous()
+    else:
+        if _is_torch(normals):
+            normals = normals.cpu().numpy()
+        nk = np.ascontiguousarray(normals, keep.dtype)
+    if len(nk.shape) != 2 or nk.shape[1] != 3:
+        raise ValueError(f"{what} normals must be Nx3")
+    return r, keep, nk
+
+
+def cloud_align(source, target, source_normals=None, target_normals=None, initial_guess=None, max_corr_dist=0.25,
+                max_normal_angle_deg=20.0, n_source=None, n_target=None, stream=None):
+    """point_to_point_align (no normals) or point_to_plane_align (both normals) on the GPU (ob_cloud_align):
+    (pose [4, 4] float64, iterations that reached the solve).  CUDA-tensor clouds give CUDA tensors (pose float64
+    [4, 4], iterations int32 [1]) and nothing waits for the GPU; n_source / n_target: optional device-resident row
+    counts (e.g. voxel_downsample's count), the arrays then holding `capacity` rows.  initial_guess may be a
+    CUDA tensor."""
+    from ._capi import CloudAlignIO
+    plane = source_normals is not None or target_normals is not None
+    if plane and (source_normals is None or target_normals is None):
+        raise ValueError("point-to-plane alignment needs both source_normals and target_normals")
+    sr, s, sn = _align_arrays(source, source_normals, n_source, "source_points")
+    tr, t, tn = _align_arrays(target, target_normals, n_target, "target_points")
+    if _is_torch(s) != _is_torch(t) or (_is_torch(s) and s.device != t.device):
+        raise ValueError("source and target must live in the same memory")
+    if s.dtype != t.dtype:  # the C ABI takes one dtype for both clouds
+        if _is_torch(s):
+            s, t = s.double(), t.double()
+            sn, tn = (None if sn is None else sn.double()), (None if tn is None else tn.double())
+        else:
+            s, t = s.astype(np.float64), t.astype(np.float64)
+            sn, tn = (None if sn is None else sn.astype(np.float64)), (None if tn is None else tn.astype(np.float64))
+        sr.dtype = tr.dtype = _capi.OB_F64
+        sr.points, tr.points = _ptr(s), _ptr(t)
+    # ob_cloud_align checks these too; here they also hold on a machine without a GPU (no stream to create yet)
+    if not math.isfinite(float(max_corr_dist)) or float(max_corr_dist) <= 0.0:
+        raise ValueError("max_corr_dist must be finite and greater than zero")
+    if plane:
+        a = float(max_normal_angle_deg)
+        if not math.isfinite(a) or a < 0.0 or a > 180.0:
+            raise ValueError("max_normal_angle_deg must be finite and in [0, 180]")
+        if int(sn.shape[0]) != int(s.shape[0]):
+            raise ValueError("source_points and source_normals must have the same number of rows")
+        if int(tn.shape[0]) != int(t.shape[0]):
+            raise ValueError("target_points and target_normals must have the same number of rows")
+    io = CloudAlignIO()
+    io.mode = _capi.OB_ALIGN_POINT_TO_PLANE if plane else _capi.OB_ALIGN_POINT_TO_POINT
+    io.source, io.target = sr, tr
+    if plane:
+        io.source_normals, io.source_normal_rows = _ptr(sn), int(sn.shape[0])
+        io.target_normals, io.target_normal_rows = _ptr(tn), int(tn.shape[0])
+    g = None
+    if initial_guess is not None:
+        if _is_torch(initial_guess):
+            g = initial_guess.double().contiguous()
+        else:
+            g = np.ascontiguousarray(initial_guess, np.float64)
+        if _numel(g) != 16:
+            raise ValueError("initial_guess must be 4x4")
+        io.initial_guess = _ptr(g)
+    io.max_corr_dist, io.max_normal_angle_deg = float(max_corr_dist), float(max_normal_angle_deg)
+    if _is_torch(s) and s.is_cuda:
+        import torch
+        pose = torch.empty((4, 4), dtype=torch.float64, device=s.device)
+        it = torch.empty(1, dtype=torch.int32, device=s.device)
+        io.pose, io.iterations = pose.data_ptr(), it.data_ptr()
+        st = _torch_stream(s, stream)
+        check(lib.ob_cloud_align(C.byref(io), st.h))
+        return pose, it
+    pose = np.empty((4, 4), np.float64)
+    it = C.c_int32(0)
+    io.pose, io.iterations = pose.ctypes.data, C.addressof(it)
+    check(lib.ob_cloud_align(C.byref(io), _stream(stream, 0).h))
+    return pose, it.value
+
+
+def cloud_nearest(target, queries, cell_size, max_dist_sq, target_normals=None, n_target=None, n_queries=None,
+                  stream=None):
+    """SpatialHashGrid3D(target[, target_normals], cell_size).nearest(target, q, max_dist_sq) for every query row
+    (ob_cloud_nearest): int32 row indices into target, -1 for none.  A CUDA-tensor target and queries give a CUDA
+    tensor and nothing waits for the GPU; numpy in, numpy out."""
+    from ._capi import CloudNearestIO
+    tr, t, tn = _align_arrays(target, target_normals, n_target, "target_points")
+    qr, q = _point_rows(queries, n_queries, "queries expects an Nx3 array")
+    if _is_torch(t) != _is_torch(q) or (_is_torch(t) and t.device != q.device):
+        raise ValueError("target and queries must live in the same memory")
+    if t.dtype != q.dtype:
+        t, q = (t.double(), q.double()) if _is_torch(t) else (t.astype(np.float64), q.astype(np.float64))
+        tn = None if tn is None else (tn.double() if _is_torch(tn) else tn.astype(np.float64))
+        tr.dtype = qr.dtype = _capi.OB_F64
+        tr.points, qr.points = _ptr(t), _ptr(q)
+    rows = int(q.shape[0])
+    io = CloudNearestIO()
+    io.target, io.queries = tr, qr
+    io.target_normals = None if tn is None else _ptr(tn)
+    io.cell_size, io.max_dist_sq = float(cell_size), float(max_dist_sq)
+    if _is_torch(q) and q.is_cuda:
+        import torch
+        out = torch.full((rows,), -1, dtype=torch.int32, device=q.device)
+        io.indices = out.data_ptr()
+        st = _torch_stream(q, stream)
+        check(lib.ob_cloud_nearest(C.byref(io), st.h))
+        return out
+    out = np.full(rows, -1, np.int32)
+    io.indices = _ptr(out)
+    check(lib.ob_cloud_nearest(C.byref(io), _stream(stream, 0).h))
+    return out
 
 
 def icp_linear_system(source, target, kernel_scale, stream=None, device=0):

@@ -18,7 +18,7 @@ static std::atomic<uint64_t> g_launches{0};
 
 static std::atomic<uint64_t> g_family[OB_FAM_COUNT];
 static const char* const kFamilies[OB_FAM_COUNT] = {"decode_pipe", "decode", "cloud", "normals", "voxel",
-                                                    "voxel_map", "icp"};
+                                                    "voxel_map", "icp", "align"};
 
 void count_launch(uint64_t n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 void count_launch_of(int family, uint64_t n) {
@@ -330,6 +330,8 @@ size_t ob_abi_sizeof(const char* name) {
     if (n == "ob_voxel_query_io") return sizeof(ob_voxel_query_io);
     if (n == "ob_icp_io") return sizeof(ob_icp_io);
     if (n == "ob_icp_system_io") return sizeof(ob_icp_system_io);
+    if (n == "ob_cloud_align_io") return sizeof(ob_cloud_align_io);
+    if (n == "ob_cloud_nearest_io") return sizeof(ob_cloud_nearest_io);
     return 0;
 }
 

@@ -1,0 +1,62 @@
+// ob_rows.cuh -- point rows of the C ABI (ob_point_rows) as the device sees them, shared by the voxel map / ICP
+// (ob_voxel_map.cu) and cloud-to-cloud ICP (ob_align.cu): a host row count or a device word clamped to the
+// capacity, float32 or float64 rows widened to double on load, and the host-side check and staging.
+#pragma once
+#include <cstdint>
+
+#include "ob_api_common.h"
+
+namespace ob {
+namespace {
+
+// rows of an input: n on the host, or a device word clamped to the capacity
+struct Rows {
+    const void* p;
+    const unsigned long long* n_dev;
+    unsigned long long n_host;
+    unsigned cap;
+};
+__device__ __forceinline__ unsigned rows_n(const Rows& r) {
+    if (r.n_dev == nullptr) return static_cast<unsigned>(r.n_host);
+    const unsigned long long n = *r.n_dev;
+    return n < r.cap ? static_cast<unsigned>(n) : r.cap;
+}
+template <typename T>
+__device__ __forceinline__ void load3(const void* base, size_t row, double* v) {
+    const T* p = static_cast<const T*>(base) + row * 3;
+    v[0] = static_cast<double>(p[0]);
+    v[1] = static_cast<double>(p[1]);
+    v[2] = static_cast<double>(p[2]);
+}
+
+// ---- host side ----
+bool dtype_ok(int32_t d) { return d == OB_F32 || d == OB_F64; }
+
+// validate an ob_point_rows and stage it: host rows go through scratch; the row capacity is returned
+ob_status stage_rows(const ob_point_rows* in, Staging& stg, Rows* r, const char* what) {
+    if (!dtype_ok(in->dtype)) return fail(OB_INVALID_ARGUMENT, "unknown dtype");
+    const bool dev_n = in->n_device != nullptr;
+    const size_t cap = dev_n ? in->capacity : in->n;
+    if (cap > 0x7fffffffu) return fail(OB_INVALID_ARGUMENT, "too many points in one call");
+    if (dev_n && !is_device_ptr(in->n_device)) return fail(OB_INVALID_ARGUMENT, "n_device must be device memory");
+    if (cap && !in->points) return fail(OB_INVALID_ARGUMENT, "null points buffer");
+    const void* d = nullptr;
+    cudaError_t e = stg.in(in->points, cap * 3 * (in->dtype == OB_F64 ? 8 : 4), &d);
+    if (e != cudaSuccess) return fail_cuda(e, what);
+    r->p = d;
+    r->n_dev = reinterpret_cast<const unsigned long long*>(in->n_device);
+    r->n_host = in->n;
+    r->cap = static_cast<unsigned>(cap);
+    return OB_OK;
+}
+
+template <typename P>
+cudaError_t scratch(Staging& stg, size_t bytes, P** p) {
+    void* d = nullptr;
+    cudaError_t e = stg.scratch(bytes, &d);
+    *p = static_cast<P*>(d);
+    return e;
+}
+
+}  // namespace
+}  // namespace ob

@@ -38,6 +38,8 @@
 #include <type_traits>
 
 #include "ob_api_common.h"
+#include "ob_ldlt.cuh"
+#include "ob_rows.cuh"
 #include "ob_voxel_common.cuh"
 
 struct ob_voxel_map {
@@ -125,26 +127,6 @@ __device__ int find_or_claim(const Table& t, int32_t x, int32_t y, int32_t z, un
     }
     atomicAdd(ctr + C_FULL, 1ull);  // cannot happen while the host keeps the load at or below one half
     return -1;
-}
-
-// rows of an input: n on the host, or a device word clamped to the capacity
-struct Rows {
-    const void* p;
-    const unsigned long long* n_dev;
-    unsigned long long n_host;
-    unsigned cap;
-};
-__device__ __forceinline__ unsigned rows_n(const Rows& r) {
-    if (r.n_dev == nullptr) return static_cast<unsigned>(r.n_host);
-    const unsigned long long n = *r.n_dev;
-    return n < r.cap ? static_cast<unsigned>(n) : r.cap;
-}
-template <typename T>
-__device__ __forceinline__ void load3(const void* base, size_t row, double* v) {
-    const T* p = static_cast<const T*>(base) + row * 3;
-    v[0] = static_cast<double>(p[0]);
-    v[1] = static_cast<double>(p[1]);
-    v[2] = static_cast<double>(p[2]);
 }
 
 // ---- add_points ----
@@ -449,88 +431,6 @@ __device__ void unpack_system(const double* v, double* jtj, double* jtr) {
     for (int j = 0; j < 6; ++j) jtr[j] = v[15 + j];
 }
 
-// ---- Eigen LDLT (ldlt_inplace<Lower>::unblocked) and LDLT::_solve_impl, inner products in index order ----
-__device__ void ldlt_solve6(const double* A, const double* rhs, double* x) {
-    double m[6][6];
-    int tr[6];
-    for (int i = 0; i < 6; ++i)
-        for (int j = 0; j < 6; ++j) m[i][j] = j <= i ? A[i * 6 + j] : 0.0;
-    bool zero_diag = false;
-    for (int k = 0; k < 6 && !zero_diag; ++k) {
-        int big = k;
-        double bv = fabs(m[k][k]);
-        for (int i = k + 1; i < 6; ++i)
-            if (fabs(m[i][i]) > bv) {
-                bv = fabs(m[i][i]);
-                big = i;
-            }
-        tr[k] = big;
-        if (k != big) {
-            for (int j = 0; j < k; ++j) {
-                const double s = m[k][j];
-                m[k][j] = m[big][j];
-                m[big][j] = s;
-            }
-            for (int i = big + 1; i < 6; ++i) {
-                const double s = m[i][k];
-                m[i][k] = m[i][big];
-                m[i][big] = s;
-            }
-            const double s = m[k][k];
-            m[k][k] = m[big][big];
-            m[big][big] = s;
-            for (int i = k + 1; i < big; ++i) {
-                const double u = m[i][k];
-                m[i][k] = m[big][i];
-                m[big][i] = u;
-            }
-        }
-        if (k > 0) {
-            double temp[6];
-            for (int j = 0; j < k; ++j) temp[j] = mul(m[j][j], m[k][j]);
-            double dot = mul(m[k][0], temp[0]);
-            for (int j = 1; j < k; ++j) dot = add(dot, mul(m[k][j], temp[j]));
-            m[k][k] = sub(m[k][k], dot);
-            for (int i = k + 1; i < 6; ++i) {
-                double s = mul(m[i][0], temp[0]);
-                for (int j = 1; j < k; ++j) s = add(s, mul(m[i][j], temp[j]));
-                m[i][k] = sub(m[i][k], s);
-            }
-        }
-        const double akk = m[k][k];
-        const bool valid = fabs(akk) > 0.0;
-        if (k == 0 && !valid) {  // the whole diagonal is zero
-            for (int j = 0; j < 6; ++j) {
-                tr[j] = j;
-                for (int i = j + 1; i < 6; ++i) m[i][j] = 0.0;
-            }
-            zero_diag = true;
-            break;
-        }
-        if (valid)
-            for (int i = k + 1; i < 6; ++i) m[i][k] = m[i][k] / akk;
-    }
-    for (int i = 0; i < 6; ++i) x[i] = rhs[i];
-    for (int k = 0; k < 6; ++k) {
-        const double s = x[k];
-        x[k] = x[tr[k]];
-        x[tr[k]] = s;
-    }
-    for (int j = 0; j < 6; ++j)
-        for (int i = j + 1; i < 6; ++i) x[i] = sub(x[i], mul(x[j], m[i][j]));
-    for (int i = 0; i < 6; ++i) x[i] = fabs(m[i][i]) > DBL_MIN ? x[i] / m[i][i] : 0.0;
-    for (int i = 4; i >= 0; --i) {
-        double s = mul(m[i + 1][i], x[i + 1]);
-        for (int j = i + 2; j < 6; ++j) s = add(s, mul(m[j][i], x[j]));
-        x[i] = sub(x[i], s);
-    }
-    for (int k = 5; k >= 0; --k) {
-        const double s = x[k];
-        x[k] = x[tr[k]];
-        x[tr[k]] = s;
-    }
-}
-
 // ---- Sophus (quaternion x, y, z, w; translation) ----
 struct SE3 {
     double q[4];  // x, y, z, w
@@ -756,34 +656,6 @@ __global__ void __launch_bounds__(kTreeThreads, 1) icp_system_kernel(const unsig
 using namespace ob;
 
 namespace {
-
-bool dtype_ok(int32_t d) { return d == OB_F32 || d == OB_F64; }
-
-// validate an ob_point_rows and stage it: host rows go through scratch; the row capacity is returned
-ob_status stage_rows(const ob_point_rows* in, Staging& stg, Rows* r, const char* what) {
-    if (!dtype_ok(in->dtype)) return fail(OB_INVALID_ARGUMENT, "unknown dtype");
-    const bool dev_n = in->n_device != nullptr;
-    const size_t cap = dev_n ? in->capacity : in->n;
-    if (cap > 0x7fffffffu) return fail(OB_INVALID_ARGUMENT, "too many points in one call");
-    if (dev_n && !is_device_ptr(in->n_device)) return fail(OB_INVALID_ARGUMENT, "n_device must be device memory");
-    if (cap && !in->points) return fail(OB_INVALID_ARGUMENT, "null points buffer");
-    const void* d = nullptr;
-    cudaError_t e = stg.in(in->points, cap * 3 * (in->dtype == OB_F64 ? 8 : 4), &d);
-    if (e != cudaSuccess) return fail_cuda(e, what);
-    r->p = d;
-    r->n_dev = reinterpret_cast<const unsigned long long*>(in->n_device);
-    r->n_host = in->n;
-    r->cap = static_cast<unsigned>(cap);
-    return OB_OK;
-}
-
-template <typename P>
-cudaError_t scratch(Staging& stg, size_t bytes, P** p) {
-    void* d = nullptr;
-    cudaError_t e = stg.scratch(bytes, &d);
-    *p = static_cast<P*>(d);
-    return e;
-}
 
 void free_table(ob_voxel_map* m) {
     cudaFree(m->key);

@@ -474,3 +474,29 @@ class AdaptiveThreshold:
 
     def compute_threshold(self):
         return float(np.sqrt(self.model_sse / self.num_samples))
+
+
+# ---- cloud-to-cloud ICP (DESIGN f-7) ------------------------------------------------------------------
+# ouster.sdk.algorithm.point_to_point_align / point_to_plane_align (python/src/cpp/_algorithm.cpp:158-245): numpy in,
+# a (4, 4) float64 numpy array out, as in the reference; CUDA tensors in give a CUDA tensor out with no host wait.
+
+def point_to_point_align(source_points, target_points, initial_guess=None, max_corr_dist=0.25):
+    """source_to_target_transform by point-to-point ICP with MAD-scaled Huber weights (at most 10 iterations);
+    initial_guess (identity when None) comes back when fewer than 20 usable points or correspondences exist."""
+    pose, _ = _c.cloud_align(_rows3(source_points, "source_points must be Nx3"),
+                             _rows3(target_points, "target_points must be Nx3"),
+                             initial_guess=initial_guess, max_corr_dist=max_corr_dist)
+    return pose
+
+
+def point_to_plane_align(source_points, target_points, source_normals, target_normals, initial_guess=None,
+                         max_corr_dist=0.25, max_normal_angle_deg=20.0):
+    """source_to_target_transform by point-to-plane ICP: correspondences whose normals differ by more than
+    max_normal_angle_deg are rejected, non-finite points and normals are ignored, normals are normalised."""
+    pose, _ = _c.cloud_align(_rows3(source_points, "source_points must be Nx3"),
+                             _rows3(target_points, "target_points must be Nx3"),
+                             _rows3(source_normals, "source_normals must be Nx3"),
+                             _rows3(target_normals, "target_normals must be Nx3"),
+                             initial_guess=initial_guess, max_corr_dist=max_corr_dist,
+                             max_normal_angle_deg=max_normal_angle_deg)
+    return pose

@@ -299,4 +299,23 @@ vp, vit = ob.icp_align(gm, om.point_cloud() + 0.02, 1.0, 0.5, 10)
 wp, wit = oi.align_points_to_map(om.point_cloud() + 0.02, om, 1.0, 0.5, 10)
 assert vit == wit and np.abs(vp - wp).max() <= 1e-12
 print("voxel map / icp ok")
+# cloud-to-cloud ICP: nearest with NaN / 1e300 rows and bad normals, both aligns (f32 and f64)
+from oracle import align as oa
+rs = np.random.default_rng(12)
+ct = np.round(rs.uniform(-2, 2, (800, 3)) / 0.1) * 0.1
+ct[:5, 0] = [np.nan, np.inf, 1e300, -1e300, np.nan]
+cn = rs.normal(size=ct.shape)
+cn[5:15] = 0.0
+cq = np.round(rs.uniform(-2, 2, (700, 3)) / 0.1) * 0.1
+assert np.array_equal(ob.cloud_nearest(ct, cq, 0.3, 0.09, target_normals=cn), oa.cloud_nearest(ct, cq, 0.3, 0.09, cn))
+cs = ct[5:] @ np.array([[1, -0.01, 0], [0.01, 1, 0], [0, 0, 1]]).T + [0.02, -0.01, 0.0]
+for dt in (np.float64, np.float32):
+    a, b, sn, tn = cs.astype(dt), ct[5:].astype(dt), cn[5:].astype(dt), cn[5:].astype(dt)
+    gp, git = ob.cloud_align(a, b, max_corr_dist=0.5)
+    wp, wit = oa.point_to_point_align(a, b, None, 0.5)
+    assert git == wit and np.abs(gp - wp).max() <= 1e-12
+    gp, git = ob.cloud_align(a, b, sn, tn, max_corr_dist=0.5, max_normal_angle_deg=180.0)
+    wp, wit = oa.point_to_plane_align(a, b, sn, tn, None, 0.5, 180.0)
+    assert git == wit and np.abs(gp - wp).max() <= 1e-12
+print("cloud align ok")
 print("SANITIZE CASES OK")
