@@ -52,7 +52,7 @@ int ob_abi_version(void);
 /* sizeof() of a public struct by name ("ob_cloud_io", "ob_field_desc", "ob_packet_layout",
  * "ob_decode_io", "ob_decode_batch", "ob_dewarp_frame_io", "ob_normals_io", "ob_encode_io", "ob_dewarp_frames_io",
  * "ob_voxel_io", "ob_point_rows", "ob_voxel_map_cull_io", "ob_voxel_query_io", "ob_icp_io", "ob_icp_system_io",
- * "ob_cloud_align_io", "ob_cloud_nearest_io");
+ * "ob_cloud_align_io", "ob_cloud_nearest_io", "ob_zone_desc", "ob_zone_render_io", "ob_zone_live", "ob_zone_state");
  * 0 for unknown names.  Lets FFI bindings verify their layout. */
 size_t ob_abi_sizeof(const char* struct_name);
 const char* ob_last_error(void);
@@ -61,7 +61,7 @@ int ob_device_count(void);
 /* kernels launched by this library since load (all threads); the bench's gpu_launches claim */
 uint64_t ob_kernel_launch_count(void);
 /* launches of one named kernel family since load: "decode_pipe" (pipelined K2), "decode" (K2, any
- * kernel), "cloud" (K1), "normals", "voxel", "voxel_map", "icp", "align"; 0 for unknown names.  Lets tests assert which code path ran. */
+ * kernel), "cloud" (K1), "normals", "voxel", "voxel_map", "icp", "align", "zone"; 0 for unknown names.  Lets tests assert which code path ran. */
 uint64_t ob_kernel_launch_count_of(const char* name);
 /* tuning hook (launch geometry and code-path selection only, never results): cloud_tw, cloud_stages,
  * cloud_threads (compute threads; a copy warp is added), cloud_ctas_per_sm, cloud_store_lag,
@@ -427,6 +427,93 @@ typedef struct ob_cloud_nearest_io {
     int32_t* indices;
 } ob_cloud_nearest_io;
 ob_status ob_cloud_nearest(const ob_cloud_nearest_io* io, ob_stream* s);
+
+/* ---- zone monitoring (DESIGN f-8) ---- */
+#define OB_ZONE_MAX_TRIANGLES 2048 /* Zone::MAX_TRIANGLES */
+#define OB_ZONE_MAX_LIVE 16        /* zone_common.py MAX_ACTIVE_ZONES */
+typedef enum ob_zone_frame { OB_ZONE_FRAME_NONE = 0, OB_ZONE_FRAME_BODY = 1, OB_ZONE_FRAME_SENSOR = 2 } ob_zone_frame;
+typedef enum ob_zone_mode { OB_ZONE_MODE_NONE = 0, OB_ZONE_MODE_OCCUPANCY = 1, OB_ZONE_MODE_VACANCY = 2 } ob_zone_mode;
+
+/* one zone of a render: its STL mesh and the Zone fields check_invariants reads */
+typedef struct ob_zone_desc {
+    const float* triangles; /* host, n_triangles x 9 floats: v0, v1, v2 of each triangle */
+    uint32_t n_triangles;
+    int32_t coordinate_frame; /* ob_zone_frame */
+    uint32_t point_count;
+    uint32_t frame_count;
+    int32_t mode; /* ob_zone_mode */
+} ob_zone_desc;
+
+/* replaces Zone::render(const BeamConfig&) for every zone of a set   ouster_core/src/zone.cpp:63-135, with
+ *          Mesh::closest_and_farthest_intersections (mesh.cpp:249-294), Triangle::intersect (triangle.cpp:19-50)
+ *          and the bounding sphere (mesh.cpp:41-60).  One launch covers every zone and pixel.
+ * body_* / sensor_*: the BeamConfig LUTs (n_rows * n_cols * 3 doubles each, host or device): make_xyz_lut with
+ * range unit 0.001 and scale_translation(sensor_to_body) * lidar_to_sensor, or lidar_to_sensor alone
+ * (beam_config.cpp:37-45).  body_* may be NULL when the set has no sensor_to_body_transform.
+ * near_mm / far_mm: n_zones x n_rows x n_cols uint32 out (host or device).  pixels_with_intersections: n_zones
+ * uint32 out (host); a zone with 0 is one Zone::render returns false for.  The call synchronises once.
+ * errors, zone by zone in order: the check_invariants texts (OB_INVALID_ARGUMENT) "Zone: point_count must be in
+ * [1, 262143]", "Zone: frame_count must be in [1, 65535]", "Zone: mode must be OCCUPANCY or VACANCY",
+ * "Zone: STL coordinate frame must be BODY or SENSOR"; the cases Zone::render reports on stderr
+ * (OB_INVALID_ARGUMENT) "Zone: Error rendering zone, STL has no triangles.", "Zone: Error rendering zone, STL has
+ * too many triangles.", "Zone: Error rendering zone, sensor_to_body_transform not set for BODY coordinate frame.";
+ * after the launch (OB_RUNTIME_ERROR) "Zone::render: range overflow" and "Zone: area of rendered zone (N) is
+ * smaller than point_count (M) specified in zone." */
+typedef struct ob_zone_render_io {
+    uint32_t n_rows, n_cols;
+    const double* body_direction;
+    const double* body_offset;
+    const double* sensor_direction;
+    const double* sensor_offset;
+    const ob_zone_desc* zones;
+    uint32_t n_zones;
+    uint32_t* near_mm;
+    uint32_t* far_mm;
+    uint32_t* pixels_with_intersections;
+} ob_zone_render_io;
+ob_status ob_zone_render(const ob_zone_render_io* io, ob_stream* s);
+
+/* one live zone of a monitor (slot = its index in power_on_live_ids, the bit it sets in the bitmask) */
+typedef struct ob_zone_live {
+    uint32_t id; /* ZoneState::id */
+    int32_t mode; /* ob_zone_mode; ZoneState::trigger_type */
+    uint32_t point_count;
+    uint32_t frame_count;
+    const uint32_t* near_mm; /* n_rows x n_cols, host or device; copied by ob_zone_monitor_create */
+    const uint32_t* far_mm;
+    uint32_t triggers; /* initial trigger and alert counters (0 for a new monitor) */
+    uint32_t alerts;
+} ob_zone_live;
+
+#pragma pack(push, 1)
+/* ZoneState (ouster_core/include/ouster/core/zone_state.h), 37 bytes */
+typedef struct ob_zone_state {
+    uint8_t live, id, error_flags, trigger_type, trigger_status;
+    uint32_t triggered_frames, count, occlusion_count, invalid_count, max_count;
+    uint32_t min_range, max_range, mean_range;
+} ob_zone_state;
+#pragma pack(pop)
+
+typedef struct ob_zone_monitor ob_zone_monitor;
+/* replaces EmulatedZoneMon (python/src/ouster/sdk/core/zone_common.py) with its zone images in device memory.
+ * max_count = #(near < far) per zone is counted on the device here.  error: "at most 16 live zones" */
+ob_status ob_zone_monitor_create(int device, uint32_t n_rows, uint32_t n_cols, const ob_zone_live* live,
+                                 uint32_t n_live, ob_zone_monitor** out);
+/* EmulatedZoneMon::calc_triggers(range, bitmask): range n_rows x n_cols uint32 (host or device, e.g. K2's RANGE);
+ * bitmask (optional, host or device) gets bit `slot` OR-ed where the zone triggers.  Per zone: count
+ * (r > 0 && near <= r <= far), occlusion (r > 0 && r <= near), invalid (r == 0 && near > 0), min / max / exact
+ * sum of the triggering ranges; then one thread runs the OCCUPANCY / VACANCY trigger and alert counters and
+ * writes the 16 ZoneState records (get_packet()) in device memory.  Device range and bitmask: nothing waits for
+ * the GPU and the call can be captured in a CUDA graph. */
+ob_status ob_zone_monitor_update(ob_zone_monitor* m, const uint32_t* range, uint32_t* bitmask, ob_stream* s);
+/* the 16 ob_zone_state records of the last update (id 255 for slots past n_live) into `out` (16 * 37 bytes, host
+ * or device; a host copy synchronises) */
+ob_status ob_zone_monitor_states(const ob_zone_monitor* m, void* out, ob_stream* s);
+/* per slot (host arrays of n_live, each optional): the trigger and alert counters, and the exact sum of the last
+ * update's triggering ranges (EmulatedZoneMon's float64 mean is range_sums / count); synchronises */
+ob_status ob_zone_monitor_counters(const ob_zone_monitor* m, uint32_t* triggers, uint32_t* alerts,
+                                   uint64_t* range_sums, ob_stream* s);
+ob_status ob_zone_monitor_destroy(ob_zone_monitor* m);
 
 /* ---- fused range -> (XYZ, destaggered range, destaggered XYZ), batched over frames ----
  * One launch performs, for every frame f and return r of the batch, what the reference does as

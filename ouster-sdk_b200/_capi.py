@@ -94,6 +94,35 @@ class CloudNearestIO(C.Structure):
                 ("max_dist_sq", C.c_double), ("indices", vp)]
 
 
+OB_ZONE_MAX_TRIANGLES, OB_ZONE_MAX_LIVE = 2048, 16
+OB_ZONE_FRAME_NONE, OB_ZONE_FRAME_BODY, OB_ZONE_FRAME_SENSOR = range(3)
+OB_ZONE_MODE_NONE, OB_ZONE_MODE_OCCUPANCY, OB_ZONE_MODE_VACANCY = range(3)
+
+
+class ZoneDesc(C.Structure):
+    _fields_ = [("triangles", vp), ("n_triangles", u32), ("coordinate_frame", C.c_int32), ("point_count", u32),
+                ("frame_count", u32), ("mode", C.c_int32)]
+
+
+class ZoneRenderIO(C.Structure):
+    _fields_ = [("n_rows", u32), ("n_cols", u32), ("body_direction", vp), ("body_offset", vp),
+                ("sensor_direction", vp), ("sensor_offset", vp), ("zones", C.POINTER(ZoneDesc)), ("n_zones", u32),
+                ("near_mm", vp), ("far_mm", vp), ("pixels_with_intersections", vp)]
+
+
+class ZoneLive(C.Structure):
+    _fields_ = [("id", u32), ("mode", C.c_int32), ("point_count", u32), ("frame_count", u32), ("near_mm", vp),
+                ("far_mm", vp), ("triggers", u32), ("alerts", u32)]
+
+
+class ZoneState(C.Structure):
+    _pack_ = 1
+    _fields_ = [("live", C.c_uint8), ("id", C.c_uint8), ("error_flags", C.c_uint8), ("trigger_type", C.c_uint8),
+                ("trigger_status", C.c_uint8), ("triggered_frames", u32), ("count", u32), ("occlusion_count", u32),
+                ("invalid_count", u32), ("max_count", u32), ("min_range", u32), ("max_range", u32),
+                ("mean_range", u32)]
+
+
 class DewarpFramesIO(C.Structure):
     _fields_ = [("lut", vp), ("range", vp), ("poses", vp), ("status", vp), ("timestamps", vp)]
 
@@ -186,6 +215,12 @@ _sig("ob_icp_align", i32, vp, C.POINTER(IcpIO), vp)
 _sig("ob_icp_linear_system", i32, C.POINTER(IcpSystemIO), vp)
 _sig("ob_cloud_align", i32, C.POINTER(CloudAlignIO), vp)
 _sig("ob_cloud_nearest", i32, C.POINTER(CloudNearestIO), vp)
+_sig("ob_zone_render", i32, C.POINTER(ZoneRenderIO), vp)
+_sig("ob_zone_monitor_create", i32, i32, u32, u32, C.POINTER(ZoneLive), u32, C.POINTER(vp))
+_sig("ob_zone_monitor_update", i32, vp, vp, vp, vp)
+_sig("ob_zone_monitor_states", i32, vp, vp, vp)
+_sig("ob_zone_monitor_counters", i32, vp, vp, vp, vp, vp)
+_sig("ob_zone_monitor_destroy", i32, vp)
 _sig("ob_dewarp_frames", i32, C.POINTER(DewarpFramesIO), sz, C.c_double, C.c_double, vp, sz, vp, vp, vp,
      C.POINTER(sz), C.POINTER(sz), vp)
 if hasattr(lib, "ob_decoder_create"):

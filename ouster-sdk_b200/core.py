@@ -1118,3 +1118,184 @@ class Decoder:
             except Exception:
                 pass
             self._h = None
+
+
+# ---- zone monitoring (DESIGN f-8) -------------------------------------------------------------------------------
+ZONE_STATE_DTYPE = np.dtype([("live", np.uint8), ("id", np.uint8), ("error_flags", np.uint8),
+                             ("trigger_type", np.uint8), ("trigger_status", np.uint8), ("triggered_frames", np.uint32),
+                             ("count", np.uint32), ("occlusion_count", np.uint32), ("invalid_count", np.uint32),
+                             ("max_count", np.uint32), ("min_range", np.uint32), ("max_range", np.uint32),
+                             ("mean_range", np.uint32)])  # ZoneState, packed: 37 bytes
+assert ZONE_STATE_DTYPE.itemsize == 37
+
+
+def _lut_pair(lut, npx, what):
+    """(direction, offset) pointers of a float64 LUT: an XYZLutT of dtype float64 (device tables) or a pair of
+    (h*w, 3) float64 arrays / CUDA tensors."""
+    if lut is None:
+        return None, None, ()
+    if isinstance(lut, XYZLutT):
+        if lut.dtype != np.float64 or lut.h * lut.w != npx:
+            raise ValueError(f"{what} must be a float64 LUT of the zone images' size")
+        d, o = C.c_void_p(), C.c_void_p()
+        check(lib.ob_lut_device_ptrs(lut._h, C.byref(d), C.byref(o)))
+        return d.value, o.value, (lut,)
+    d, o = lut
+    keep = []
+    for a in (d, o):
+        if _is_torch(a):
+            a = a.double().contiguous()
+        else:
+            a = np.ascontiguousarray(a, np.float64)
+        if _numel(a) != npx * 3:
+            raise ValueError(f"{what} must hold h*w*3 values")
+        keep.append(a)
+    return _ptr(keep[0]), _ptr(keep[1]), tuple(keep)
+
+
+def zone_render(zones, h, w, sensor_lut, body_lut=None, device_out=None, stream=None, device=0):
+    """Zone::render of every zone in one launch (ob_zone_render).
+
+    zones: sequence of dicts with `triangles` ([n, 9] or [n, 3, 3] float32: v0, v1, v2), `coordinate_frame`
+    (1 BODY, 2 SENSOR) and optional `point_count`, `frame_count`, `mode` (default 1, 1, 1 OCCUPANCY).
+    sensor_lut / body_lut: BeamConfig's LUTs without / with sensor_to_body (see _lut_pair).
+    -> (near_mm, far_mm [n_zones, h, w] uint32, pixels_with_intersections numpy uint32 [n_zones]).  The images are
+    CUDA int32 tensors (same bits) when device_out is True, or by default when a LUT lives on the GPU."""
+    from ._capi import ZoneDesc, ZoneRenderIO
+    zones = list(zones)
+    npx = int(h) * int(w)
+    sd, so, keep_s = _lut_pair(sensor_lut, npx, "sensor_lut")
+    bd, bo, keep_b = _lut_pair(body_lut, npx, "body_lut")
+    descs = (ZoneDesc * max(len(zones), 1))()
+    tris = []
+    for i, z in enumerate(zones):
+        t = np.ascontiguousarray(z["triangles"], np.float32).reshape(-1, 9)
+        tris.append(t)
+        descs[i].triangles, descs[i].n_triangles = t.ctypes.data, len(t)
+        descs[i].coordinate_frame = int(z["coordinate_frame"])
+        descs[i].point_count = int(z.get("point_count", 1))
+        descs[i].frame_count = int(z.get("frame_count", 1))
+        descs[i].mode = int(z.get("mode", _capi.OB_ZONE_MODE_OCCUPANCY))
+    on_dev = [a for a in keep_s + keep_b if (isinstance(a, XYZLutT) or (_is_torch(a) and a.is_cuda))]
+    if device_out is None:
+        device_out = bool(on_dev)
+    shape = (len(zones), int(h), int(w))
+    if device_out:
+        import torch
+        dev = on_dev[0].device if on_dev else device
+        dev = torch.device("cuda", dev) if isinstance(dev, int) else dev
+        near = torch.empty(shape, dtype=torch.int32, device=dev)
+        far = torch.empty(shape, dtype=torch.int32, device=dev)
+        st = stream or Stream(dev.index, cuda_stream=torch.cuda.current_stream(dev).cuda_stream)
+    else:
+        near, far = np.empty(shape, np.uint32), np.empty(shape, np.uint32)
+        st = _stream(stream, device)
+    px = np.zeros(max(len(zones), 1), np.uint32)
+    io = ZoneRenderIO()
+    io.n_rows, io.n_cols = int(h), int(w)
+    io.sensor_direction, io.sensor_offset, io.body_direction, io.body_offset = sd, so, bd, bo
+    io.zones, io.n_zones = descs, len(zones)
+    io.near_mm, io.far_mm, io.pixels_with_intersections = _ptr(near), _ptr(far), px.ctypes.data
+    check(lib.ob_zone_render(C.byref(io), st.h))
+    return near, far, px[:len(zones)]
+
+
+class ZoneMonitor:
+    """Device-resident EmulatedZoneMon (ob_zone_monitor): up to 16 live zones' near/far images in HBM; update()
+    runs _calc_counts and the trigger counters of one frame and leaves the 16 ZoneState records on the device.
+
+    live: sequence of dicts with `id`, `mode`, `point_count`, `frame_count`, `near_mm`, `far_mm` ((h, w) uint32,
+    numpy or CUDA) and optional initial `triggers` / `alerts`.  The slot of a zone (its bitmask bit) is its index."""
+
+    def __init__(self, live, h, w, device=0):
+        from ._capi import ZoneLive
+        live = list(live)
+        arr = (ZoneLive * max(len(live), 1))()
+        keep = []
+        for i, z in enumerate(live):
+            ims = []
+            for k in ("near_mm", "far_mm"):
+                a = z[k]
+                a = a.contiguous() if _is_torch(a) else np.ascontiguousarray(a, np.uint32)
+                if _numel(a) != int(h) * int(w):
+                    raise ValueError("zone images must be h x w")
+                ims.append(a)
+            keep += ims
+            arr[i].id, arr[i].mode = int(z["id"]), int(z["mode"])
+            arr[i].point_count, arr[i].frame_count = int(z["point_count"]), int(z["frame_count"])
+            arr[i].near_mm, arr[i].far_mm = _ptr(ims[0]), _ptr(ims[1])
+            arr[i].triggers, arr[i].alerts = int(z.get("triggers", 0)), int(z.get("alerts", 0))
+        hd = C.c_void_p()
+        check(lib.ob_zone_monitor_create(device, int(h), int(w), arr, len(live), C.byref(hd)))
+        self._h, self.h, self.w, self.n_live, self.device = hd, int(h), int(w), len(live), device
+        self._st = None
+        self._wrapped = None
+
+    def __del__(self):
+        if getattr(self, "_h", None) and lib is not None:
+            try:
+                lib.ob_zone_monitor_destroy(self._h)
+            except Exception:
+                pass
+            self._h = None
+
+    def _stream_for(self, x, stream):
+        if stream is not None:
+            return stream
+        if _is_torch(x) and x.is_cuda:
+            import torch
+            h = torch.cuda.current_stream(x.device).cuda_stream
+            if self._wrapped is None or self._wrapped[0] != h:  # one wrapper per torch stream, reused per frame
+                self._wrapped = (h, Stream(x.device.index, cuda_stream=h))
+            return self._wrapped[1]
+        return _stream(None, self.device)
+
+    def update(self, range_img, bitmask=None, stream=None):
+        """calc_triggers(range, bitmask): range (h, w) uint32 (numpy, or a CUDA int32 / uint32 tensor such as K2's
+        RANGE); bitmask (optional, same shape, uint32 / int32) gets bit `slot` OR-ed where a zone triggers.  CUDA
+        inputs: nothing waits for the GPU."""
+        if _numel(range_img) != self.h * self.w:
+            raise ValueError("range image must be h x w")
+        if _is_torch(range_img):
+            import torch
+            if range_img.dtype not in (torch.int32, torch.uint32):
+                raise ValueError("range must be uint32")
+            r = range_img.contiguous()
+        else:
+            r = np.ascontiguousarray(range_img, np.uint32)
+        if bitmask is not None:
+            # written in place, so neither a copy nor a conversion will do
+            if _is_torch(bitmask):
+                import torch
+                ok = bitmask.dtype in (torch.int32, torch.uint32) and bitmask.is_contiguous()
+            else:
+                ok = isinstance(bitmask, np.ndarray) and bitmask.dtype in (np.uint32, np.int32) and \
+                    bitmask.flags["C_CONTIGUOUS"]
+            if not ok or _numel(bitmask) != self.h * self.w:
+                raise ValueError("bitmask must be a contiguous h x w uint32 / int32 array")
+        st = self._stream_for(r, stream)
+        self._st = st
+        check(lib.ob_zone_monitor_update(self._h, _ptr(r), None if bitmask is None else _ptr(bitmask), st.h))
+
+    def states(self, device=False, stream=None):
+        """The 16 ZoneState records of the last update: numpy (ZONE_STATE_DTYPE) or, with device=True, a CUDA
+        uint8 tensor [16, 37] written on the stream without waiting."""
+        st = stream or self._st or _stream(None, self.device)
+        if device:
+            import torch
+            out = torch.empty((16, 37), dtype=torch.uint8, device=torch.device("cuda", st.device))
+            check(lib.ob_zone_monitor_states(self._h, out.data_ptr(), st.h))
+            return out
+        out = np.zeros(16, ZONE_STATE_DTYPE)
+        check(lib.ob_zone_monitor_states(self._h, out.ctypes.data, st.h))
+        return out
+
+    def counters(self, stream=None):
+        """(triggers, alerts, range_sums): per-slot lists of the trigger and alert counters and of the exact sum of
+        the last update's triggering ranges; waits for the stream."""
+        n = max(self.n_live, 1)
+        t, a, r = np.zeros(n, np.uint32), np.zeros(n, np.uint32), np.zeros(n, np.uint64)
+        st = stream or self._st or _stream(None, self.device)
+        check(lib.ob_zone_monitor_counters(self._h, t.ctypes.data, a.ctypes.data, r.ctypes.data, st.h))
+        return ([int(v) for v in t[:self.n_live]], [int(v) for v in a[:self.n_live]],
+                [int(v) for v in r[:self.n_live]])

@@ -18,7 +18,7 @@ static std::atomic<uint64_t> g_launches{0};
 
 static std::atomic<uint64_t> g_family[OB_FAM_COUNT];
 static const char* const kFamilies[OB_FAM_COUNT] = {"decode_pipe", "decode", "cloud", "normals", "voxel",
-                                                    "voxel_map", "icp", "align"};
+                                                    "voxel_map", "icp", "align", "zone"};
 
 void count_launch(uint64_t n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 void count_launch_of(int family, uint64_t n) {
@@ -332,6 +332,10 @@ size_t ob_abi_sizeof(const char* name) {
     if (n == "ob_icp_system_io") return sizeof(ob_icp_system_io);
     if (n == "ob_cloud_align_io") return sizeof(ob_cloud_align_io);
     if (n == "ob_cloud_nearest_io") return sizeof(ob_cloud_nearest_io);
+    if (n == "ob_zone_desc") return sizeof(ob_zone_desc);
+    if (n == "ob_zone_render_io") return sizeof(ob_zone_render_io);
+    if (n == "ob_zone_live") return sizeof(ob_zone_live);
+    if (n == "ob_zone_state") return sizeof(ob_zone_state);
     return 0;
 }
 

@@ -500,3 +500,433 @@ def point_to_plane_align(source_points, target_points, source_normals, target_no
                              initial_guess=initial_guess, max_corr_dist=max_corr_dist,
                              max_normal_angle_deg=max_normal_angle_deg)
     return pose
+
+
+# ---- zone monitoring (DESIGN f-8) -----------------------------------------------------------------------------
+# ouster.sdk.core's Mesh / Stl / Zone / ZoneSet / Zrb (python/src/cpp/client/zone_monitor.cpp) and EmulatedZoneMon
+# (python/src/ouster/sdk/core/zone_common.py).  Rendering and the per-frame occupancy run on the GPU; STL parsing
+# is host code.  ZRB / ZoneSet files, hashes and JSON are not provided (DESIGN 9).
+import re as _re  # noqa: E402
+from fractions import Fraction as _Fraction  # noqa: E402
+import struct as _struct  # noqa: E402
+import sys as _sys  # noqa: E402
+
+MAX_ACTIVE_ZONES = 16
+MAX_AVAILABLE_ZONES = 128
+
+
+class CoordinateFrame(enum.IntEnum):
+    NONE = 0
+    BODY = 1
+    SENSOR = 2
+
+
+class ZoneMode(enum.IntEnum):
+    NONE = 0
+    OCCUPANCY = 1
+    VACANCY = 2
+
+
+_STL_HEADER_BYTES = 80
+_NUM = rb"(-?[0-9\.]+(?:[eE][+-]\d+)?)"
+_VERTEX_RE = _re.compile(rb"^\s*vertex\s+" + _NUM + rb"\s+" + _NUM + rb"\s+" + _NUM, _re.ASCII)
+_STOF_RE = _re.compile(rb"[+-]?(?:\d+\.?\d*|\.\d+)(?:[eE][+-]?\d+)?", _re.ASCII)
+
+
+def _stl_error(message, line=b""):
+    """mesh.cpp:86-92"""
+    msg = "STL Parsing Error: " + message
+    if line:
+        msg += ": '" + line.decode("latin-1") + "'"
+    print(msg, file=_sys.stderr)
+
+
+_FLT_MIN = _Fraction(2) ** -126
+_FLT_INF_EDGE = _Fraction(2) ** 128 - _Fraction(2) ** 103  # halfway between FLT_MAX and 2^128
+
+
+def _stof(s):
+    """std::stof on a token the vertex regex accepted: strtof's longest numeric prefix, rounded once to the nearest
+    float (ties to even).  No prefix, or a result strtof flags with ERANGE (overflow, or a nonzero value that ends
+    up subnormal or zero), raises ValueError, where std::stof throws."""
+    m = _STOF_RE.match(s)
+    if not m:
+        raise ValueError("stof: no conversion")
+    q = _Fraction(m.group(0).decode())
+    if abs(q) >= _FLT_INF_EDGE:
+        raise ValueError("stof: out of range")
+    if q == 0:
+        return np.float32(-0.0) if m.group(0)[:1] == b"-" else np.float32(0.0)
+    # float(q) rounds once to double; rounding that to float can land one step off, so pick the nearest neighbour
+    f = np.float32(float(q))
+    with np.errstate(over="ignore"):
+        cands = [c for c in (np.nextafter(f, np.float32(-np.inf)), f, np.nextafter(f, np.float32(np.inf)))
+                 if np.isfinite(c)]
+    best = min(cands, key=lambda c: (abs(_Fraction(float(c)) - q), int(np.array(c).view(np.uint32)) & 1))
+    if abs(_Fraction(float(best))) < _FLT_MIN and _Fraction(float(best)) != q:
+        raise ValueError("stof: out of range")
+    return np.float32(best)
+
+
+def _ascii_lines(data):
+    """read_stl_ascii_line (mesh.cpp:73-84): trimmed of ' \\t\\r', blank and '#' lines skipped, lower-cased"""
+    for raw in data.split(b"\n"):
+        line = raw.strip(b" \t\r")
+        if not line or line[:1] == b"#":
+            continue
+        yield line.lower()
+
+
+def _load_stl_ascii(data):
+    """Mesh::load_from_stl_ascii, mesh.cpp:94-173: (n, 3, 3) float32 or None"""
+    lines = _ascii_lines(data)
+    line = next(lines, None)
+    if line is None or not _re.search(rb"^\s*solid\b", line):
+        _stl_error("Failed to find 'solid' header", line or b"")
+        return None
+    tris = []
+    for line in lines:
+        if _re.search(rb"^\s*facet\b", line):
+            line = next(lines, None)
+            if line is None or not _re.search(rb"^\s*outer\s+loop", line):
+                _stl_error("Expected 'outer loop'", line or b"")
+                return None
+            verts = []
+            for _ in range(3):
+                line = next(lines, None)
+                m = _VERTEX_RE.search(line) if line is not None else None
+                if m is None:
+                    _stl_error("Expected 'vertex'", line or b"")
+                    return None
+                verts.append([_stof(m.group(k)) for k in (1, 2, 3)])
+            for word in (b"endloop", b"endfacet"):
+                line = next(lines, None)
+                if line is None or not _re.search(rb"^\s*" + word, line):
+                    _stl_error(f"Expected '{word.decode()}'", line or b"")
+                    return None
+            tris.append(verts)
+        elif _re.search(rb"^\s*endsolid\b", line):
+            return np.array(tris, np.float32).reshape(-1, 3, 3)
+        else:
+            _stl_error("Unexpected line outside of a facet", line)
+            return None
+    _stl_error("File ended unexpectedly without 'endsolid'")
+    return None
+
+
+def _load_stl_binary(data):
+    """Mesh::load_from_stl_binary, mesh.cpp:175-207: 80-byte header, uint32 count, then 50-byte records (a
+    normal and three vertices, 12 floats, and a 2-byte attribute count that may be cut short at the end)"""
+    if len(data) < _STL_HEADER_BYTES:
+        _stl_error("File too short.")
+        return None
+    if len(data) < _STL_HEADER_BYTES + 4:
+        _stl_error("Unknown # of n_tris.")
+        return None
+    n = _struct.unpack_from("<I", data, _STL_HEADER_BYTES)[0]
+    if n and len(data) < 84 + 50 * (n - 1) + 48:
+        _stl_error("Mismatch in # of n_tris.")
+        return None
+    rec = np.dtype([("normal", "<f4", 3), ("v", "<f4", (3, 3)), ("attr", "<u2")])
+    full = min(n, (len(data) - 84) // 50)
+    tris = np.frombuffer(data, rec, full, 84)["v"] if full else np.zeros((0, 3, 3), np.float32)
+    if full < n:  # the last record without its attribute bytes
+        tail = np.frombuffer(data, "<f4", 12, 84 + 50 * full)[3:].reshape(1, 3, 3)
+        tris = np.concatenate([tris, tail])
+    return np.ascontiguousarray(tris, np.float32)
+
+
+def load_stl_triangles(data):
+    """Mesh::load_from_stl_bytes (mesh.cpp:209-241): ASCII when "endsolid" (any case) starts after the 80-byte
+    header, else binary.  -> (n, 3, 3) float32 vertices, or None where the reference returns false."""
+    pos = bytes(data).lower().find(b"endsolid")
+    if pos > _STL_HEADER_BYTES:
+        return _load_stl_ascii(bytes(data))
+    return _load_stl_binary(bytes(data))
+
+
+class Mesh:
+    """Mesh (mesh.h): the triangles of an STL as an (n, 3, 3) float32 array."""
+
+    def __init__(self, triangles=None):
+        self._t = np.zeros((0, 3, 3), np.float32) if triangles is None else \
+            np.ascontiguousarray(triangles, np.float32).reshape(-1, 3, 3)
+
+    @property
+    def triangles(self):
+        return self._t
+
+    def load_from_stl_bytes(self, data):
+        t = load_stl_triangles(data)
+        if t is None:
+            return False
+        self._t = t
+        return True
+
+    def load_from_stl(self, path):
+        with open(path, "rb") as f:
+            return self.load_from_stl_bytes(f.read())
+
+
+class Stl:
+    """Stl (stl.h): the file's bytes and the zone's coordinate frame."""
+
+    def __init__(self, path_or_bytes):
+        if isinstance(path_or_bytes, (bytes, bytearray)):
+            self.blob = bytes(path_or_bytes)
+        else:
+            with open(path_or_bytes, "rb") as f:
+                self.blob = f.read()
+        self.coordinate_frame = CoordinateFrame.NONE
+
+    def to_mesh(self):
+        m = Mesh()
+        if not m.load_from_stl_bytes(self.blob):
+            raise RuntimeError("Stl: failed to parse STL")
+        return m
+
+
+class Zrb:
+    """Zrb (zrb.h): near / far range images in mm and the transforms they were rendered with."""
+
+    def __init__(self, near_range_mm=None, far_range_mm=None, serial_number=0, beam_to_lidar_transform=None,
+                 lidar_to_sensor_transform=None, sensor_to_body_transform=None):
+        self.near_range_mm = np.zeros((0, 0), np.uint32) if near_range_mm is None else near_range_mm
+        self.far_range_mm = np.zeros((0, 0), np.uint32) if far_range_mm is None else far_range_mm
+        self.serial_number = serial_number
+        self.beam_to_lidar_transform = np.eye(4) if beam_to_lidar_transform is None else beam_to_lidar_transform
+        self.lidar_to_sensor_transform = np.eye(4) if lidar_to_sensor_transform is None else lidar_to_sensor_transform
+        self.sensor_to_body_transform = np.eye(4) if sensor_to_body_transform is None else sensor_to_body_transform
+        self.stl_hash = None
+
+
+def _sensor_value(info, key, default=None):
+    return info.get(key, default) if isinstance(info, dict) else getattr(info, key, default)
+
+
+class BeamConfig:
+    """BeamConfig (beam_config.cpp:23-52): the sensor's beams and the two LUTs zones are rendered with, built on
+    the GPU in float64 (range unit 0.001; the BODY LUT uses scale_translation(sensor_to_body) * lidar_to_sensor)."""
+
+    def __init__(self, n_cols, px_altitudes, px_azimuths, beam_to_lidar_transform, lidar_to_sensor_transform,
+                 sensor_to_body_transform=None, m_per_zmbin=0.0074927621875, serial_number=0, device=0):
+        self.n_cols, self.n_rows = int(n_cols), len(px_altitudes)
+        self.beam_to_lidar_transform = np.array(beam_to_lidar_transform, np.float64).reshape(4, 4)
+        self.lidar_to_sensor_transform = np.array(lidar_to_sensor_transform, np.float64).reshape(4, 4)
+        self.sensor_to_body_transform = None if sensor_to_body_transform is None else \
+            np.array(sensor_to_body_transform, np.float64).reshape(4, 4)
+        self.m_per_zmbin, self.serial_number = m_per_zmbin, serial_number
+        self.px_altitudes, self.px_azimuths = list(px_altitudes), list(px_azimuths)
+        if not self.beam_to_lidar_transform.any():
+            raise RuntimeError("BeamConfig: beam_to_lidar_transform not set")
+        if not self.lidar_to_sensor_transform.any():
+            raise RuntimeError("BeamConfig: lidar_to_sensor_transform not set")
+        lut = lambda tr: _c.XYZLutT.from_intrinsics(self.n_cols, self.n_rows, 0.001, self.beam_to_lidar_transform,
+                                                    tr, self.px_azimuths, self.px_altitudes, np.float64, device)
+        self.lut_no_sensor_to_body_transform = lut(self.lidar_to_sensor_transform)
+        self.lut = None
+        if self.sensor_to_body_transform is not None:
+            s2b = self.sensor_to_body_transform.copy()
+            s2b[:3, 3] *= 1000
+            self.lut = lut(s2b @ self.lidar_to_sensor_transform)
+
+    @classmethod
+    def from_sensor_info(cls, info, sensor_to_body_transform=None, device=0):
+        return cls(_sensor_value(info, "w"), _sensor_value(info, "beam_altitude_angles"),
+                   _sensor_value(info, "beam_azimuth_angles"), _sensor_value(info, "beam_to_lidar_transform"),
+                   _sensor_value(info, "lidar_to_sensor_transform"), sensor_to_body_transform,
+                   serial_number=_sensor_value(info, "sn", 0), device=device)
+
+
+class Zone:
+    """Zone (zone.h).  render() runs on the GPU."""
+    MAX_TRIANGLES = 2048
+
+    def __init__(self):
+        self.point_count, self.frame_count, self.mode = 0, 0, ZoneMode.NONE
+        self.stl, self.zrb = None, None
+
+    def check_invariants(self):
+        """zone.cpp:18-46"""
+        if self.point_count == 0:
+            raise RuntimeError("Zone: point_count must be in [1, 262143]")
+        if self.frame_count == 0:
+            raise RuntimeError("Zone: frame_count must be in [1, 65535]")
+        if self.stl is None and self.zrb is None:
+            raise RuntimeError("Zone: must have either STL or ZRB")
+        if self.mode not in (ZoneMode.OCCUPANCY, ZoneMode.VACANCY):
+            raise RuntimeError("Zone: mode must be OCCUPANCY or VACANCY")
+        if self.stl is not None:
+            if not self.stl.blob:
+                raise RuntimeError("Zone: STL blob cannot be empty")
+            if self.stl.coordinate_frame == CoordinateFrame.NONE:
+                raise RuntimeError("Zone: STL coordinate frame must be BODY or SENSOR")
+        if self.zrb is not None and np.count_nonzero(self.zrb.far_range_mm != 0) < self.point_count:
+            raise RuntimeError("Zone: ZRB far range image has fewer nonzero pixels than point_count")
+
+    def _renderable(self, config):
+        """The early returns of Zone::render (zone.cpp:64-85): the mesh, or None after the reference's message."""
+        self.check_invariants()
+        if self.stl is None:
+            print("Zone: Error rendering zone, no STL provided.", file=_sys.stderr)
+            return None
+        tris = self.stl.to_mesh().triangles
+        if len(tris) == 0:
+            print("Zone: Error rendering zone, STL has no triangles.", file=_sys.stderr)
+            return None
+        if len(tris) > self.MAX_TRIANGLES:
+            print("Zone: Error rendering zone, STL has too many triangles.", file=_sys.stderr)
+            return None
+        if self.stl.coordinate_frame == CoordinateFrame.BODY and config.sensor_to_body_transform is None:
+            print("Zone: Error rendering zone, sensor_to_body_transform not set for BODY coordinate frame.",
+                  file=_sys.stderr)
+            return None
+        return tris
+
+    def render(self, config):
+        """Zone::render(BeamConfig): True with self.zrb set, False where the reference returns false."""
+        return _render_zones([self], config)[0]
+
+
+def _render_zones(zones, config):
+    """Zone::render for several zones in one launch; -> list of bools"""
+    todo, meshes = [], []
+    ok = [False] * len(zones)
+    for i, z in enumerate(zones):
+        tris = z._renderable(config)
+        if tris is not None:
+            todo.append(i)
+            meshes.append({"triangles": tris, "coordinate_frame": int(z.stl.coordinate_frame),
+                           "point_count": z.point_count, "frame_count": z.frame_count, "mode": int(z.mode)})
+    if not todo:
+        return ok
+    try:
+        near, far, px = _c.zone_render(meshes, config.n_rows, config.n_cols, config.lut_no_sensor_to_body_transform,
+                                       config.lut, device_out=False)
+    except _c._capi.OusterB200Error as e:
+        raise RuntimeError(str(e).split("] ", 1)[-1]) from None
+    s2b = config.sensor_to_body_transform if config.sensor_to_body_transform is not None else np.eye(4)
+    for k, i in enumerate(todo):
+        zones[i].zrb = Zrb(near[k], far[k], config.serial_number, config.beam_to_lidar_transform.copy(),
+                           config.lidar_to_sensor_transform.copy(), s2b.copy())
+        ok[i] = bool(px[k] > 0)
+    return ok
+
+
+class ZoneSet:
+    """A minimal ZoneSet (zone_monitor.h): zones by id, power_on_live_ids and sensor_to_body_transform."""
+
+    def __init__(self):
+        self.zones = {}
+        self.power_on_live_ids = []
+        self.sensor_to_body_transform = None
+
+    def render(self, sensor_info, device=0):
+        """ZoneSet::render (zone_monitor.cpp:399-448): every zone with an STL, in one GPU launch."""
+        config = BeamConfig.from_sensor_info(sensor_info, self.sensor_to_body_transform, device)
+        ids = [i for i, z in self.zones.items() if not (z.zrb is not None and z.stl is None)]
+        ok = _render_zones([self.zones[i] for i in ids], config)
+        for i, good in zip(ids, ok):
+            if not good:
+                raise RuntimeError(f"ZoneSet::render: zone {i} was out of sensor FOV.")
+            self.zones[i].zrb.serial_number = _sensor_value(sensor_info, "sn", 0)
+
+
+class EmulatedZoneMon:
+    """EmulatedZoneMon (zone_common.py:14-136) over a device-resident ZoneMonitor.  calc_triggers takes numpy or
+    CUDA range images; with CUDA input nothing waits for the GPU until an attribute or get_packet() is read."""
+
+    def __init__(self, zone_set, device=0):
+        if not zone_set.zones:
+            raise ValueError("ZoneSet must have at least one zone defined")
+        if not all(zone.zrb is not None for zone in zone_set.zones.values()):
+            raise ValueError("EmulatedZoneMon: all zones in ZoneSet must have a valid ZRB")
+        self.zone_set, self.device = zone_set, device
+        self._counts = ({}, {}, {}, {}, {}, {})
+        self._triggers = [0] * MAX_AVAILABLE_ZONES
+        self._alerts = [0] * MAX_AVAILABLE_ZONES
+        self.update_count = 0
+        self.rendered_zones = {}
+        self.live_zones = list(zone_set.power_on_live_ids)
+        self.debug = False
+        self.max_counts = {}
+        for zone_id, zone in zone_set.zones.items():
+            self.max_counts[zone_id] = int(np.count_nonzero(np.asarray(zone.zrb.near_range_mm) <
+                                                            np.asarray(zone.zrb.far_range_mm)))
+            self.rendered_zones[zone_id] = zone.zrb
+        self._mon = None
+        self._dirty = False
+
+    def _monitor(self, h, w):
+        if self._mon is None or (self._mon.h, self._mon.w) != (h, w):
+            if len(self.live_zones) > MAX_ACTIVE_ZONES:
+                raise ValueError("at most 16 live zones")
+            live = []
+            for zone_id in self.live_zones:
+                z, zrb = self.zone_set.zones[zone_id], self.rendered_zones[zone_id]
+                live.append({"id": zone_id, "mode": int(z.mode), "point_count": z.point_count,
+                             "frame_count": z.frame_count, "near_mm": zrb.near_range_mm, "far_mm": zrb.far_range_mm,
+                             "triggers": self._triggers[zone_id], "alerts": self._alerts[zone_id]})
+            self._mon = _c.ZoneMonitor(live, h, w, self.device)
+        return self._mon
+
+    def set_live_zones(self, live_zones):
+        self._pull()
+        self.live_zones = list(live_zones)
+        self._mon = None
+
+    def calc_triggers(self, range_field, bitmask_field=None):
+        t = _dev(range_field)
+        r = t if t is not None else np.ascontiguousarray(range_field, np.uint32)
+        h, w = int(r.shape[0]), int(r.shape[1])
+        b = None
+        if bitmask_field is not None:
+            b = _dev(bitmask_field)
+            if b is None:
+                b = bitmask_field
+                if not isinstance(b, np.ndarray) or b.dtype != np.uint32 or not b.flags["C_CONTIGUOUS"]:
+                    raise ValueError("bitmask_field must be a C-contiguous uint32 array")
+        self._monitor(h, w).update(r, b)
+        self._dirty = True
+        if t is None:
+            self._pull()
+
+    def _pull(self):
+        """read the last update's records and counters back into the reference's attributes"""
+        if not self._dirty:
+            return
+        self._dirty = False
+        st = self._mon.states()
+        trig, alerts, sums = self._mon.counters()
+        dicts = ({}, {}, {}, {}, {}, {})
+        keys = ("count", "occlusion_count", "invalid_count", "min_range", "max_range")
+        for slot, zone_id in enumerate(self.live_zones):
+            for d, k in zip(dicts, keys):
+                d[zone_id] = int(st[slot][k])
+            # np.mean of the triggering uint32 ranges: their sum is exact in float64 below 2^53, then one division
+            cnt = int(st[slot]["count"])
+            dicts[5][zone_id] = np.float64(sums[slot]) / cnt if cnt else 0
+            self._triggers[zone_id], self._alerts[zone_id] = trig[slot], alerts[slot]
+        self._counts = dicts
+
+    def _get(i):
+        return property(lambda self: (self._pull(), self._counts[i])[1])
+
+    zone_counts, occlusion_counts, invalid_counts = _get(0), _get(1), _get(2)
+    zone_mins, zone_maxes, zone_avgs = _get(3), _get(4), _get(5)
+    del _get
+    zone_triggers = property(lambda self: (self._pull(), self._triggers)[1])
+    zone_alerts = property(lambda self: (self._pull(), self._alerts)[1])
+
+    @property
+    def triggered_zone_ids(self):
+        return [zone_id for zone_id, alerts in enumerate(self.zone_alerts) if alerts > 0]
+
+    def get_packet(self):
+        """the 16 ZoneState records (recarray; id 255 for unused slots)"""
+        if self._mon is None:
+            zmu = np.zeros(MAX_ACTIVE_ZONES, _c.ZONE_STATE_DTYPE)
+            zmu["id"][len(self.live_zones):] = 255
+            return zmu.view(np.recarray)
+        self._pull()
+        return self._mon.states().view(np.recarray)
