@@ -65,8 +65,8 @@ inline core::DenseArray<double> normals(const core::ArrayRef<const double>& xyz,
     return out;
 }
 
-/// Dual-return overload (normals.h:100-108, normals.cpp:432-483): both returns share the vertical pixel
-/// subtent of the first and see each other's points as neighbours.
+/// Dual-return overload (normals.h:100-108, normals.cpp:432-483): the returns see each other's points as
+/// neighbours; the second uses the first's vertical pixel subtent when that is > 0, else derives its own.
 /// @throws additionally std::runtime_error "normals: range2 dimensions mismatch".
 inline std::pair<core::DenseArray<double>, core::DenseArray<double>> normals(
     const core::ArrayRef<const double>& xyz, const core::ArrayRef<const uint32_t>& range,

@@ -201,8 +201,10 @@ ob_status ob_dewarp_frames(const ob_dewarp_frames_io* frames, size_t n_frames, d
  *                                ouster_algorithm/include/ouster/algorithm/normals.h:58-108
  *          compute_unit_normals / compute_vertical_subtent   ouster_algorithm/src/normals.cpp:32-407
  * Inputs are DESTAGGERED images (e.g. ob_cloud_io.xyz_destaggered / range_destaggered, in place on the
- * device); xyz2/range2/normals2 all set = the dual-return overload (both returns share the vertical
- * pixel subtent of the first and see each other's points as neighbours).  dtype = scalar type of
+ * device); xyz2/range2/normals2 all set = the dual-return overload (the returns see each other's points
+ * as neighbours; the second return's pass uses the first return's vertical pixel subtent when that is
+ * > 0, and otherwise derives its own from xyz2/range2, as compute_unit_normals ignores an override of 0).
+ * dtype = scalar type of
  * xyz* and normals* (the reference is double; float inputs are widened, results rounded once).
  * n_frames > 1 batches independent frames (strides in ELEMENTS, 0 = dense).
  * errors (OB_RUNTIME_ERROR, the reference's std::runtime_error texts): "normals: target_distance_m
@@ -226,7 +228,7 @@ typedef struct ob_normals_io {
     double min_angle_of_incidence_rad; /* reference default 1 deg (normals.h:25) */
     double target_distance_m;          /* reference default 0.025 (normals.h:23) */
     double vertical_subtent_rad;       /* > 0: use this instead of deriving it from the first return */
-    double* vertical_subtent_out;      /* optional, n_frames doubles: the per-pixel vertical subtent used */
+    double* vertical_subtent_out;      /* optional, n_frames doubles: the first return's vertical pixel subtent */
 } ob_normals_io;
 ob_status ob_normals(ob_dtype dtype, const ob_normals_io* io, ob_stream* s);
 

@@ -246,8 +246,9 @@ int orc_normals_compute(const double* xyz, const uint32_t* range, const double* 
 }
 
 /* normals(xyz, range, xyz2, range2, origins, ...) -- normals.cpp:432-483: one vertical subtent from
- * the first return, shared by both passes.  n2 / xyz2 / range2 may be NULL (single-return overload,
- * normals.cpp:411-430). */
+ * the first return, passed to both passes; orc_normals_compute ignores a subtent of 0, so then the
+ * second pass derives its own from (xyz2, range2).  n2 / xyz2 / range2 may be NULL (single-return
+ * overload, normals.cpp:411-430). */
 int orc_normals(const double* xyz, const uint32_t* range, const double* xyz2, const uint32_t* range2,
                 size_t h, size_t w, const double* origins, size_t search, double min_aoi_rad,
                 double target_m, double subtent_override, double* n1, double* n2) {

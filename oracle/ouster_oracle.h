@@ -209,7 +209,9 @@ size_t orc_dewarp_frame_f32(float* out, uint32_t* col_idx, uint64_t* ts_out, con
 /* ---- surface normals on destaggered XYZ -- ouster_algorithm/src/normals.cpp:32-483 (orc_normals.c) ----
  * xyz: h*w x 3 doubles (destaggered), range: h x w, origins: w x 3 (per-column sensor origin) or NULL.
  * orc_normals: single return when xyz2/range2 are NULL (normals.cpp:411-430), else both returns with
- * one shared vertical subtent (:432-483).  subtent_override <= 0: derive it from the first return.
+ * the first return's vertical subtent passed to both passes (:432-483); a pass given a subtent <= 0
+ * derives its own, so the second return's pass uses the subtent of (xyz2, range2) when the first
+ * return's is 0.  subtent_override <= 0: derive it from the first return.
  * returns 0, -1 "normals: target_distance_m must be positive", -2 "normals: min_angle_of_incidence_rad
  * must be positive". */
 double orc_normals_vertical_subtent(const double* xyz, const uint32_t* range, const double* origins,

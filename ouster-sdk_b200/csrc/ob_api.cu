@@ -185,6 +185,15 @@ cudaError_t Staging::out(void* p, size_t bytes, void** dev) {
     return cudaSuccess;
 }
 
+cudaError_t Staging::inout(void* p, size_t bytes, void** dev) {
+    const void* d = nullptr;
+    cudaError_t e = in(p, bytes, &d);
+    if (e != cudaSuccess) return e;
+    if (d != p) pending_.push_back({p, const_cast<void*>(d), bytes});
+    *dev = const_cast<void*>(d);
+    return cudaSuccess;
+}
+
 cudaError_t Staging::scratch(size_t bytes, void** dev) {
     void* d = nullptr;
     cudaError_t e = cudaMallocAsync(&d, bytes ? bytes : 16, st_);

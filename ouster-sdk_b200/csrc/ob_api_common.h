@@ -16,12 +16,15 @@ void reduce_shifts(const int32_t* shifts, size_t h, size_t w, int inverse, std::
 // Per-call staging of host buffers through stream-ordered device scratch.
 // in():  host -> scratch (H2D issued immediately); device pointers pass through.
 // out(): scratch now, D2H issued by flush() after the kernel; device pointers pass through.
+// inout(): as out(), but the host contents are uploaded first, so bytes the kernel leaves alone
+//          (padding between strided frames) come back unchanged.
 class Staging {
    public:
     explicit Staging(cudaStream_t st) : st_(st) {}
     ~Staging();
     cudaError_t in(const void* p, size_t bytes, const void** dev);
     cudaError_t out(void* p, size_t bytes, void** dev);
+    cudaError_t inout(void* p, size_t bytes, void** dev);
     cudaError_t scratch(size_t bytes, void** dev);
     cudaError_t flush();
 

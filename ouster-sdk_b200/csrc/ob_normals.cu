@@ -35,7 +35,7 @@ struct NormalsParams {
     const uint32_t* range[2];  // per return: n_frames x H x W
     void* out[2];              // per return: normals, same layout as xyz
     const double* origins;     // W x 3 per frame (stride origins_fs) or null = zeros
-    double* subtent;           // n_frames doubles (device): vertical pixel subtent used
+    double* subtent[2];        // per return: n_frames doubles (device), the vertical pixel subtent derived from it
     unsigned long long xyz_fs, range_fs, out_fs, origins_fs;  // frame strides in elements
     unsigned H, W, n_frames, search;
     double desired_sq, tan_safe, h_subtent, subtent_override;
@@ -80,16 +80,19 @@ __device__ __forceinline__ void beam_of(const T* xyz, const double* origins, uns
 
 // compute_vertical_subtent (normals.cpp:32-76): candidates are visited in the reference's order
 // (mid, mid, mid-1, mid+1, ...); a warp examines 32 of them at a time, the first hit in that order wins.
+// Warp r of block f derives the subtent of return r of frame f (warp 1 only runs for dual returns).
 template <typename T>
 __global__ void normals_subtent_kernel(const __grid_constant__ NormalsParams p) {
     const unsigned f = blockIdx.x;
-    const unsigned lane = threadIdx.x;
-    const T* xyz = static_cast<const T*>(p.xyz[0]) + f * p.xyz_fs;
-    const uint32_t* range = p.range[0] + f * p.range_fs;
+    const unsigned lane = threadIdx.x & 31;
+    const unsigned ret = threadIdx.x >> 5;
+    const T* xyz = static_cast<const T*>(p.xyz[ret]) + f * p.xyz_fs;
+    const uint32_t* range = p.range[ret] + f * p.range_fs;
     const double* origins = p.origins ? p.origins + f * p.origins_fs : nullptr;
+    double* subtent = p.subtent[ret];
     const unsigned W = p.W, H = p.H;
     if (p.subtent_override > 0.0) {
-        if (lane == 0) p.subtent[f] = p.subtent_override;
+        if (lane == 0) subtent[f] = p.subtent_override;
         return;
     }
     const unsigned mid = W / 2;
@@ -126,14 +129,14 @@ __global__ void normals_subtent_kernel(const __grid_constant__ NormalsParams p) 
         if (mask != 0) {
             const int src = __ffs(mask) - 1;
             const double v = __shfl_sync(0xffffffffu, value, src);
-            if (lane == 0) p.subtent[f] = v;
+            if (lane == 0) subtent[f] = v;
             return;
         }
     }
     if (lane == 0) {  // no valid pair: 90 degrees of vertical field of view over the image height
         const unsigned long long hm1 = static_cast<unsigned long long>(H) - 1ull;  // size_t arithmetic of the reference
         const unsigned long long intervals = hm1 > 1ull ? hm1 : 1ull;
-        p.subtent[f] = (0.5 * 3.14159265358979323846) / static_cast<double>(intervals);
+        subtent[f] = (0.5 * 3.14159265358979323846) / static_cast<double>(intervals);
     }
 }
 
@@ -243,11 +246,16 @@ __global__ void __launch_bounds__(256) normals_kernel(const __grid_constant__ No
         load3(xyz, idx, center);
         beam_of(xyz, origins, p.W, u, v, beam);
         if (dot3(beam, beam) <= kEps) break;
+        // The dual-return overload passes the first return's subtent to both passes, but
+        // compute_unit_normals only honours an override > 0 (normals.cpp:134-140, 447-479): when the
+        // first return's subtent is 0, the second return's pass derives its own from (xyz2, range2).
+        double v_subtent = p.subtent[0][f];
+        if (ret == 1 && !(v_subtent > 0.0)) v_subtent = p.subtent[1][f];
         // calc_max_distance_threshold (normals.cpp:143-151)
         const double two_pi = 2.0 * 3.14159265358979323846;
         const double perimeter = mul(two_pi, mul(static_cast<double>(cr), 0.001));
         const double nh = (perimeter / (two_pi / p.h_subtent)) / p.tan_safe;
-        const double nv = (perimeter / (two_pi / p.subtent[f])) / p.tan_safe;
+        const double nv = (perimeter / (two_pi / v_subtent)) / p.tan_safe;
         const unsigned max_up = min(p.search, u), max_down = min(p.search, p.H - 1 - u);
         double vd[3] = {0, 0, 0}, hd[3] = {0, 0, 0};
         bool vflip = false, hflip = false, vthin = true, hthin = true;
@@ -330,18 +338,24 @@ extern "C" ob_status ob_normals(ob_dtype dtype, const ob_normals_io* io, ob_stre
     NormalsParams p{};
     const void* d = nullptr;
     void* o = nullptr;
+    // a host output with padding between frames is uploaded first so the padding survives the copy back
+    const size_t out_bytes = ((F - 1) * out_fs + n_px * 3) * esz;
+    const bool padded = F > 1 && out_fs != n_px * 3;
+    auto stage_out = [&](void* host, void** dev) {
+        return padded ? stg.inout(host, out_bytes, dev) : stg.out(host, out_bytes, dev);
+    };
     cudaError_t e = stg.in(io->xyz, ((F - 1) * xyz_fs + n_px * 3) * esz, &d);
     p.xyz[0] = d;
     if (e == cudaSuccess) e = stg.in(io->range, ((F - 1) * range_fs + n_px) * 4, &d);
     p.range[0] = static_cast<const uint32_t*>(d);
-    if (e == cudaSuccess) e = stg.out(io->normals, ((F - 1) * out_fs + n_px * 3) * esz, &o);
+    if (e == cudaSuccess) e = stage_out(io->normals, &o);
     p.out[0] = o;
     if (dual) {
         if (e == cudaSuccess) e = stg.in(io->xyz2, ((F - 1) * xyz_fs + n_px * 3) * esz, &d);
         p.xyz[1] = d;
         if (e == cudaSuccess) e = stg.in(io->range2, ((F - 1) * range_fs + n_px) * 4, &d);
         p.range[1] = static_cast<const uint32_t*>(d);
-        if (e == cudaSuccess) e = stg.out(io->normals2, ((F - 1) * out_fs + n_px * 3) * esz, &o);
+        if (e == cudaSuccess) e = stage_out(io->normals2, &o);
         p.out[1] = o;
     }
     if (e == cudaSuccess && io->sensor_origins_xyz) {
@@ -349,12 +363,15 @@ extern "C" ob_status ob_normals(ob_dtype dtype, const ob_normals_io* io, ob_stre
         p.origins = static_cast<const double*>(d);
     }
     void* sub = nullptr;
+    void* sub2 = nullptr;
     if (e == cudaSuccess) {
         if (io->vertical_subtent_out) e = stg.out(io->vertical_subtent_out, F * 8, &sub);
         else e = stg.scratch(F * 8, &sub);
     }
+    if (e == cudaSuccess && dual) e = stg.scratch(F * 8, &sub2);
     if (e != cudaSuccess) return fail_cuda(e, "stage normals buffers");
-    p.subtent = static_cast<double*>(sub);
+    p.subtent[0] = static_cast<double*>(sub);
+    p.subtent[1] = static_cast<double*>(sub2);
     p.xyz_fs = xyz_fs;
     p.range_fs = range_fs;
     p.out_fs = out_fs;
@@ -371,12 +388,13 @@ extern "C" ob_status ob_normals(ob_dtype dtype, const ob_normals_io* io, ob_stre
     if (F > 65535) return fail(OB_INVALID_ARGUMENT, "too many frames in one call");
     const dim3 grid((p.W + 31) / 32, (p.H + 7) / 8, static_cast<unsigned>(F));
     if (grid.y > 65535) return fail(OB_INVALID_ARGUMENT, "frame too tall");
+    const unsigned sub_threads = dual ? 64 : 32;  // one warp per return
     if (dtype == OB_F64) {
-        normals_subtent_kernel<double><<<static_cast<unsigned>(F), 32, 0, st>>>(p);
+        normals_subtent_kernel<double><<<static_cast<unsigned>(F), sub_threads, 0, st>>>(p);
         normals_kernel<double><<<grid, 256, 0, st>>>(p, 0);
         if (dual) normals_kernel<double><<<grid, 256, 0, st>>>(p, 1);
     } else {
-        normals_subtent_kernel<float><<<static_cast<unsigned>(F), 32, 0, st>>>(p);
+        normals_subtent_kernel<float><<<static_cast<unsigned>(F), sub_threads, 0, st>>>(p);
         normals_kernel<float><<<grid, 256, 0, st>>>(p, 0);
         if (dual) normals_kernel<float><<<grid, 256, 0, st>>>(p, 1);
     }
