@@ -52,7 +52,8 @@ int ob_abi_version(void);
 /* sizeof() of a public struct by name ("ob_cloud_io", "ob_field_desc", "ob_packet_layout",
  * "ob_decode_io", "ob_decode_batch", "ob_dewarp_frame_io", "ob_normals_io", "ob_encode_io", "ob_dewarp_frames_io",
  * "ob_voxel_io", "ob_point_rows", "ob_voxel_map_cull_io", "ob_voxel_query_io", "ob_icp_io", "ob_icp_system_io",
- * "ob_cloud_align_io", "ob_cloud_nearest_io", "ob_zone_desc", "ob_zone_render_io", "ob_zone_live", "ob_zone_state");
+ * "ob_cloud_align_io", "ob_cloud_nearest_io", "ob_zone_desc", "ob_zone_render_io", "ob_zone_live", "ob_zone_state",
+ * "ob_image_params", "ob_image_state");
  * 0 for unknown names.  Lets FFI bindings verify their layout. */
 size_t ob_abi_sizeof(const char* struct_name);
 const char* ob_last_error(void);
@@ -61,7 +62,7 @@ int ob_device_count(void);
 /* kernels launched by this library since load (all threads); the bench's gpu_launches claim */
 uint64_t ob_kernel_launch_count(void);
 /* launches of one named kernel family since load: "decode_pipe" (pipelined K2), "decode" (K2, any
- * kernel), "cloud" (K1), "normals", "voxel", "voxel_map", "icp", "align", "zone"; 0 for unknown names.  Lets tests assert which code path ran. */
+ * kernel), "cloud" (K1), "normals", "voxel", "voxel_map", "icp", "align", "zone", "image"; 0 for unknown names.  Lets tests assert which code path ran. */
 uint64_t ob_kernel_launch_count_of(const char* name);
 /* tuning hook (launch geometry and code-path selection only, never results): cloud_tw, cloud_stages,
  * cloud_threads (compute threads; a copy warp is added), cloud_ctas_per_sm, cloud_store_lag,
@@ -516,6 +517,57 @@ ob_status ob_zone_monitor_states(const ob_zone_monitor* m, void* out, ob_stream*
 ob_status ob_zone_monitor_counters(const ob_zone_monitor* m, uint32_t* triggers, uint32_t* alerts,
                                    uint64_t* range_sums, ob_stream* s);
 ob_status ob_zone_monitor_destroy(ob_zone_monitor* m);
+
+/* ---- image post-processing (DESIGN f-9) ----
+ * replaces AutoExposure, BeamUniformityCorrector and LocalToneMapper   ouster_core/src/image_processing.cpp
+ * One handle holds one processor's state (lo/hi, their damped states, the update counter, the dark count) in
+ * device memory; an update reads and writes it only on the stream, so with device buffers nothing waits for the
+ * host and a sequence of updates can be captured in a CUDA graph. */
+typedef enum ob_image_kind {
+    OB_IMAGE_AUTO_EXPOSURE = 0,
+    OB_IMAGE_BEAM_UNIFORMITY = 1,
+    OB_IMAGE_LOCAL_TONE_MAP = 2
+} ob_image_kind;
+typedef enum ob_image_layout {
+    OB_IMAGE_MONO = 0,   /* rows x cols of dtype, in place (AE, BUC) */
+    OB_IMAGE_RGB = 1,    /* rows x cols x 3 of dtype, in place (AE, LTM) */
+    OB_IMAGE_RGB_F16 = 2 /* rows x cols x 3 float16 bits in, float32 out, dtype OB_F32 (AE, LTM) */
+} ob_image_layout;
+
+/* the constructor arguments; BUC ignores all of them (damping 0.92, update every 8) */
+typedef struct ob_image_params {
+    double lo_percentile, hi_percentile; /* each in [0, 1) */
+    int32_t update_every;                /* >= 1 */
+    int32_t color_correct;               /* LTM only */
+    double damping;
+    double compress_dr_max_lum; /* LTM only; the bool constructor maps true / false to 0.2 / 0.0 */
+} ob_image_params;
+
+/* a snapshot of a processor's state (reference member names in brackets) */
+typedef struct ob_image_state {
+    double lo, hi, lo_state, hi_state; /* [lo_, hi_, lo_state_, hi_state_], -1 until initialised (AE, LTM) */
+    int32_t counter;                   /* [counter_] */
+    int32_t initialized;               /* [initialized_] (AE, LTM) */
+    uint32_t dark_count_rows;          /* [dark_count_.size()] (BUC), 0 before the first update */
+    uint32_t reserved;
+} ob_image_state;
+
+typedef struct ob_image_proc ob_image_proc;
+/* errors: "lo_percentile and hi_percentile must be in [0, 1)", "update_every must be >= 1", "unknown kind" */
+ob_status ob_image_proc_create(int device, int kind /* ob_image_kind */, const ob_image_params* params,
+                               ob_image_proc** out);
+/* one update(image, update_state) of the reference.  MONO / RGB: `out` is the image, updated in place, and `in`
+ * is NULL or equal to `out`.  RGB_F16: `in` holds rows x cols x 3 float16 bits, converted into `out` with
+ * f16_bits_to_f32_bits_fast_nan_zero before the update.  Host or device buffers; a host image synchronises.
+ * errors: "layout not supported by this processor", "image too large", "stream and processor are on different
+ * devices" */
+ob_status ob_image_proc_update(ob_image_proc* p, int layout /* ob_image_layout */, int dtype /* ob_dtype */,
+                               const void* in, void* out, uint32_t rows, uint32_t cols, int update_state,
+                               ob_stream* s);
+/* synchronising read of the state; dark_count (optional, host) gets min(dark_count_rows, cap) doubles */
+ob_status ob_image_proc_state(const ob_image_proc* p, ob_image_state* state, double* dark_count, size_t cap,
+                              ob_stream* s);
+ob_status ob_image_proc_destroy(ob_image_proc* p);
 
 /* ---- fused range -> (XYZ, destaggered range, destaggered XYZ), batched over frames ----
  * One launch performs, for every frame f and return r of the batch, what the reference does as

@@ -123,6 +123,20 @@ class ZoneState(C.Structure):
                 ("mean_range", u32)]
 
 
+OB_IMAGE_AUTO_EXPOSURE, OB_IMAGE_BEAM_UNIFORMITY, OB_IMAGE_LOCAL_TONE_MAP = range(3)
+OB_IMAGE_MONO, OB_IMAGE_RGB, OB_IMAGE_RGB_F16 = range(3)
+
+
+class ImageParams(C.Structure):
+    _fields_ = [("lo_percentile", C.c_double), ("hi_percentile", C.c_double), ("update_every", C.c_int32),
+                ("color_correct", C.c_int32), ("damping", C.c_double), ("compress_dr_max_lum", C.c_double)]
+
+
+class ImageState(C.Structure):
+    _fields_ = [("lo", C.c_double), ("hi", C.c_double), ("lo_state", C.c_double), ("hi_state", C.c_double),
+                ("counter", C.c_int32), ("initialized", C.c_int32), ("dark_count_rows", u32), ("reserved", u32)]
+
+
 class DewarpFramesIO(C.Structure):
     _fields_ = [("lut", vp), ("range", vp), ("poses", vp), ("status", vp), ("timestamps", vp)]
 
@@ -221,6 +235,10 @@ _sig("ob_zone_monitor_update", i32, vp, vp, vp, vp)
 _sig("ob_zone_monitor_states", i32, vp, vp, vp)
 _sig("ob_zone_monitor_counters", i32, vp, vp, vp, vp, vp)
 _sig("ob_zone_monitor_destroy", i32, vp)
+_sig("ob_image_proc_create", i32, i32, i32, C.POINTER(ImageParams), C.POINTER(vp))
+_sig("ob_image_proc_update", i32, vp, i32, i32, vp, vp, u32, u32, i32, vp)
+_sig("ob_image_proc_state", i32, vp, C.POINTER(ImageState), vp, sz, vp)
+_sig("ob_image_proc_destroy", i32, vp)
 _sig("ob_dewarp_frames", i32, C.POINTER(DewarpFramesIO), sz, C.c_double, C.c_double, vp, sz, vp, vp, vp,
      C.POINTER(sz), C.POINTER(sz), vp)
 if hasattr(lib, "ob_decoder_create"):

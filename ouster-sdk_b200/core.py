@@ -1299,3 +1299,98 @@ class ZoneMonitor:
         check(lib.ob_zone_monitor_counters(self._h, t.ctypes.data, a.ctypes.data, r.ctypes.data, st.h))
         return ([int(v) for v in t[:self.n_live]], [int(v) for v in a[:self.n_live]],
                 [int(v) for v in r[:self.n_live]])
+
+
+class ImageProcessor:
+    """Device-resident image post-processor (ob_image_proc): one AutoExposure, BeamUniformityCorrector or
+    LocalToneMapper with its state in device memory.  kind: "auto_exposure", "beam_uniformity" or
+    "local_tone_map"; the keyword arguments are the constructor's (ignored by beam_uniformity), and those left out
+    take the kind's default constructor values."""
+
+    KINDS = {"auto_exposure": _capi.OB_IMAGE_AUTO_EXPOSURE, "beam_uniformity": _capi.OB_IMAGE_BEAM_UNIFORMITY,
+             "local_tone_map": _capi.OB_IMAGE_LOCAL_TONE_MAP}
+    # the reference's default constructors (image_processing.cpp:201-205, 508-509, header defaults)
+    DEFAULTS = {"auto_exposure": dict(lo_percentile=0.1, hi_percentile=0.1, update_every=3, damping=0.9,
+                                      compress_dr_max_lum=0.0, color_correct=False),
+                "beam_uniformity": dict(lo_percentile=0.0, hi_percentile=0.0, update_every=8, damping=0.92,
+                                        compress_dr_max_lum=0.0, color_correct=False),
+                "local_tone_map": dict(lo_percentile=0.0, hi_percentile=0.2, update_every=1, damping=0.3,
+                                       compress_dr_max_lum=0.2, color_correct=True)}
+
+    def __init__(self, kind, lo_percentile=None, hi_percentile=None, update_every=None, damping=None,
+                 compress_dr_max_lum=None, color_correct=None, device=0):
+        given = dict(lo_percentile=lo_percentile, hi_percentile=hi_percentile, update_every=update_every,
+                     damping=damping, compress_dr_max_lum=compress_dr_max_lum, color_correct=color_correct)
+        a = {k: (self.DEFAULTS[kind][k] if v is None else v) for k, v in given.items()}
+        p = _capi.ImageParams(float(a["lo_percentile"]), float(a["hi_percentile"]), int(a["update_every"]),
+                              int(bool(a["color_correct"])), float(a["damping"]), float(a["compress_dr_max_lum"]))
+        hd = C.c_void_p()
+        check(lib.ob_image_proc_create(device, self.KINDS[kind], C.byref(p), C.byref(hd)))
+        self._h, self.kind, self.device = hd, kind, device
+        self._st = None
+        self._wrapped = None
+
+    def __del__(self):
+        if getattr(self, "_h", None) and lib is not None:
+            try:
+                lib.ob_image_proc_destroy(self._h)
+            except Exception:
+                pass
+            self._h = None
+
+    def _stream_for(self, x, stream):
+        if stream is not None:
+            return stream
+        if _is_torch(x) and x.is_cuda:
+            import torch
+            h = torch.cuda.current_stream(x.device).cuda_stream
+            if self._wrapped is None or self._wrapped[0] != h:  # one wrapper per torch stream, reused per frame
+                self._wrapped = (h, Stream(x.device.index, cuda_stream=h))
+            return self._wrapped[1]
+        return _stream(None, self.device)
+
+    def update(self, image, out=None, update_state=True, stream=None):
+        """update(image, update_state).  image: (h, w) or (h, w, 3) float32 / float64, C-contiguous numpy array or
+        torch tensor, updated in place; or (h, w, 3) float16, converted into `out` ((h, w, 3) float32, allocated
+        when None and returned).  CUDA tensors run on the torch current stream and nothing waits for the GPU."""
+        shape = tuple(image.shape)
+        dt = _np_dtype(image) if not (_is_torch(image) and str(image.dtype) == "torch.float16") else np.dtype(np.float16)
+        if len(shape) == 3 and shape[2] != 3 or len(shape) not in (2, 3):
+            raise ValueError("Expected an H x W x 3 array")
+        contiguous = image.is_contiguous() if _is_torch(image) else image.flags["C_CONTIGUOUS"]
+        if not contiguous:
+            raise TypeError("image must be C-contiguous")
+        rows, cols = shape[0], shape[1]
+        st = self._stream_for(image, stream)
+        self._st = st
+        if dt == np.float16:
+            if len(shape) != 3:
+                raise ValueError("Expected an H x W x 3 array")
+            if out is None:
+                if _is_torch(image):
+                    import torch
+                    out = torch.empty(shape, dtype=torch.float32, device=image.device)
+                else:
+                    out = np.empty(shape, np.float32)
+            check(lib.ob_image_proc_update(self._h, _capi.OB_IMAGE_RGB_F16, _capi.OB_F32, _ptr(image), _ptr(out),
+                                           rows, cols, int(bool(update_state)), st.h))
+            return out
+        if dt not in (np.float32, np.float64):
+            raise TypeError("image must be float32 or float64")
+        layout = _capi.OB_IMAGE_MONO if len(shape) == 2 else _capi.OB_IMAGE_RGB
+        dtype = _capi.OB_F32 if dt == np.float32 else _capi.OB_F64
+        check(lib.ob_image_proc_update(self._h, layout, dtype, None, _ptr(image), rows, cols,
+                                       int(bool(update_state)), st.h))
+        return None
+
+    def state(self, stream=None):
+        """Synchronising read of the state: dict with lo, hi, lo_state, hi_state, counter, initialized and
+        dark_count (float64 array, BeamUniformityCorrector)."""
+        st = stream or self._st or _stream(None, self.device)
+        s = _capi.ImageState()
+        probe = _capi.ImageState()
+        check(lib.ob_image_proc_state(self._h, C.byref(probe), None, 0, st.h))
+        dc = np.zeros(max(probe.dark_count_rows, 1), np.float64)
+        check(lib.ob_image_proc_state(self._h, C.byref(s), dc.ctypes.data, dc.size, st.h))
+        return dict(lo=s.lo, hi=s.hi, lo_state=s.lo_state, hi_state=s.hi_state, counter=s.counter,
+                    initialized=bool(s.initialized), dark_count=dc[:s.dark_count_rows])

@@ -18,7 +18,7 @@ static std::atomic<uint64_t> g_launches{0};
 
 static std::atomic<uint64_t> g_family[OB_FAM_COUNT];
 static const char* const kFamilies[OB_FAM_COUNT] = {"decode_pipe", "decode", "cloud", "normals", "voxel",
-                                                    "voxel_map", "icp", "align", "zone"};
+                                                    "voxel_map", "icp", "align", "zone", "image"};
 
 void count_launch(uint64_t n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 void count_launch_of(int family, uint64_t n) {
@@ -345,6 +345,8 @@ size_t ob_abi_sizeof(const char* name) {
     if (n == "ob_zone_render_io") return sizeof(ob_zone_render_io);
     if (n == "ob_zone_live") return sizeof(ob_zone_live);
     if (n == "ob_zone_state") return sizeof(ob_zone_state);
+    if (n == "ob_image_params") return sizeof(ob_image_params);
+    if (n == "ob_image_state") return sizeof(ob_image_state);
     return 0;
 }
 

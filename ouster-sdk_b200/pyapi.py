@@ -930,3 +930,92 @@ class EmulatedZoneMon:
             return zmu.view(np.recarray)
         self._pull()
         return self._mon.states().view(np.recarray)
+
+
+# ---- image post-processing (ouster.sdk.core.AutoExposure & co., processing.cpp:785-880) -------------------------
+# numpy float32 / float64 images are updated in place and the call returns None; a float16 H x W x 3 image returns a
+# new float32 array.  Torch CUDA tensors (or device DLPack exporters) are processed in place on the torch current
+# stream without waiting for the GPU; the processor's state stays on the device between calls.
+
+def _image_arg(image, allowed):
+    """(array, kind) for an update() argument: kind "f16" or "float"; TypeError as nanobind's overload resolution
+    raises it for any other dtype or a non-C-contiguous array"""
+    d = _dev(image)
+    if d is not None:
+        torch = _torch()
+        kinds = {torch.float16: "f16", torch.float32: "float", torch.float64: "float"}
+        ok = d.dtype in kinds and kinds[d.dtype] in allowed and d.is_contiguous()
+        a, k = d, kinds.get(d.dtype)
+    else:
+        a = image
+        kinds = {np.dtype(np.float16): "f16", np.dtype(np.float32): "float", np.dtype(np.float64): "float"}
+        ok = isinstance(a, np.ndarray) and a.dtype in kinds and kinds[a.dtype] in allowed and a.flags["C_CONTIGUOUS"]
+        k = kinds.get(a.dtype) if isinstance(a, np.ndarray) else None
+    if not ok:
+        raise TypeError("update(): incompatible function arguments")
+    return a, k
+
+
+class _ImageProc:
+    _kind = None
+    _allowed = ()
+
+    def __init__(self, **kw):
+        self._p = _c.ImageProcessor(self._kind, **kw)
+
+    def update(self, image, update_state=True):
+        a, k = _image_arg(image, self._allowed)
+        if k == "f16" or a.ndim == 3:
+            if a.ndim != 3 or a.shape[2] != 3:
+                raise ValueError("Expected an H x W x 3 array")
+            if self._mono_only:
+                raise TypeError("update(): incompatible function arguments")
+        elif a.ndim != 2 or self._rgb_only:
+            raise TypeError("update(): incompatible function arguments")
+        return self._p.update(a, update_state=bool(update_state))
+
+    def _state(self):
+        return self._p.state()
+
+
+class AutoExposure(_ImageProc):
+    """AutoExposure(), AutoExposure(update_every), AutoExposure(lo_percentile, hi_percentile, update_every,
+    damping=0.9): mono and RGB float32 / float64 in place, float16 RGB to a new float32 array"""
+    _kind, _allowed, _mono_only, _rgb_only = "auto_exposure", ("f16", "float"), False, False
+
+    def __init__(self, *args, **kw):
+        names = ("lo_percentile", "hi_percentile", "update_every", "damping")
+        kw.update(zip(names[2:] if len(args) == 1 else names, args))
+        if len(args) not in (0, 1, 3, 4):
+            raise TypeError("__init__(): incompatible function arguments")
+        kw.setdefault("update_every", 3)
+        super().__init__(**kw)
+
+
+class BeamUniformityCorrector(_ImageProc):
+    """BeamUniformityCorrector(): mono float32 / float64 in place"""
+    _kind, _allowed, _mono_only, _rgb_only = "beam_uniformity", ("float",), True, False
+
+    def __init__(self):
+        super().__init__()
+
+
+class LocalToneMapper(_ImageProc):
+    """LocalToneMapper(), LocalToneMapper(update_every), LocalToneMapper(lo, hi, update_every, damping,
+    compress_dr_max_lum | compress_dr, color_correct): float16 RGB to a new float32 array, as the Python binding
+    takes it"""
+    _kind, _allowed, _mono_only, _rgb_only = "local_tone_map", ("f16",), False, True
+
+    def __init__(self, *args, **kw):
+        names = ("lo_percentile", "hi_percentile", "update_every", "damping", "compress_dr_max_lum", "color_correct")
+        if "compress_dr" in kw:
+            kw["compress_dr_max_lum"] = kw.pop("compress_dr")
+        kw.update(zip(names[2:] if len(args) == 1 else names, args))
+        if len(args) not in (0, 1, 6):
+            raise TypeError("__init__(): incompatible function arguments")
+        c = kw.get("compress_dr_max_lum", 0.2)
+        kw["compress_dr_max_lum"] = (0.2 if c else 0.0) if isinstance(c, bool) else float(c)
+        defaults = dict(lo_percentile=0.0, hi_percentile=0.2, update_every=1, damping=0.3, color_correct=True)
+        for k, v in defaults.items():
+            kw.setdefault(k, v)
+        super().__init__(**kw)

@@ -318,4 +318,25 @@ for dt in (np.float64, np.float32):
     wp, wit = oa.point_to_plane_align(a, b, sn, tn, None, 0.5, 180.0)
     assert git == wit and np.abs(gp - wp).max() <= 1e-12
 print("cloud align ok")
+# image post-processing: every kernel of AE (mono, rgb, f16), BUC (f32, f64; median with masked columns) and LTM
+from oracle import image as oimg
+ri = np.random.default_rng(13)
+for dt in (np.float32, np.float64):
+    for kind, shape in (("auto_exposure", (12, 96)), ("auto_exposure", (12, 96, 3)), ("beam_uniformity", (12, 96)),
+                        ("local_tone_map", (12, 96, 3))):
+        proc = ob.ImageProcessor(kind)
+        ref = {"auto_exposure": oimg.AutoExposure, "beam_uniformity": oimg.BeamUniformityCorrector,
+               "local_tone_map": oimg.LocalToneMapper}[kind]()
+        for f in range(3):
+            a = ri.uniform(0, 2, shape).astype(dt)
+            a[..., ::7] = 0
+            g, want = a.copy(), a.copy()
+            proc.update(g)
+            ref.update(want)
+            assert np.array_equal(g, want, equal_nan=True), (kind, shape, f)
+for kind, ref in (("auto_exposure", oimg.AutoExposure()), ("local_tone_map", oimg.LocalToneMapper())):
+    proc = ob.ImageProcessor(kind)
+    src = ri.uniform(0, 1, (12, 96, 3)).astype(np.float16)
+    assert np.array_equal(proc.update(src), ref.update(src), equal_nan=True)
+print("image ok")
 print("SANITIZE CASES OK")
