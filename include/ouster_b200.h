@@ -53,7 +53,8 @@ int ob_abi_version(void);
  * "ob_decode_io", "ob_decode_batch", "ob_dewarp_frame_io", "ob_normals_io", "ob_encode_io", "ob_dewarp_frames_io",
  * "ob_voxel_io", "ob_point_rows", "ob_voxel_map_cull_io", "ob_voxel_query_io", "ob_icp_io", "ob_icp_system_io",
  * "ob_cloud_align_io", "ob_cloud_nearest_io", "ob_zone_desc", "ob_zone_render_io", "ob_zone_live", "ob_zone_state",
- * "ob_image_params", "ob_image_state");
+ * "ob_image_params", "ob_image_state", "ob_frame_field", "ob_frame_ops_io", "ob_frame_rows_entry",
+ * "ob_frame_rows_io");
  * 0 for unknown names.  Lets FFI bindings verify their layout. */
 size_t ob_abi_sizeof(const char* struct_name);
 const char* ob_last_error(void);
@@ -62,7 +63,7 @@ int ob_device_count(void);
 /* kernels launched by this library since load (all threads); the bench's gpu_launches claim */
 uint64_t ob_kernel_launch_count(void);
 /* launches of one named kernel family since load: "decode_pipe" (pipelined K2), "decode" (K2, any
- * kernel), "cloud" (K1), "normals", "voxel", "voxel_map", "icp", "align", "zone", "image"; 0 for unknown names.  Lets tests assert which code path ran. */
+ * kernel), "cloud" (K1), "normals", "voxel", "voxel_map", "icp", "align", "zone", "image", "frame_ops"; 0 for unknown names.  Lets tests assert which code path ran. */
 uint64_t ob_kernel_launch_count_of(const char* name);
 /* tuning hook (launch geometry and code-path selection only, never results): cloud_tw, cloud_stages,
  * cloud_threads (compute threads; a copy warp is added), cloud_ctas_per_sm, cloud_store_lag,
@@ -568,6 +569,84 @@ ob_status ob_image_proc_update(ob_image_proc* p, int layout /* ob_image_layout *
 ob_status ob_image_proc_state(const ob_image_proc* p, ob_image_state* state, double* dark_count, size_t cap,
                               ob_stream* s);
 ob_status ob_image_proc_destroy(ob_image_proc* p);
+
+/* ---- frame operations (DESIGN f-10) ----
+ * replaces frame_ops::clip, filter_field, filter_uv, mask   ouster_core/src/frame_ops.cpp:151-286
+ *          frame_ops.filter_xyz                             python/src/ouster/sdk/core/frame_ops.py:83-136
+ *          frame_ops::select_by_index (pixel rows)          ouster_core/src/frame_ops.cpp:125-138, 296-323
+ * ob_frame_mask_fields is one masked write over the pixel fields of a batch of frames of one shape (h x w): every
+ * pixel the predicate hits becomes static_cast<T>(invalid) in each target.  The field table lists per frame the
+ * targets (first- or second-return predicate), the fields to zero-fill, and the predicate's sources.  Field
+ * selection, the reference's error texts and the per-type skip rules are the caller's (the C++ and Python
+ * layers); this entry point refuses what it cannot write exactly:
+ *  - a NaN / infinite invalid for an integer target, or one the type cannot hold after truncation toward zero
+ *    ("invalid value cannot be represented in the field's type"; the reference's cast is undefined there);
+ *  - a VALUE source of a type outside u8..f64 ("filter_field requires a pixel field with shape (h, w) to build a
+ *    mask").
+ * Every argument is checked before anything is launched, so a failing call modifies nothing.
+ * Field data, sources and poses may be device, pinned or pageable memory (host buffers are staged and the call
+ * synchronises); the shift and row tables are read on the host and travel with the launch, so a call on device
+ * buffers never waits for the host and can be captured in a CUDA graph. */
+typedef enum ob_frame_predicate {
+    OB_FRAME_CLIP = 0,      /* each target's own value: hit unless lower <= (double)v <= upper (NaN: hit) */
+    OB_FRAME_VALUE = 1,     /* source value: hit if lower <= (double)v <= upper (filter_field; mask: u8, [0, 0]) */
+    OB_FRAME_ROWS = 2,      /* hit if lower <= row < upper (filter_uv "u") */
+    OB_FRAME_COLS = 3,      /* hit if lower <= (col + shift[row]) mod w < upper (filter_uv "v") */
+    OB_FRAME_XYZ_RANGE = 4, /* hit if lower <= p[axis] <= upper, p = lut(range) (then the column's pose), in the
+                             * LUT dtype with the bounds rounded to it (filter_xyz) */
+    OB_FRAME_XYZ_POINTS = 5 /* as XYZ_RANGE on given h x w x 3 points of type 9 (f32) or 10 (f64) */
+} ob_frame_predicate;
+typedef enum ob_frame_role {
+    OB_FRAME_TARGET = 0,  /* written where the first-return predicate hits (CLIP: its own predicate) */
+    OB_FRAME_TARGET2 = 1, /* written where the second-return predicate hits */
+    OB_FRAME_ZERO = 2,    /* every byte set to 0 (elem_bytes: bytes of one pixel, 1 to 65535) */
+    OB_FRAME_SOURCE = 3,  /* first-return source: VALUE field, XYZ_RANGE range (u32), XYZ_POINTS points */
+    OB_FRAME_SOURCE2 = 4  /* second-return source */
+} ob_frame_role;
+
+typedef struct ob_frame_field {
+    void* data;          /* h x w pixels (ZERO: h x w x elements; XYZ_POINTS source: h x w x 3) */
+    int32_t type;        /* ChanFieldType tag (chanfield.h): 1..10 for targets and VALUE sources */
+    int32_t role;        /* ob_frame_role */
+    uint32_t frame;      /* frame of the batch this entry belongs to */
+    uint32_t elem_bytes; /* ZERO only: bytes of one pixel, extra dims included */
+} ob_frame_field;
+
+typedef struct ob_frame_ops_io {
+    uint32_t n_frames, h, w;
+    int32_t predicate; /* ob_frame_predicate */
+    const ob_frame_field* fields; /* host table, any order, at most 512 entries per frame */
+    size_t n_fields;
+    double lower, upper, invalid;
+    const int32_t* pixel_shift_by_row; /* COLS: h entries, host memory */
+    const ob_lut* lut;                 /* XYZ_RANGE */
+    const void* poses;                 /* XYZ_RANGE, optional: n_frames x w x 16 of the LUT dtype */
+    int32_t axis;                      /* XYZ_*: 0, 1 or 2 */
+    int32_t reserved;
+} ob_frame_ops_io;
+
+/* errors: "unknown frame predicate", "unknown field role", "axis_idx must be in the range [0, 2]",
+ * "Frame dimensions do not match lut.", "range must be uint32", "points must be float32 or float64",
+ * "target field type is not a numeric pixel type" and the two above.  Launch family "frame_ops". */
+ob_status ob_frame_mask_fields(const ob_frame_ops_io* io, ob_stream* s);
+
+/* one selected-rows copy per entry: dst row k = src row rows[k], row_bytes each (extra dims included) */
+typedef struct ob_frame_rows_entry {
+    const void* src;
+    void* dst;
+    size_t row_bytes;
+    size_t src_rows;
+} ob_frame_rows_entry;
+
+typedef struct ob_frame_rows_io {
+    const ob_frame_rows_entry* entries; /* host table */
+    uint32_t n_entries;
+    uint32_t n_rows;       /* at most 2048 */
+    const uint32_t* rows;  /* host memory; each < src_rows of every entry */
+} ob_frame_rows_io;
+
+/* errors: "row index out of range", "too many rows for one call".  Launch family "frame_ops". */
+ob_status ob_frame_select_rows(const ob_frame_rows_io* io, ob_stream* s);
 
 /* ---- fused range -> (XYZ, destaggered range, destaggered XYZ), batched over frames ----
  * One launch performs, for every frame f and return r of the batch, what the reference does as

@@ -57,6 +57,12 @@ ob_status obh_sensor_destroy(obh_sensor* s);
 /* default field set of the sensor's profile and firmware (get_field_types(info)) */
 ob_status obh_frame_create(const obh_sensor* s, obh_frame** out);
 ob_status obh_frame_add_field(obh_frame* f, const char* name, int32_t ty_tag, size_t extra_dim);
+/* LidarFrame::add_field(name, type, extra_dims, field_class) (lidar_frame.h): field_class is a FieldClass
+ * (1 PIXEL_FIELD, 2 COLUMN_FIELD, 3 PACKET_FIELD, 4 FRAME_FIELD); extra_dim > 1 adds one trailing dimension */
+ob_status obh_frame_add_field_class(obh_frame* f, const char* name, int32_t ty_tag, size_t extra_dim,
+                                    int32_t field_class);
+/* class and shape of a field: *ndim dimensions into shape[0..min(*ndim, 8)) */
+ob_status obh_frame_field_shape(obh_frame* f, const char* name, int32_t* field_class, size_t* ndim, size_t* shape);
 size_t obh_frame_n_fields(const obh_frame* f);
 ob_status obh_frame_field_at(obh_frame* f, size_t i, char* name, size_t name_cap, int32_t* ty_tag,
                              size_t* elem_bytes /* incl. trailing dims */, void** data);

@@ -11,3 +11,4 @@ from .host import get_device, set_device  # noqa: F401,E402
 from .host import FrameBatcher, FramePipeline, PcapLidarSource, LidarFrame, LidarScan, ScanBatcher, SensorInfo, frame_to_packets  # noqa: F401,E402
 from . import sharding  # noqa: F401,E402
 from . import pyapi  # noqa: F401,E402
+from . import frame_ops  # noqa: F401,E402

@@ -137,6 +137,34 @@ class ImageState(C.Structure):
                 ("counter", C.c_int32), ("initialized", C.c_int32), ("dark_count_rows", u32), ("reserved", u32)]
 
 
+OB_FRAME_CLIP, OB_FRAME_VALUE, OB_FRAME_ROWS, OB_FRAME_COLS, OB_FRAME_XYZ_RANGE, OB_FRAME_XYZ_POINTS = range(6)
+OB_FRAME_TARGET, OB_FRAME_TARGET2, OB_FRAME_ZERO, OB_FRAME_SOURCE, OB_FRAME_SOURCE2 = range(5)
+
+
+class FrameField(C.Structure):
+    """ob_frame_field"""
+    _fields_ = [("data", vp), ("type", C.c_int32), ("role", C.c_int32), ("frame", u32), ("elem_bytes", u32)]
+
+
+class FrameOpsIO(C.Structure):
+    """ob_frame_ops_io"""
+    _fields_ = [("n_frames", u32), ("h", u32), ("w", u32), ("predicate", C.c_int32), ("fields", C.POINTER(FrameField)),
+                ("n_fields", sz), ("lower", C.c_double), ("upper", C.c_double), ("invalid", C.c_double),
+                ("pixel_shift_by_row", C.POINTER(C.c_int32)), ("lut", vp), ("poses", vp), ("axis", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
+class FrameRowsEntry(C.Structure):
+    """ob_frame_rows_entry"""
+    _fields_ = [("src", vp), ("dst", vp), ("row_bytes", sz), ("src_rows", sz)]
+
+
+class FrameRowsIO(C.Structure):
+    """ob_frame_rows_io"""
+    _fields_ = [("entries", C.POINTER(FrameRowsEntry)), ("n_entries", u32), ("n_rows", u32),
+                ("rows", C.POINTER(u32))]
+
+
 class DewarpFramesIO(C.Structure):
     _fields_ = [("lut", vp), ("range", vp), ("poses", vp), ("status", vp), ("timestamps", vp)]
 
@@ -239,6 +267,8 @@ _sig("ob_image_proc_create", i32, i32, i32, C.POINTER(ImageParams), C.POINTER(vp
 _sig("ob_image_proc_update", i32, vp, i32, i32, vp, vp, u32, u32, i32, vp)
 _sig("ob_image_proc_state", i32, vp, C.POINTER(ImageState), vp, sz, vp)
 _sig("ob_image_proc_destroy", i32, vp)
+_sig("ob_frame_mask_fields", i32, C.POINTER(FrameOpsIO), vp)
+_sig("ob_frame_select_rows", i32, C.POINTER(FrameRowsIO), vp)
 _sig("ob_dewarp_frames", i32, C.POINTER(DewarpFramesIO), sz, C.c_double, C.c_double, vp, sz, vp, vp, vp,
      C.POINTER(sz), C.POINTER(sz), vp)
 if hasattr(lib, "ob_decoder_create"):

@@ -18,7 +18,8 @@ static std::atomic<uint64_t> g_launches{0};
 
 static std::atomic<uint64_t> g_family[OB_FAM_COUNT];
 static const char* const kFamilies[OB_FAM_COUNT] = {"decode_pipe", "decode", "cloud", "normals", "voxel",
-                                                    "voxel_map", "icp", "align", "zone", "image"};
+                                                    "voxel_map", "icp", "align", "zone", "image",
+                                                    "frame_ops"};
 
 void count_launch(uint64_t n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 void count_launch_of(int family, uint64_t n) {
@@ -347,6 +348,10 @@ size_t ob_abi_sizeof(const char* name) {
     if (n == "ob_zone_state") return sizeof(ob_zone_state);
     if (n == "ob_image_params") return sizeof(ob_image_params);
     if (n == "ob_image_state") return sizeof(ob_image_state);
+    if (n == "ob_frame_field") return sizeof(ob_frame_field);
+    if (n == "ob_frame_ops_io") return sizeof(ob_frame_ops_io);
+    if (n == "ob_frame_rows_entry") return sizeof(ob_frame_rows_entry);
+    if (n == "ob_frame_rows_io") return sizeof(ob_frame_rows_io);
     return 0;
 }
 

@@ -34,6 +34,8 @@ _sig("obh_sensor_calculate_crc", u64, vp, vp, sz)
 _sig("obh_sensor_destroy", i32, vp)
 _sig("obh_frame_create", i32, vp, PP(vp))
 _sig("obh_frame_add_field", i32, vp, C.c_char_p, C.c_int32, sz)
+_sig("obh_frame_add_field_class", i32, vp, C.c_char_p, C.c_int32, sz, C.c_int32)
+_sig("obh_frame_field_shape", i32, vp, C.c_char_p, PP(C.c_int32), PP(sz), PP(sz))
 _sig("obh_frame_n_fields", sz, vp)
 _sig("obh_frame_field_at", i32, vp, sz, C.c_char_p, sz, PP(C.c_int32), PP(sz), PP(vp))
 _sig("obh_frame_field", i32, vp, C.c_char_p, PP(C.c_int32), PP(sz), PP(vp))
@@ -114,7 +116,7 @@ class SensorInfo:
     """SensorInfo + PacketFormat of one sensor stream."""
 
     def __init__(self, profile, h, w, columns_per_packet=16, header_type="STANDARD",
-                 pixel_shift_by_row=None, init_id=0, sn=0, fw_rev="UNKNOWN", column_window=None):
+                 pixel_shift_by_row=None, init_id=0, sn=0, fw_rev="UNKNOWN", column_window=None, prod_line=""):
         cw = column_window or (0, w - 1)
         sh = None
         if pixel_shift_by_row is not None:
@@ -129,13 +131,15 @@ class SensorInfo:
         self.profile, self.h, self.w, self.columns_per_packet = profile, h, w, columns_per_packet
         self.pixel_shift_by_row = sh if sh is not None else np.zeros(h, np.int32)
         self.init_id, self.sn = init_id, sn
+        self.header_type, self.fw_rev, self.column_window = header_type, fw_rev, tuple(cw)
+        self.prod_line = prod_line
 
     @classmethod
     def from_meta(cls, meta, fw_rev="UNKNOWN"):
         """From a tests/golden/*.json fixture dict."""
         s = cls(meta["profile"], meta["h"], meta["w"], meta["columns_per_packet"], meta["header_type"],
                 meta["pixel_shift_by_row"], meta["init_id"], meta["prod_sn"], fw_rev,
-                tuple(meta["column_window"]))
+                tuple(meta["column_window"]), meta.get("prod_line", ""))
         s.set_intrinsics(meta["beam_azimuth_angles"], meta["beam_altitude_angles"],
                          meta["beam_to_lidar_transform"], meta["lidar_to_sensor_transform"])
         return s
@@ -233,6 +237,7 @@ class LidarFrame:
             hd = vp(_borrowed)
             self._owned = False
         self._h, self.info = hd, info
+        self.sensor_info = info   # None for a frame selected without update_metadata (frame_ops)
         ts, mid, st, pts, af = vp(), vp(), vp(), vp(), vp()
         w, h, npk = sz(), sz(), sz()
         check(lib.obh_frame_headers(hd, C.byref(ts), C.byref(mid), C.byref(st), C.byref(pts), C.byref(af),
@@ -260,8 +265,27 @@ class LidarFrame:
             raise RuntimeError("No valid columns in LidarFrame")
         return b.value
 
-    def add_field(self, name, dtype, extra_dim=1):
-        check(lib.obh_frame_add_field(self._h, name.encode(), NP_TAG[np.dtype(dtype)], extra_dim))
+    def add_field(self, name, dtype, extra_dim=1, tag=None, field_class=1):
+        """`tag`: a ChanFieldType tag for types numpy does not name (12: FLOAT16, stored as uint16 bits);
+        `field_class`: a FieldClass (1 PIXEL_FIELD, 2 COLUMN_FIELD, 3 PACKET_FIELD, 4 FRAME_FIELD)."""
+        check(lib.obh_frame_add_field_class(self._h, name.encode(),
+                                            NP_TAG[np.dtype(dtype)] if tag is None else int(tag), extra_dim,
+                                            int(field_class)))
+
+    def field_class(self, name):
+        """FieldClass of a field (1 PIXEL_FIELD, 2 COLUMN_FIELD, 3 PACKET_FIELD, 4 FRAME_FIELD)."""
+        return self._shape(name)[0]
+
+    def _shape(self, name):
+        cls, nd, shp = C.c_int32(), sz(), (sz * 8)()
+        check(lib.obh_frame_field_shape(self._h, name.encode(), C.byref(cls), C.byref(nd), shp))
+        return cls.value, tuple(shp[i] for i in range(min(nd.value, 8)))
+
+    def field_tag(self, name):
+        """ChanFieldType tag of a field."""
+        tag = C.c_int32()
+        check(lib.obh_frame_field(self._h, name.encode(), C.byref(tag), None, None))
+        return tag.value
 
     @property
     def fields(self):
@@ -278,10 +302,8 @@ class LidarFrame:
     def field(self, name):
         tag, eb, data = C.c_int32(), sz(), vp()
         check(lib.obh_frame_field(self._h, name.encode(), C.byref(tag), C.byref(eb), C.byref(data)))
-        dt = np.dtype(TAG_NP[tag.value])
-        k = eb.value // dt.itemsize
-        shape = (self.h, self.w) if k == 1 else (self.h, self.w, k)
-        return _as_array(data.value, dt, shape)
+        dt = np.dtype(TAG_NP.get(tag.value, np.uint8))
+        return _as_array(data.value, dt, self._shape(name)[1])
 
     @property
     def frame_id(self):

@@ -224,6 +224,27 @@ ob_status obh_frame_add_field(obh_frame* f, const char* name, int32_t tag, size_
     });
 }
 
+ob_status obh_frame_add_field_class(obh_frame* f, const char* name, int32_t tag, size_t extra, int32_t cls) {
+    return guard([&] {
+        if (!f || !name) throw std::invalid_argument("null pointer");
+        if (cls < 1 || cls > 4) throw std::invalid_argument("unknown field class");
+        std::vector<size_t> ed;
+        if (extra > 1) ed.push_back(extra);
+        f->ref().add_field(name, static_cast<ChanFieldType>(tag), ed, static_cast<FieldClass>(cls));
+    });
+}
+
+ob_status obh_frame_field_shape(obh_frame* f, const char* name, int32_t* cls, size_t* ndim, size_t* shape) {
+    return guard([&] {
+        if (!f || !name) throw std::invalid_argument("null pointer");
+        const Field& fld = f->ref().field(name);
+        if (cls) *cls = static_cast<int32_t>(f->ref().field_type(name).field_class);
+        if (ndim) *ndim = fld.shape().size();
+        if (shape)
+            for (size_t i = 0; i < fld.shape().size() && i < 8; ++i) shape[i] = fld.shape()[i];
+    });
+}
+
 size_t obh_frame_n_fields(const obh_frame* f) { return f ? f->ref().fields().size() : 0; }
 
 ob_status obh_frame_field_at(obh_frame* f, size_t i, char* name, size_t cap, int32_t* tag,

@@ -339,4 +339,37 @@ for kind, ref in (("auto_exposure", oimg.AutoExposure()), ("local_tone_map", oim
     src = ri.uniform(0, 1, (12, 96, 3)).astype(np.float16)
     assert np.array_equal(proc.update(src), ref.update(src), equal_nan=True)
 print("image ok")
+# frame operations: every predicate of the masked write (aligned and ragged runs) and the row gather
+import json
+from oracle import frame_ops as ofo
+FIX32 = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden",
+                     "OS-1-32-G_v2.1.1_1024x10.json")
+rf = np.random.default_rng(17)
+for h, w in ((3, 37), (4, 64)):
+    si = ob.SensorInfo("RNG19_RFL8_SIG16_NIR16_DUAL", h, w, 1, pixel_shift_by_row=rf.integers(-5, 6, h))
+    for op in ("clip", "filter_field", "u", "v", "mask"):
+        fr = ob.LidarFrame(si)
+        for n in fr.fields:
+            fr.field(n)[...] = rf.integers(0, 200, fr.field(n).shape).astype(fr.field(n).dtype)
+        o = ofo.Frame(h, w, si.pixel_shift_by_row)
+        for n in fr.fields:
+            o.add(n, fr.field(n).copy(), fr.field_tag(n))
+        m = (rf.random((h, w)) < 0.5).astype(np.uint8)
+        {"clip": lambda f, mod: mod.clip(f, [], 20, 150, 1),
+         "filter_field": lambda f, mod: mod.filter_field(f, "RANGE", 20, 150),
+         "u": lambda f, mod: mod.filter_uv(f, "u", 1, 2), "v": lambda f, mod: mod.filter_uv(f, "v", 3, 9),
+         "mask": lambda f, mod: mod.mask(f, [], m)}[op](fr, ob.frame_ops)
+        {"clip": lambda f: ofo.clip(f, [], 20, 150, 1), "filter_field": lambda f: ofo.filter_field(f, "RANGE", 20, 150),
+         "u": lambda f: ofo.filter_uv(f, "u", 1, 2), "v": lambda f: ofo.filter_uv(f, "v", 3, 9),
+         "mask": lambda f: ofo.mask(f, [], m)}[op](o)
+        for n in fr.fields:
+            assert np.array_equal(fr.field(n), o.field(n)), (op, n)
+    sel = ob.frame_ops.select_by_index(fr, [h - 1, 0])
+    assert np.array_equal(sel.field("RANGE"), fr.field("RANGE")[[h - 1, 0]])
+si32 = ob.SensorInfo.from_meta(json.load(open(FIX32)))
+lut = ob.pyapi.XYZLutFloat(si32)
+fr32 = ob.LidarFrame(si32)
+fr32.field("RANGE")[...] = rf.integers(0, 20000, fr32.field("RANGE").shape)
+ob.frame_ops.filter_xyz(fr32, lut, 2, -0.2, 0.2, dewarp_points=True)
+print("frame ops ok")
 print("SANITIZE CASES OK")
