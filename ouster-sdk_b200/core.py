@@ -4,7 +4,8 @@ Reference interfaces mirrored (python binding python/src/cpp/client/processing.c
   XYZLut / XYZLutFloat .__call__(range|frame)   :340-357, 640-700
   destagger(info|shifts, field, inverse)         :527-638
 Arrays may be numpy arrays (host) or torch tensors (host or CUDA); CUDA tensors are used
-in place (zero copy), host arrays are staged by the C library.
+in place (zero copy), host arrays are staged by the C library.  A call given no `stream=` runs on
+the torch current stream when its data are CUDA tensors, else on the library's stream (_stream_for).
 """
 import ctypes as C
 
@@ -60,22 +61,59 @@ def _np_dtype(x):
     return x.dtype
 
 
-class PinnedBuffer:
+def _contig(a, dtype=None, floats=False):
+    """`a` (numpy array or torch tensor) made contiguous in its own memory.  dtype: a numpy dtype to convert to; a
+    torch tensor is converted only to a floating dtype, since device data carries unsigned integers in signed
+    tensors of the same width.  floats: float32 and float64 stay, anything else becomes float64."""
+    if _is_torch(a):
+        import torch
+        if floats and a.dtype not in (torch.float32, torch.float64):
+            a = a.double()
+        elif dtype is not None and np.dtype(dtype).kind == "f":
+            a = a.to(getattr(torch, np.dtype(dtype).name))
+        return a.contiguous()
+    a = np.ascontiguousarray(a, dtype)
+    return a.astype(np.float64) if floats and a.dtype not in (np.float32, np.float64) else a
+
+
+def _empty(ref, shape, dtype, fill=None):
+    """Output of a call on `ref`: a torch tensor on ref's device when ref is a CUDA tensor, else a numpy array, of
+    numpy `dtype` (unsigned integers wider than a byte come as the signed torch type of the same width: same bits),
+    filled with `fill` when given."""
+    dtype = np.dtype(dtype)
+    if _is_torch(ref) and ref.is_cuda:
+        import torch
+        tdt = getattr(torch, dtype.name[1:] if dtype.kind == "u" and dtype.itemsize > 1 else dtype.name)
+        if fill is None:
+            return torch.empty(shape, dtype=tdt, device=ref.device)
+        return torch.full(shape, fill, dtype=tdt, device=ref.device)
+    return np.empty(shape, dtype) if fill is None else np.full(shape, fill, dtype)
+
+
+class _Handle:
+    """Base of the objects that own a C handle: when one is collected, the C function named by `_release` frees the
+    handle held in the attribute named by `_handle`.  An object that only borrows its handle sets `_owned = False`."""
+    _release, _handle, _owned = None, "_h", True
+
+    def __del__(self):
+        h = getattr(self, self._handle, None)
+        if h and self._owned and lib is not None:
+            try:
+                getattr(lib, self._release)(h)
+            except Exception:
+                pass
+            setattr(self, self._handle, None)
+
+
+class PinnedBuffer(_Handle):
     """numpy view over cudaHostAlloc'd memory (ob_host_alloc)."""
+    _release, _handle = "ob_host_free", "ptr"
 
     def __init__(self, nbytes):
         p = C.c_void_p()
         check(lib.ob_host_alloc(nbytes, C.byref(p)))
         self.ptr, self.nbytes = p.value, nbytes
         self.raw = np.ctypeslib.as_array((C.c_uint8 * nbytes).from_address(p.value))
-
-    def __del__(self):
-        if getattr(self, "ptr", None) and lib is not None:
-            try:
-                lib.ob_host_free(self.ptr)
-            except Exception:
-                pass
-            self.ptr = None
 
 
 def pinned_empty(shape, dtype):
@@ -96,8 +134,9 @@ class _Holder:
         _Holder._keep.append(buf)  # pinned buffers live for the process (few, large)
 
 
-class Stream:
+class Stream(_Handle):
     """ob_stream: CUDA stream + staging; one per caller thread / sensor stream."""
+    _release, _handle = "ob_stream_destroy", "h"
 
     def __init__(self, device=0, cuda_stream=None):
         h = C.c_void_p()
@@ -114,16 +153,9 @@ class Stream:
     def sync(self):
         check(lib.ob_stream_sync(self.h))
 
-    def __del__(self):
-        if getattr(self, "h", None) and lib is not None:
-            try:
-                lib.ob_stream_destroy(self.h)
-            except Exception:
-                pass
-            self.h = None
-
 
 _default_streams = {}
+_torch_streams = {}
 
 
 def _stream(stream, device=0):
@@ -134,10 +166,26 @@ def _stream(stream, device=0):
     return _default_streams[device]
 
 
-class XYZLutT:
+def _stream_for(x=None, stream=None, device=0):
+    """The stream a call on `x` runs on: `stream` when given; for a CUDA tensor, the torch current stream of its
+    device, so the call is ordered after the torch work that wrote `x`; otherwise the library's stream of `device`.
+    A torch stream is wrapped once per (device, stream) and the wrapper kept: wrapping configures the device's
+    memory pool, which a CUDA graph capture must not see, so a captured call reuses the wrapper an earlier call on
+    that stream made."""
+    if stream is None and _is_torch(x) and x.is_cuda:
+        import torch
+        key = (x.device.index, torch.cuda.current_stream(x.device).cuda_stream)
+        if key not in _torch_streams:
+            _torch_streams[key] = Stream(*key)
+        return _torch_streams[key]
+    return _stream(stream, device)
+
+
+class XYZLutT(_Handle):
     """XYZLutT<T> (ouster_core/include/ouster/core/xyzlut.h:76-158) with device-resident tables.
 
     `direction`/`offset` are fetched lazily from the device (the reference keeps host copies)."""
+    _release = "ob_lut_destroy"
 
     def __init__(self, handle, h, w, dtype, device):
         self._h, self.h, self.w, self.dtype, self.device = handle, h, w, np.dtype(dtype), device
@@ -225,14 +273,6 @@ class XYZLutT:
         """lut(range) -> (h*w, 3) points, staggered order (xyzlut.h:139-150)."""
         return cartesian(self, rng, out=out, stream=stream)
 
-    def __del__(self):
-        if getattr(self, "_h", None) and lib is not None:
-            try:
-                lib.ob_lut_destroy(self._h)
-            except Exception:
-                pass
-            self._h = None
-
 
 def XYZLut(info, use_extrinsics=True, device=0):
     """Python `XYZLut` (double), python/src/cpp/client/processing.cpp:640-700."""
@@ -251,7 +291,6 @@ def _numel(x):
 def cartesian(lut, rng, out=None, stream=None):
     """cartesian(range, lut) / lut(range).  Raises ValueError("unexpected image dimensions")
     on size mismatch (ouster_core/src/xyzlut.cpp:117-119)."""
-    st = _stream(stream, lut.device)
     if _np_dtype(rng) != np.dtype(np.uint32):
         if _is_torch(rng):
             raise ValueError("range must be uint32")
@@ -259,12 +298,8 @@ def cartesian(lut, rng, out=None, stream=None):
     n = _numel(rng)
     own = out is None
     if own:
-        if _is_torch(rng) and rng.is_cuda:
-            import torch
-            out = torch.empty((n, 3), dtype=torch.float64 if lut.dtype == np.float64 else torch.float32,
-                              device=rng.device)
-        else:
-            out = np.empty((n, 3), lut.dtype)
+        out = _empty(rng, (n, 3), lut.dtype)
+    st = _stream_for(rng, stream, lut.device)
     check(lib.ob_cartesian(lut._h, _ptr(rng), n, _ptr(out), st.h))
     if own and not (_is_torch(out) and out.is_cuda):
         st.sync()
@@ -274,7 +309,6 @@ def cartesian(lut, rng, out=None, stream=None):
 def destagger(img, pixel_shift_by_row, inverse=False, out=None, stream=None, device=0):
     """destagger<T>(img, pixel_shift_by_row, inverse) for (H,W) or (H,W,...) images
     (ouster_core/include/ouster/core/impl/lidar_frame_impl.h:733-860)."""
-    st = _stream(stream, device)
     shape = tuple(img.shape)
     if len(shape) < 2:
         raise ValueError("image must be at least 2-dimensional")
@@ -289,6 +323,7 @@ def destagger(img, pixel_shift_by_row, inverse=False, out=None, stream=None, dev
         else:
             img = np.ascontiguousarray(img)
             out = np.empty_like(img)
+    st = _stream_for(img, stream, device)
     check(lib.ob_destagger(_itemsize(img), k, _ptr(img), sh.ctypes.data, sh.size, h, w,
                            int(bool(inverse)), _ptr(out), st.h))
     if own and not (_is_torch(out) and out.is_cuda):
@@ -299,7 +334,6 @@ def destagger(img, pixel_shift_by_row, inverse=False, out=None, stream=None, dev
 def dewarp(points, poses, out=None, stream=None, device=0):
     """dewarp(points (H, W, 3), poses (W, 4, 4)) -> (H, W, 3): per-column pose application
     (python/src/cpp/client/processing.cpp:132-161; pose_util.h:37-59).  float32 or float64."""
-    st = _stream(stream, device)
     dt = _np_dtype(points)
     if dt not in (np.dtype(np.float32), np.dtype(np.float64)):
         raise ValueError("points must be float32 or float64")
@@ -317,6 +351,7 @@ def dewarp(points, poses, out=None, stream=None, device=0):
         else:
             points = np.ascontiguousarray(points)
             out = np.empty_like(points)
+    st = _stream_for(points, stream, device)
     status = lib.ob_dewarp(_capi.OB_F64 if dt == np.float64 else _capi.OB_F32, _ptr(points), _ptr(poses),
                            n_points, n_poses, _ptr(out), st.h)
     if status == _capi.OB_RUNTIME_ERROR:
@@ -338,15 +373,12 @@ def dewarp_frame(lut, rng, poses, status, timestamps=None, min_range=0.0, max_ra
     tensor [1] (inputs in device memory too): nothing waits for the GPU; returns (out, out_count), the count
     being written in stream order (a count above the capacity means the list was cut there)."""
     from ._capi import DewarpFrameIO
-    st = _stream(stream, lut.device)
     n_px = lut.h * lut.w
     if _numel(rng) != n_px:
         raise ValueError("unexpected image dimensions")
     if max_range == float("inf"):
         max_range = 4294967.295
-    rng = rng if _is_torch(rng) else np.ascontiguousarray(rng, np.uint32)
-    poses = poses if _is_torch(poses) else np.ascontiguousarray(poses, np.float64)
-    status = status if _is_torch(status) else np.ascontiguousarray(status, np.uint32)
+    rng, poses, status = _contig(rng, np.uint32), _contig(poses, np.float64), _contig(status, np.uint32)
     if _numel(poses) != lut.w * 16 or _numel(status) != lut.w:
         raise ValueError("poses must be [W, 4, 4] and status [W]")
     io = DewarpFrameIO()
@@ -356,6 +388,7 @@ def dewarp_frame(lut, rng, poses, status, timestamps=None, min_range=0.0, max_ra
         if out_count is None or provenance:
             raise ValueError("the asynchronous form takes out= and out_count= (device tensors) and no provenance")
         io.points, io.capacity = _ptr(out), _numel(out) // 3
+        st = _stream_for(rng, stream, lut.device)
         check(lib.ob_dewarp_frame(lut._h, C.byref(io), C.cast(_ptr(out_count), C.POINTER(C.c_size_t)), st.h))
         return out, out_count
     pts = np.empty((n_px, 3), lut.dtype)
@@ -364,10 +397,11 @@ def dewarp_frame(lut, rng, poses, status, timestamps=None, min_range=0.0, max_ra
     if provenance:
         if timestamps is None:
             raise ValueError("provenance needs the column timestamps")
-        timestamps = timestamps if _is_torch(timestamps) else np.ascontiguousarray(timestamps, np.uint64)
+        timestamps = _contig(timestamps, np.uint64)
         ci, ts_out = np.empty(n_px, np.uint32), np.empty(n_px, np.uint64)
         io.timestamps, io.col_idx, io.timestamps_out = _ptr(timestamps), ci.ctypes.data, ts_out.ctypes.data
     n = C.c_size_t(0)
+    st = _stream_for(rng, stream, lut.device)
     check(lib.ob_dewarp_frame(lut._h, C.byref(io), C.byref(n), st.h))
     if provenance:
         return pts[:n.value], ci[:n.value], ts_out[:n.value]
@@ -400,7 +434,6 @@ def normals(xyz, rng, *args, sensor_origins_xyz=None, pixel_search_range=1,
           "min_angle_of_incidence_rad": min_angle_of_incidence_rad, "target_distance_m": target_distance_m}
     for nm, v in zip(names, pos):
         kw[nm] = v
-    st = _stream(stream, device)
     if len(rng.shape) != 2:
         raise RuntimeError("normals: xyz dimensions mismatch")
     h, w = int(rng.shape[0]), int(rng.shape[1])
@@ -427,16 +460,7 @@ def normals(xyz, rng, *args, sensor_origins_xyz=None, pixel_search_range=1,
         raise TypeError("normals(): incompatible function arguments (sensor_origins_xyz must be (W, 3))")
     if org.shape[0] != w:
         raise RuntimeError("normals: sensor_origins size must match image width")
-
-    def prep_rng(a):
-        if _is_torch(a):
-            return a
-        return np.ascontiguousarray(a, np.uint32)
-
-    def prep_xyz(a):
-        return a if _is_torch(a) else np.ascontiguousarray(a)
-
-    xyz, rng = prep_xyz(xyz), prep_rng(rng)
+    xyz, rng = _contig(xyz), _contig(rng, np.uint32)
     on_dev = _is_torch(xyz) and xyz.is_cuda
 
     def new_out():
@@ -451,7 +475,7 @@ def normals(xyz, rng, *args, sensor_origins_xyz=None, pixel_search_range=1,
     io.xyz, io.range, io.normals = _ptr(xyz), _ptr(rng), _ptr(n1)
     n2 = None
     if dual:
-        xyz2, range2 = prep_xyz(xyz2), prep_rng(range2)
+        xyz2, range2 = _contig(xyz2), _contig(range2, np.uint32)
         n2 = new_out()
         io.xyz2, io.range2, io.normals2 = _ptr(xyz2), _ptr(range2), _ptr(n2)
     io.sensor_origins_xyz, io.n_origins = _ptr(org), w
@@ -461,6 +485,7 @@ def normals(xyz, rng, *args, sensor_origins_xyz=None, pixel_search_range=1,
     io.vertical_subtent_rad = float(vertical_subtent)
     sub = np.zeros(1, np.float64)
     io.vertical_subtent_out = sub.ctypes.data
+    st = _stream_for(xyz, stream, device)
     status = lib.ob_normals(_capi.OB_F64 if dt == np.float64 else _capi.OB_F32, C.byref(io), st.h)
     if status == _capi.OB_RUNTIME_ERROR:
         raise RuntimeError(lib.ob_last_error().decode())
@@ -491,16 +516,7 @@ def voxel_downsample(points, voxel_size, mode="shuffle_first", normals=None, max
     a CUDA int64 [1] count of the valid rows, appended to the tuple.  ValueError texts of the reference."""
     from ._capi import VoxelIO
     m = VOXEL_MODES[mode]
-    on_dev = _is_torch(points) and points.is_cuda
-
-    def prep(a):
-        if _is_torch(a):
-            import torch
-            return (a if a.dtype in (torch.float32, torch.float64) else a.double()).contiguous()
-        a = np.ascontiguousarray(a)
-        return a if a.dtype in (np.float32, np.float64) else a.astype(np.float64)
-
-    points = prep(points)
+    points = _contig(points, floats=True)
     if len(points.shape) != 2:
         raise ValueError("points must be [n, cols]")
     rows, cols = int(points.shape[0]), int(points.shape[1])
@@ -509,27 +525,18 @@ def voxel_downsample(points, voxel_size, mode="shuffle_first", normals=None, max
     if m == _capi.OB_VOXEL_POINT_NORMAL:
         if normals is None:
             raise ValueError("point_normal needs normals")
-        nrm = prep(normals)
+        nrm = _contig(normals, floats=True)
         if _np_dtype(nrm) != dt:
-            nrm = nrm.to(points.dtype) if _is_torch(nrm) else nrm.astype(dt)
+            nrm = _contig(nrm, dt)
         if tuple(nrm.shape) != (rows, 3) or cols != 3:
             raise ValueError("voxel_downsample_with_normals expects Nx3 inputs" if cols != 3 or nrm.shape[-1] != 3
                              else "voxel_downsample_with_normals points/normals size mismatch")
+    if n is not None and not (_is_torch(points) and points.is_cuda):
+        raise ValueError("a device-side row count needs device inputs")
     out_cols = 3 if m == _capi.OB_VOXEL_POINT_NORMAL else cols
-    if on_dev:
-        import torch
-        dev = points.device
-        st = stream or Stream(dev.index, cuda_stream=torch.cuda.current_stream(dev).cuda_stream)
-        out = torch.empty((rows, out_cols), dtype=torch.float64, device=dev)
-        out_n = torch.empty((rows, 3), dtype=torch.float64, device=dev) if nrm is not None else None
-        idx = torch.empty(rows, dtype=torch.int32, device=dev)
-    else:
-        if n is not None:
-            raise ValueError("a device-side row count needs device inputs")
-        st = _stream(stream, device)
-        out = np.empty((rows, out_cols), np.float64)
-        out_n = np.empty((rows, 3), np.float64) if nrm is not None else None
-        idx = np.empty(rows, np.uint32)
+    out = _empty(points, (rows, out_cols), np.float64)
+    out_n = _empty(points, (rows, 3), np.float64) if nrm is not None else None
+    idx = _empty(points, (rows,), np.uint32)
     io = VoxelIO()
     io.mode, io.dtype = m, _capi.OB_F64 if dt == np.float64 else _capi.OB_F32
     io.points, io.cols, io.normals = _ptr(points), cols, _ptr(nrm)
@@ -543,11 +550,11 @@ def voxel_downsample(points, voxel_size, mode="shuffle_first", normals=None, max
             raise ValueError("n must be a CUDA int64 tensor with one element")
         count = torch.zeros(1, dtype=torch.int64, device=points.device)
         io.n_device, io.capacity, io.n_out = n.data_ptr(), rows, count.data_ptr()
-        check(lib.ob_voxel_downsample(C.byref(io), st.h))
+        check(lib.ob_voxel_downsample(C.byref(io), _stream_for(points, stream, device).h))
         return head + (count,)
     cnt = C.c_size_t(0)
     io.n, io.n_out = rows, C.addressof(cnt)
-    check(lib.ob_voxel_downsample(C.byref(io), st.h))
+    check(lib.ob_voxel_downsample(C.byref(io), _stream_for(points, stream, device).h))
     k = cnt.value
     return tuple(a[:k] for a in head)
 
@@ -555,24 +562,11 @@ def voxel_downsample(points, voxel_size, mode="shuffle_first", normals=None, max
 DBL_MAX = float(np.finfo(np.float64).max)
 
 
-def _torch_stream(x, stream):
-    import torch
-    return stream or Stream(x.device.index, cuda_stream=torch.cuda.current_stream(x.device).cuda_stream)
-
-
 def _point_rows(points, n=None, what="add_points expects an Nx3 array"):
     """(PointRows, kept array) for [rows, 3] float32 / float64 points (numpy or torch); n: optional CUDA int64 [1]
     device-resident row count, then `points` holds `capacity` rows."""
     from ._capi import PointRows
-    if _is_torch(points):
-        import torch
-        if points.dtype not in (torch.float32, torch.float64):
-            points = points.double()
-        points = points.contiguous()
-    else:
-        points = np.ascontiguousarray(points)
-        if points.dtype not in (np.float32, np.float64):
-            points = points.astype(np.float64)
+    points = _contig(points, floats=True)
     if len(points.shape) != 2 or points.shape[1] != 3:
         raise ValueError(what)
     r = PointRows()
@@ -590,10 +584,11 @@ def _point_rows(points, n=None, what="add_points expects an Nx3 array"):
     return r, points
 
 
-class VoxelMap:
+class VoxelMap(_Handle):
     """Device-resident VoxelHashMap3d (ob_voxel_map, voxel_hash_map.cpp:14-247) with first_n_point insertion.
     Points may be numpy arrays or torch tensors (CUDA tensors stay on the device); results are float64.
     point_cloud() and the extracted rows list voxels in creation order (DESIGN 9)."""
+    _release = "ob_voxel_map_destroy"
 
     def __init__(self, voxel_size, max_distance=100.0, max_points_per_voxel=20, min_pts_threshold=1, device=0):
         h = C.c_void_p()
@@ -602,17 +597,6 @@ class VoxelMap:
         self._h, self.device = h, device
         self.voxel_size, self.max_distance = float(voxel_size), float(max_distance)
         self.max_points_per_voxel, self.min_pts_threshold = int(max_points_per_voxel), int(min_pts_threshold)
-
-    def __del__(self):
-        if getattr(self, "_h", None) and lib is not None:
-            try:
-                lib.ob_voxel_map_destroy(self._h)
-            except Exception:
-                pass
-            self._h = None
-
-    def _st(self, x, stream):
-        return _torch_stream(x, stream) if _is_torch(x) and x.is_cuda else _stream(stream, self.device)
 
     def clear(self, stream=None):
         check(lib.ob_voxel_map_clear(self._h, _stream(stream, self.device).h))
@@ -625,18 +609,13 @@ class VoxelMap:
 
     def add_points(self, points, n=None, stream=None):
         r, keep = _point_rows(points, n)
-        st = self._st(keep, stream)  # held: a wrapped stream is destroyed with its Python object
-        check(lib.ob_voxel_map_add_points(self._h, C.byref(r), st.h))
+        check(lib.ob_voxel_map_add_points(self._h, C.byref(r), _stream_for(keep, stream, self.device).h))
 
     def remove_far(self, origin, extract=False, stream=None):
         """remove_voxels_far_from_location(origin); extract=True returns the erased points (numpy [m, 3])."""
         from ._capi import VoxelMapCullIO
-        if _is_torch(origin):
-            org = origin.double().contiguous().reshape(3)
-            st = _torch_stream(org, stream) if org.is_cuda else _stream(stream, self.device)
-        else:
-            org = np.ascontiguousarray(origin, np.float64).reshape(3)
-            st = _stream(stream, self.device)
+        org = _contig(origin, np.float64).reshape(3)
+        st = _stream_for(org, stream, self.device)
         io = VoxelMapCullIO()
         io.origin = _ptr(org)
         if not extract:
@@ -670,15 +649,10 @@ class VoxelMap:
         from ._capi import VoxelQueryIO
         r, keep = _point_rows(points, n, "VoxelHashMap method expects a 3-element point")
         rows = int(keep.shape[0])
-        if _is_torch(keep) and keep.is_cuda:
-            import torch
-            nb = torch.zeros((rows, 3), dtype=torch.float64, device=keep.device)
-            d2 = torch.empty(rows, dtype=torch.float64, device=keep.device)
-        else:
-            nb, d2 = np.zeros((rows, 3), np.float64), np.empty(rows, np.float64)
+        nb, d2 = _empty(keep, (rows, 3), np.float64, fill=0), _empty(keep, (rows,), np.float64)
         io = VoxelQueryIO()
         io.queries, io.max_distance_sq, io.neighbors, io.distances_sq = r, float(max_distance_sq), _ptr(nb), _ptr(d2)
-        st = self._st(keep, stream)
+        st = _stream_for(keep, stream, self.device)
         check(lib.ob_voxel_map_closest_neighbors(self._h, C.byref(io), st.h))
         if not _is_torch(nb):
             st.sync()
@@ -695,19 +669,10 @@ def icp_align(voxel_map, source, max_distance, kernel_scale, max_num_iterations=
     io = IcpIO()
     io.source, io.max_distance, io.kernel_scale = r, float(max_distance), float(kernel_scale)
     io.max_num_iterations, io.convergence_criterion = int(max_num_iterations), float(convergence_criterion)
-    if _is_torch(keep) and keep.is_cuda:
-        import torch
-        pose = torch.empty((4, 4), dtype=torch.float64, device=keep.device)
-        it = torch.empty(1, dtype=torch.int32, device=keep.device)
-        io.pose, io.iterations = pose.data_ptr(), it.data_ptr()
-        st = _torch_stream(keep, stream)
-        check(lib.ob_icp_align(voxel_map._h, C.byref(io), st.h))
-        return pose, it
-    pose = np.empty((4, 4), np.float64)
-    it = C.c_int32(0)
-    io.pose, io.iterations = pose.ctypes.data, C.addressof(it)
-    check(lib.ob_icp_align(voxel_map._h, C.byref(io), _stream(stream, voxel_map.device).h))
-    return pose, it.value
+    pose, it = _empty(keep, (4, 4), np.float64), _empty(keep, (1,), np.int32)
+    io.pose, io.iterations = _ptr(pose), _ptr(it)
+    check(lib.ob_icp_align(voxel_map._h, C.byref(io), _stream_for(keep, stream, voxel_map.device).h))
+    return (pose, it) if _is_torch(it) else (pose, int(it[0]))
 
 
 def _align_arrays(points, normals, n, what):
@@ -717,11 +682,10 @@ def _align_arrays(points, normals, n, what):
         return r, keep, None
     if _is_torch(keep):
         import torch
-        nk = torch.as_tensor(normals, device=keep.device).to(keep.dtype).contiguous()
-    else:
-        if _is_torch(normals):
-            normals = normals.cpu().numpy()
-        nk = np.ascontiguousarray(normals, keep.dtype)
+        normals = torch.as_tensor(normals, device=keep.device)
+    elif _is_torch(normals):
+        normals = normals.cpu().numpy()
+    nk = _contig(normals, _np_dtype(keep))
     if len(nk.shape) != 2 or nk.shape[1] != 3:
         raise ValueError(f"{what} normals must be Nx3")
     return r, keep, nk
@@ -743,12 +707,7 @@ def cloud_align(source, target, source_normals=None, target_normals=None, initia
     if _is_torch(s) != _is_torch(t) or (_is_torch(s) and s.device != t.device):
         raise ValueError("source and target must live in the same memory")
     if s.dtype != t.dtype:  # the C ABI takes one dtype for both clouds
-        if _is_torch(s):
-            s, t = s.double(), t.double()
-            sn, tn = (None if sn is None else sn.double()), (None if tn is None else tn.double())
-        else:
-            s, t = s.astype(np.float64), t.astype(np.float64)
-            sn, tn = (None if sn is None else sn.astype(np.float64)), (None if tn is None else tn.astype(np.float64))
+        s, t, sn, tn = (None if a is None else _contig(a, np.float64) for a in (s, t, sn, tn))
         sr.dtype = tr.dtype = _capi.OB_F64
         sr.points, tr.points = _ptr(s), _ptr(t)
     # ob_cloud_align checks these too; here they also hold on a machine without a GPU (no stream to create yet)
@@ -770,27 +729,15 @@ def cloud_align(source, target, source_normals=None, target_normals=None, initia
         io.target_normals, io.target_normal_rows = _ptr(tn), int(tn.shape[0])
     g = None
     if initial_guess is not None:
-        if _is_torch(initial_guess):
-            g = initial_guess.double().contiguous()
-        else:
-            g = np.ascontiguousarray(initial_guess, np.float64)
+        g = _contig(initial_guess, np.float64)
         if _numel(g) != 16:
             raise ValueError("initial_guess must be 4x4")
         io.initial_guess = _ptr(g)
     io.max_corr_dist, io.max_normal_angle_deg = float(max_corr_dist), float(max_normal_angle_deg)
-    if _is_torch(s) and s.is_cuda:
-        import torch
-        pose = torch.empty((4, 4), dtype=torch.float64, device=s.device)
-        it = torch.empty(1, dtype=torch.int32, device=s.device)
-        io.pose, io.iterations = pose.data_ptr(), it.data_ptr()
-        st = _torch_stream(s, stream)
-        check(lib.ob_cloud_align(C.byref(io), st.h))
-        return pose, it
-    pose = np.empty((4, 4), np.float64)
-    it = C.c_int32(0)
-    io.pose, io.iterations = pose.ctypes.data, C.addressof(it)
-    check(lib.ob_cloud_align(C.byref(io), _stream(stream, 0).h))
-    return pose, it.value
+    pose, it = _empty(s, (4, 4), np.float64), _empty(s, (1,), np.int32)
+    io.pose, io.iterations = _ptr(pose), _ptr(it)
+    check(lib.ob_cloud_align(C.byref(io), _stream_for(s, stream).h))
+    return (pose, it) if _is_torch(it) else (pose, int(it[0]))
 
 
 def cloud_nearest(target, queries, cell_size, max_dist_sq, target_normals=None, n_target=None, n_queries=None,
@@ -804,25 +751,16 @@ def cloud_nearest(target, queries, cell_size, max_dist_sq, target_normals=None, 
     if _is_torch(t) != _is_torch(q) or (_is_torch(t) and t.device != q.device):
         raise ValueError("target and queries must live in the same memory")
     if t.dtype != q.dtype:
-        t, q = (t.double(), q.double()) if _is_torch(t) else (t.astype(np.float64), q.astype(np.float64))
-        tn = None if tn is None else (tn.double() if _is_torch(tn) else tn.astype(np.float64))
+        t, q, tn = (None if a is None else _contig(a, np.float64) for a in (t, q, tn))
         tr.dtype = qr.dtype = _capi.OB_F64
         tr.points, qr.points = _ptr(t), _ptr(q)
-    rows = int(q.shape[0])
     io = CloudNearestIO()
     io.target, io.queries = tr, qr
     io.target_normals = None if tn is None else _ptr(tn)
     io.cell_size, io.max_dist_sq = float(cell_size), float(max_dist_sq)
-    if _is_torch(q) and q.is_cuda:
-        import torch
-        out = torch.full((rows,), -1, dtype=torch.int32, device=q.device)
-        io.indices = out.data_ptr()
-        st = _torch_stream(q, stream)
-        check(lib.ob_cloud_nearest(C.byref(io), st.h))
-        return out
-    out = np.full(rows, -1, np.int32)
+    out = _empty(q, (int(q.shape[0]),), np.int32, fill=-1)
     io.indices = _ptr(out)
-    check(lib.ob_cloud_nearest(C.byref(io), _stream(stream, 0).h))
+    check(lib.ob_cloud_nearest(C.byref(io), _stream_for(q, stream).h))
     return out
 
 
@@ -830,10 +768,7 @@ def icp_linear_system(source, target, kernel_scale, stream=None, device=0):
     """build_linear_system(correspondences, kernel_scale) (icp_registration.cpp) on the GPU with the reference's
     deterministic-reduce tree: (jtj [6, 6], lower triangle, jtr [6]) float64 numpy arrays."""
     from ._capi import IcpSystemIO
-    def f64(a):  # the C ABI reads dense float64 rows
-        return a.double().contiguous() if _is_torch(a) else np.ascontiguousarray(a, np.float64)
-
-    s, t = f64(source), f64(target)
+    s, t = _contig(source, np.float64), _contig(target, np.float64)  # the C ABI reads dense float64 rows
     if tuple(s.shape) != tuple(t.shape) or len(s.shape) != 2 or s.shape[1] != 3:
         raise ValueError("source and target must both be [n, 3]")
     if _is_torch(s) != _is_torch(t) or (_is_torch(s) and s.device != t.device):
@@ -842,8 +777,7 @@ def icp_linear_system(source, target, kernel_scale, stream=None, device=0):
     io = IcpSystemIO()
     io.source, io.target, io.n, io.kernel_scale = _ptr(s), _ptr(t), int(s.shape[0]), float(kernel_scale)
     io.jtj, io.jtr = jtj.ctypes.data, jtr.ctypes.data
-    st = _torch_stream(s, stream) if _is_torch(s) and s.is_cuda else _stream(stream, device)
-    check(lib.ob_icp_linear_system(C.byref(io), st.h))
+    check(lib.ob_icp_linear_system(C.byref(io), _stream_for(s, stream, device).h))
     return jtj, jtr
 
 
@@ -862,9 +796,8 @@ def dewarp_frames(frames, min_range=0.0, max_range=float("inf"), provenance=Fals
             continue
         lut = fr["lut"]
         lut0 = lut0 or lut
-        rng = fr["range"] if _is_torch(fr["range"]) else np.ascontiguousarray(fr["range"], np.uint32)
-        poses = fr["poses"] if _is_torch(fr["poses"]) else np.ascontiguousarray(fr["poses"], np.float64)
-        status = fr["status"] if _is_torch(fr["status"]) else np.ascontiguousarray(fr["status"], np.uint32)
+        rng, poses, status = _contig(fr["range"], np.uint32), _contig(fr["poses"], np.float64), \
+            _contig(fr["status"], np.uint32)
         if _numel(rng) != lut.h * lut.w:
             raise ValueError("unexpected image dimensions")
         if _numel(poses) != lut.w * 16 or _numel(status) != lut.w:
@@ -873,7 +806,7 @@ def dewarp_frames(frames, min_range=0.0, max_range=float("inf"), provenance=Fals
         if provenance:
             if ts is None:
                 raise ValueError("provenance needs the column timestamps")
-            ts = ts if _is_torch(ts) else np.ascontiguousarray(ts, np.uint64)
+            ts = _contig(ts, np.uint64)
         keep += [rng, poses, status, ts]
         ios[i].lut, ios[i].range, ios[i].poses, ios[i].status = lut._h, _ptr(rng), _ptr(poses), _ptr(status)
         ios[i].timestamps = _ptr(ts) if provenance else None
@@ -956,7 +889,7 @@ def scan_to_cloud(lut, pixel_shift_by_row, rng, xyz=None, range_destaggered=None
     plan_scan_to_cloud(lut, pixel_shift_by_row, rng, xyz, range_destaggered, xyz_destaggered, stream, poses)()
 
 
-class Decoder:
+class Decoder(_Handle):
     """ob_decoder: device-side PacketFormat decode table.
 
     layout: dict with packet_header_size, col_header_size, channel_data_size, col_size,
@@ -965,6 +898,7 @@ class Decoder:
             (offset, mask, shift) tuples.
     fields: list of dicts {name, offset, mask, shift, elem_size, range_return, zero_pattern}.
     """
+    _release = "ob_decoder_destroy"
 
     def __init__(self, layout, fields, device=0):
         from ._capi import FieldDesc, PacketLayout
@@ -1111,14 +1045,6 @@ class Decoder:
                            pixel_shift_by_row, xyz, range_destaggered, timestamp, measurement_id, status,
                            stream, frame_luts)()
 
-    def __del__(self):
-        if getattr(self, "_h", None) and lib is not None:
-            try:
-                lib.ob_decoder_destroy(self._h)
-            except Exception:
-                pass
-            self._h = None
-
 
 # ---- zone monitoring (DESIGN f-8) -------------------------------------------------------------------------------
 ZONE_STATE_DTYPE = np.dtype([("live", np.uint8), ("id", np.uint8), ("error_flags", np.uint8),
@@ -1143,10 +1069,7 @@ def _lut_pair(lut, npx, what):
     d, o = lut
     keep = []
     for a in (d, o):
-        if _is_torch(a):
-            a = a.double().contiguous()
-        else:
-            a = np.ascontiguousarray(a, np.float64)
+        a = _contig(a, np.float64)
         if _numel(a) != npx * 3:
             raise ValueError(f"{what} must hold h*w*3 values")
         keep.append(a)
@@ -1179,17 +1102,14 @@ def zone_render(zones, h, w, sensor_lut, body_lut=None, device_out=None, stream=
     on_dev = [a for a in keep_s + keep_b if (isinstance(a, XYZLutT) or (_is_torch(a) and a.is_cuda))]
     if device_out is None:
         device_out = bool(on_dev)
-    shape = (len(zones), int(h), int(w))
+    ref = None  # an empty CUDA tensor on the output device when the images stay there
     if device_out:
         import torch
         dev = on_dev[0].device if on_dev else device
-        dev = torch.device("cuda", dev) if isinstance(dev, int) else dev
-        near = torch.empty(shape, dtype=torch.int32, device=dev)
-        far = torch.empty(shape, dtype=torch.int32, device=dev)
-        st = stream or Stream(dev.index, cuda_stream=torch.cuda.current_stream(dev).cuda_stream)
-    else:
-        near, far = np.empty(shape, np.uint32), np.empty(shape, np.uint32)
-        st = _stream(stream, device)
+        ref = torch.empty(0, device=torch.device("cuda", dev) if isinstance(dev, int) else dev)
+    shape = (len(zones), int(h), int(w))
+    near, far = _empty(ref, shape, np.uint32), _empty(ref, shape, np.uint32)
+    st = _stream_for(ref, stream, device)
     px = np.zeros(max(len(zones), 1), np.uint32)
     io = ZoneRenderIO()
     io.n_rows, io.n_cols = int(h), int(w)
@@ -1200,12 +1120,13 @@ def zone_render(zones, h, w, sensor_lut, body_lut=None, device_out=None, stream=
     return near, far, px[:len(zones)]
 
 
-class ZoneMonitor:
+class ZoneMonitor(_Handle):
     """Device-resident EmulatedZoneMon (ob_zone_monitor): up to 16 live zones' near/far images in HBM; update()
     runs _calc_counts and the trigger counters of one frame and leaves the 16 ZoneState records on the device.
 
     live: sequence of dicts with `id`, `mode`, `point_count`, `frame_count`, `near_mm`, `far_mm` ((h, w) uint32,
     numpy or CUDA) and optional initial `triggers` / `alerts`.  The slot of a zone (its bitmask bit) is its index."""
+    _release = "ob_zone_monitor_destroy"
 
     def __init__(self, live, h, w, device=0):
         from ._capi import ZoneLive
@@ -1215,8 +1136,7 @@ class ZoneMonitor:
         for i, z in enumerate(live):
             ims = []
             for k in ("near_mm", "far_mm"):
-                a = z[k]
-                a = a.contiguous() if _is_torch(a) else np.ascontiguousarray(a, np.uint32)
+                a = _contig(z[k], np.uint32)
                 if _numel(a) != int(h) * int(w):
                     raise ValueError("zone images must be h x w")
                 ims.append(a)
@@ -1229,26 +1149,6 @@ class ZoneMonitor:
         check(lib.ob_zone_monitor_create(device, int(h), int(w), arr, len(live), C.byref(hd)))
         self._h, self.h, self.w, self.n_live, self.device = hd, int(h), int(w), len(live), device
         self._st = None
-        self._wrapped = None
-
-    def __del__(self):
-        if getattr(self, "_h", None) and lib is not None:
-            try:
-                lib.ob_zone_monitor_destroy(self._h)
-            except Exception:
-                pass
-            self._h = None
-
-    def _stream_for(self, x, stream):
-        if stream is not None:
-            return stream
-        if _is_torch(x) and x.is_cuda:
-            import torch
-            h = torch.cuda.current_stream(x.device).cuda_stream
-            if self._wrapped is None or self._wrapped[0] != h:  # one wrapper per torch stream, reused per frame
-                self._wrapped = (h, Stream(x.device.index, cuda_stream=h))
-            return self._wrapped[1]
-        return _stream(None, self.device)
 
     def update(self, range_img, bitmask=None, stream=None):
         """calc_triggers(range, bitmask): range (h, w) uint32 (numpy, or a CUDA int32 / uint32 tensor such as K2's
@@ -1260,9 +1160,7 @@ class ZoneMonitor:
             import torch
             if range_img.dtype not in (torch.int32, torch.uint32):
                 raise ValueError("range must be uint32")
-            r = range_img.contiguous()
-        else:
-            r = np.ascontiguousarray(range_img, np.uint32)
+        r = _contig(range_img, np.uint32)
         if bitmask is not None:
             # written in place, so neither a copy nor a conversion will do
             if _is_torch(bitmask):
@@ -1273,8 +1171,7 @@ class ZoneMonitor:
                     bitmask.flags["C_CONTIGUOUS"]
             if not ok or _numel(bitmask) != self.h * self.w:
                 raise ValueError("bitmask must be a contiguous h x w uint32 / int32 array")
-        st = self._stream_for(r, stream)
-        self._st = st
+        st = self._st = _stream_for(r, stream, self.device)
         check(lib.ob_zone_monitor_update(self._h, _ptr(r), None if bitmask is None else _ptr(bitmask), st.h))
 
     def states(self, device=False, stream=None):
@@ -1301,11 +1198,12 @@ class ZoneMonitor:
                 [int(v) for v in r[:self.n_live]])
 
 
-class ImageProcessor:
+class ImageProcessor(_Handle):
     """Device-resident image post-processor (ob_image_proc): one AutoExposure, BeamUniformityCorrector or
     LocalToneMapper with its state in device memory.  kind: "auto_exposure", "beam_uniformity" or
     "local_tone_map"; the keyword arguments are the constructor's (ignored by beam_uniformity), and those left out
     take the kind's default constructor values."""
+    _release = "ob_image_proc_destroy"
 
     KINDS = {"auto_exposure": _capi.OB_IMAGE_AUTO_EXPOSURE, "beam_uniformity": _capi.OB_IMAGE_BEAM_UNIFORMITY,
              "local_tone_map": _capi.OB_IMAGE_LOCAL_TONE_MAP}
@@ -1328,26 +1226,6 @@ class ImageProcessor:
         check(lib.ob_image_proc_create(device, self.KINDS[kind], C.byref(p), C.byref(hd)))
         self._h, self.kind, self.device = hd, kind, device
         self._st = None
-        self._wrapped = None
-
-    def __del__(self):
-        if getattr(self, "_h", None) and lib is not None:
-            try:
-                lib.ob_image_proc_destroy(self._h)
-            except Exception:
-                pass
-            self._h = None
-
-    def _stream_for(self, x, stream):
-        if stream is not None:
-            return stream
-        if _is_torch(x) and x.is_cuda:
-            import torch
-            h = torch.cuda.current_stream(x.device).cuda_stream
-            if self._wrapped is None or self._wrapped[0] != h:  # one wrapper per torch stream, reused per frame
-                self._wrapped = (h, Stream(x.device.index, cuda_stream=h))
-            return self._wrapped[1]
-        return _stream(None, self.device)
 
     def update(self, image, out=None, update_state=True, stream=None):
         """update(image, update_state).  image: (h, w) or (h, w, 3) float32 / float64, C-contiguous numpy array or
@@ -1361,22 +1239,17 @@ class ImageProcessor:
         if not contiguous:
             raise TypeError("image must be C-contiguous")
         rows, cols = shape[0], shape[1]
-        st = self._stream_for(image, stream)
-        self._st = st
+        if dt == np.float16 and len(shape) != 3:
+            raise ValueError("Expected an H x W x 3 array")
+        if dt not in (np.float16, np.float32, np.float64):
+            raise TypeError("image must be float32 or float64")
+        st = self._st = _stream_for(image, stream, self.device)
         if dt == np.float16:
-            if len(shape) != 3:
-                raise ValueError("Expected an H x W x 3 array")
             if out is None:
-                if _is_torch(image):
-                    import torch
-                    out = torch.empty(shape, dtype=torch.float32, device=image.device)
-                else:
-                    out = np.empty(shape, np.float32)
+                out = _empty(image, shape, np.float32)
             check(lib.ob_image_proc_update(self._h, _capi.OB_IMAGE_RGB_F16, _capi.OB_F32, _ptr(image), _ptr(out),
                                            rows, cols, int(bool(update_state)), st.h))
             return out
-        if dt not in (np.float32, np.float64):
-            raise TypeError("image must be float32 or float64")
         layout = _capi.OB_IMAGE_MONO if len(shape) == 2 else _capi.OB_IMAGE_RGB
         dtype = _capi.OB_F32 if dt == np.float32 else _capi.OB_F64
         check(lib.ob_image_proc_update(self._h, layout, dtype, None, _ptr(image), rows, cols,

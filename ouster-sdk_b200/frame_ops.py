@@ -92,22 +92,6 @@ def _resolve_pixel_fields(fr, filtered_fields, python=False):
     return [f for f in present if fr.field_class(f) == PIXEL_FIELD]
 
 
-_wrapped = {}
-
-
-def _stream(fs):
-    """The torch stream of device frames, wrapped once per stream: wrapping configures the device's memory pool,
-    which a CUDA graph capture must not see, so a stream used for capture is wrapped by an earlier (warm-up) call."""
-    if fs and fs[0].device:
-        import torch
-        t = fs[0].array(fs[0].names[0])
-        key = (t.device.index, torch.cuda.current_stream(t.device).cuda_stream)
-        if key not in _wrapped:
-            _wrapped[key] = _c.Stream(key[0], cuda_stream=key[1])
-        return _wrapped[key]
-    return _c._stream(None)
-
-
 def _targets(fr, names, role_of=None):
     """(name, tag, role) of the fields the per-type visit writes; raises the reference's dimension text for a
     handled type that is not (h, w)."""
@@ -143,7 +127,7 @@ def _run(fs, predicate, per_frame, lower=0.0, upper=0.0, invalid=0.0, shifts=Non
     io.lut = lut._h if lut is not None else None
     io.poses = _c._ptr(poses) if poses is not None else None
     io.axis = int(axis)
-    st = _stream(fs)
+    st = _c._stream_for(fs[0].array(fs[0].names[0]) if fs[0].device else None)
     _c.check(_c.lib.ob_frame_mask_fields(C.byref(io), st.h))
     if fs[0].device:
         _keep(fs[0], (tab, sh, poses) + tuple(keep))
@@ -446,7 +430,7 @@ def reduce_by_factor_metadata(metadata, factor):
     return select_by_index_metadata(metadata, _reduce_factor_to_indices(factor, metadata.h))
 
 
-def _gather(pairs, rows, src_rows, fs):
+def _gather(pairs, rows, src_rows):
     """One ob_frame_select_rows call over (src, dst) arrays of the same row length."""
     if not pairs:
         return
@@ -458,8 +442,7 @@ def _gather(pairs, rows, src_rows, fs):
     io = _capi.FrameRowsIO()
     io.entries, io.n_entries, io.n_rows = tab, len(pairs), len(rows)
     io.rows = r.ctypes.data_as(C.POINTER(C.c_uint32))
-    st = _stream(fs)   # held across the call: the handle is released with the object
-    _c.check(_c.lib.ob_frame_select_rows(C.byref(io), st.h))
+    _c.check(_c.lib.ob_frame_select_rows(C.byref(io), _c._stream_for(pairs[0][0]).h))
 
 
 def select_by_index(frame, indices, update_metadata=False):
@@ -517,7 +500,7 @@ def select_by_index(frame, indices, update_metadata=False):
                 pairs.append((np.ascontiguousarray(fr.array(n)), out.field(n)))
             out.sensor_info = info if update_metadata else None
         outs.append(out)
-    _gather(pairs, indices, fs[0].h if fs else 0, fs)
+    _gather(pairs, indices, fs[0].h if fs else 0)
     return outs if many else outs[0]
 
 

@@ -6,6 +6,7 @@ import ctypes as C
 import numpy as np
 
 from ._capi import FieldDesc, PacketLayout, check, lib
+from .core import _Handle
 
 vp, sz, i32, u32, u64, i64 = C.c_void_p, C.c_size_t, C.c_int, C.c_uint32, C.c_uint64, C.c_int64
 PP = C.POINTER
@@ -112,8 +113,9 @@ def _as_array(ptr, dtype, shape):
     return raw.view(dtype).reshape(shape)
 
 
-class SensorInfo:
+class SensorInfo(_Handle):
     """SensorInfo + PacketFormat of one sensor stream."""
+    _release = "obh_sensor_destroy"
 
     def __init__(self, profile, h, w, columns_per_packet=16, header_type="STANDARD",
                  pixel_shift_by_row=None, init_id=0, sn=0, fw_rev="UNKNOWN", column_window=None, prod_line=""):
@@ -216,17 +218,10 @@ class SensorInfo:
         p = np.ascontiguousarray(packet)
         return lib.obh_sensor_calculate_crc(self._h, p.ctypes.data, p.size)
 
-    def __del__(self):
-        if getattr(self, "_h", None) and lib is not None:
-            try:
-                lib.obh_sensor_destroy(self._h)
-            except Exception:
-                pass
-            self._h = None
 
-
-class LidarFrame:
+class LidarFrame(_Handle):
     """LidarFrame / LidarScan: named row-major fields + per-column / per-packet headers (host)."""
+    _release = "obh_frame_destroy"
 
     def __init__(self, info, _borrowed=None):
         if _borrowed is None:
@@ -325,14 +320,6 @@ class LidarFrame:
     def set_status(self, frame_status, shutdown_countdown=0, shot_limiting_countdown=0):
         lib.obh_frame_set_status(self._h, frame_status, shutdown_countdown, shot_limiting_countdown)
 
-    def __del__(self):
-        if getattr(self, "_h", None) and getattr(self, "_owned", False) and lib is not None:
-            try:
-                lib.obh_frame_destroy(self._h)
-            except Exception:
-                pass
-        self._h = None
-
 
 def frame_to_packets(frame, info, init_id=0, prod_sn=0, device=False):
     """impl::frame_to_packets -> (packets uint8 [n, size], host_ts uint64 [n]).  device=True: the
@@ -346,11 +333,12 @@ def frame_to_packets(frame, info, init_id=0, prod_sn=0, device=False):
     return out[:n.value].copy(), ts[:n.value].copy()
 
 
-class PcapLidarSource:
+class PcapLidarSource(_Handle):
     """Capture file -> page-locked ring of lidar packets (include/ouster/core/pcap_source.h; replaces the
     read loop of ouster_pcap/src/pcap_packet_source.cpp for this path).  `next_burst` returns numpy VIEWS of
     the ring ([n, packet_size] uint8 with the ring's stride, [n] uint64 capture timestamps in ns), valid
     until the next call -- feed them to FrameBatcher.batch_burst / FramePipeline.push_burst as they are."""
+    _release = "obh_pcap_close"
 
     def __init__(self, path, lidar_packet_size, dst_port=0, ring_packets=256):
         hd = vp()
@@ -390,15 +378,10 @@ class PcapLidarSource:
             lib.obh_pcap_close(self._h)
             self._h = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
-
-class FrameBatcher:
+class FrameBatcher(_Handle):
     """FrameBatcher / ScanBatcher: host state machine + one fused GPU decode per frame."""
+    _release = "obh_batcher_destroy"
 
     def __init__(self, info):
         hd = vp()
@@ -499,14 +482,6 @@ class FrameBatcher:
         rdd = _as_array(rd.value, np.uint32, (h, w)) if rd.value else None
         return pts, rdd
 
-    def __del__(self):
-        if getattr(self, "_h", None) and lib is not None:
-            try:
-                lib.obh_batcher_destroy(self._h)
-            except Exception:
-                pass
-            self._h = None
-
 
 class FinishedSlot:
     """A finished FramePipeline slot: .frame (LidarFrame view), .xyz[r], .range_destaggered[r].
@@ -539,9 +514,10 @@ class FinishedSlot:
         return self._rd
 
 
-class FramePipeline:
+class FramePipeline(_Handle):
     """Ring of LidarFrames with `depth` frames in flight on the GPU (frame_pipeline.h): the host
     state machine of frame k+1 overlaps the H2D / fused kernel / D2H of frame k."""
+    _release = "obh_pipeline_destroy"
 
     def __init__(self, info, depth=3, lut=None, pixel_shift_by_row=None):
         sh, n = None, 0
@@ -589,14 +565,6 @@ class FramePipeline:
     @property
     def dropped_packets(self):
         return lib.obh_pipeline_dropped_packets(self._h)
-
-    def __del__(self):
-        if getattr(self, "_h", None) and lib is not None:
-            try:
-                lib.obh_pipeline_destroy(self._h)
-            except Exception:
-                pass
-            self._h = None
 
 
 LidarScan = LidarFrame

@@ -77,11 +77,7 @@ class _XYZLutBase:
             torch = _torch()
             if t.dtype not in (torch.int32, torch.uint32):
                 raise ValueError("range must be uint32")
-            out = torch.empty((self.h * self.w, 3), device=t.device,
-                              dtype=torch.float64 if self._dtype == np.float64 else torch.float32)
-            st = _c.Stream(t.device.index, cuda_stream=torch.cuda.current_stream(t.device).cuda_stream)
-            _c.check(_c.lib.ob_cartesian(self._lut._h, t.contiguous().data_ptr(), self.h * self.w, out.data_ptr(), st.h))
-            return out.reshape(self.h, self.w, 3)
+            return _c.cartesian(self._lut, t.contiguous().view(torch.uint32)).reshape(self.h, self.w, 3)
         if is_scan:
             if rng.shape != (self.h, self.w):
                 raise ValueError("Frame dimensions do not match lut.")
@@ -109,9 +105,7 @@ def destagger(info, fields, inverse=False):
             raise ValueError("Invalid dimensions for destaggering")
         if t.shape[0] != info.h or t.shape[1] != info.w or t.numel() == 0:
             raise ValueError("Image resolution must match SensorInfo.")
-        torch = _torch()
-        st = _c.Stream(t.device.index, cuda_stream=torch.cuda.current_stream(t.device).cuda_stream)
-        return _c.destagger(t.contiguous(), info.pixel_shift_by_row, inverse, stream=st, device=t.device.index)
+        return _c.destagger(t.contiguous(), info.pixel_shift_by_row, inverse)
     a = np.asarray(fields)
     if a.ndim < 2 or a.ndim > 3:
         raise ValueError("Invalid dimensions for destaggering")
@@ -145,8 +139,7 @@ def dewarp(points, poses):
         dt = torch.float32 if tp.dtype == torch.float32 else torch.float64
         tq = _dev(poses)
         tq = tq.to(dt) if tq is not None else torch.as_tensor(np.ascontiguousarray(poses), dtype=dt, device=tp.device)
-        st = _c.Stream(tp.device.index, cuda_stream=torch.cuda.current_stream(tp.device).cuda_stream)
-        return _c.dewarp(tp.to(dt).contiguous(), tq.contiguous(), stream=st, device=tp.device.index)
+        return _c.dewarp(tp.to(dt).contiguous(), tq.contiguous())
     p, q = _floating(points, "points and poses"), _floating(poses, "points and poses")
     dt = np.float32 if p.dtype == np.float32 else np.float64
     return _c.dewarp(np.ascontiguousarray(p, dt), np.ascontiguousarray(q, dt))
@@ -173,8 +166,7 @@ def normals(xyz, range, *args, **kwargs):
     if "sensor_origins_xyz" in kwargs and isinstance(kwargs["sensor_origins_xyz"], np.ndarray):
         kwargs["sensor_origins_xyz"] = torch.as_tensor(np.ascontiguousarray(kwargs["sensor_origins_xyz"], np.float64),
                                                        device=t.device)
-    st = _c.Stream(t.device.index, cuda_stream=torch.cuda.current_stream(t.device).cuda_stream)
-    return _c.normals(t.contiguous(), _dev(range), *conv, stream=st, device=t.device.index, **kwargs)
+    return _c.normals(t.contiguous(), _dev(range), *conv, **kwargs)
 
 
 class VoxelDownsampleStrategy(enum.IntEnum):
