@@ -1,6 +1,6 @@
 // ob_api.cu -- C-ABI glue: error state, streams, staging of host buffers, LUT handles and the
-// entry points declared in include/ouster_b200.h (everything except the decode path, which
-// lives in ob_decode.cu).
+// entry points declared in include/ouster_b200.h (everything except the decoder, decode and
+// encode entry points, which live in ob_api_decode.cu).
 #include <atomic>
 #include <cmath>
 #include <cstdlib>
@@ -272,18 +272,10 @@ struct ob_lut {
     bool analytic_on{false};
 };
 
-// used by ob_decode.cu
 namespace ob {
-void lut_view(const ob_lut* lut, const void** dir, const void** off, int* dtype, size_t* h,
-              size_t* w, int* device) {
-    *dir = lut->dir;
-    *off = lut->off;
-    *dtype = lut->dtype;
-    *h = lut->h;
-    *w = lut->w;
-    *device = lut->device;
+LutView lut_view(const ob_lut* lut) {
+    return LutView{lut->dir, lut->off, lut->dtype, lut->h, lut->w, lut->device, lut->analytic_on ? lut->an : nullptr};
 }
-const void* lut_analytic(const ob_lut* lut) { return lut->analytic_on ? lut->an : nullptr; }
 cudaStream_t stream_handle(ob_stream* s) { return s->st; }
 
 cudaError_t stream_table(ob_stream* s, int which, const void* host, size_t bytes, const void** dev) {

@@ -40,9 +40,15 @@ class Staging {
 };
 
 // accessors for the opaque handles (defined in ob_api.cu)
-void lut_view(const ob_lut* lut, const void** dir, const void** off, int* dtype, size_t* h,
-              size_t* w, int* device);
-const void* lut_analytic(const ob_lut* lut);  // device LutAnalyticT<T> when the LUT-free mode is on, else null
+struct LutView {
+    const void* dir;
+    const void* off;
+    int dtype;
+    size_t h, w;
+    int device;
+    const void* an;  // device LutAnalyticT<T> when the LUT-free mode is on, else null
+};
+LutView lut_view(const ob_lut* lut);
 cudaStream_t stream_handle(ob_stream* s);
 // device copy of a small per-launch table (which: 0 decode frames, 1 encode frames), re-uploaded only when
 // its contents changed since the stream's previous launch of that kind

@@ -1,4 +1,5 @@
-// ob_api_decode.cu -- C-ABI glue of the packet-decode path (ob_decoder_*, ob_decode_frames).
+// ob_api_decode.cu -- C-ABI glue of the packet decode and encode: ob_decoder_*, the three decode entry points
+// (ob_decode_frames, ob_decode_batch_run, ob_decode_job_*) and ob_encode_frames.
 #include <algorithm>
 #include <cstring>
 #include <memory>
@@ -45,6 +46,184 @@ static const void* maps_for(const DecodeLayout& L, int device, const void* dir, 
     uint32_t bw = 0, bh = 0;
     if (!dir || !off || !decode_pipe_box(L, device, dtype, &bw, &bh)) return nullptr;
     return lut_tensor_maps(dir, off, dtype, L.H, L.W, bw, bh, device);
+}
+
+static bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+
+constexpr size_t kMaxSlots = size_t(1) << 20;  // packet slots of one frame
+
+// The outputs of a decoded frame in one numbering: field k < OB_MAX_FIELDS, the three column headers, then XYZ and
+// destaggered range of each return (the order in which the paths stage them)
+enum : int { kOutTs = OB_MAX_FIELDS, kOutMid, kOutStatus, kOutReturns, kOuts = kOutReturns + 2 * OB_MAX_RETURNS };
+static bool is_xyz(int k) { return k >= kOutReturns && (k - kOutReturns) % 2 == 0; }
+
+// bytes of output k of one frame (XYZ in the call's LUT dtype)
+static size_t out_bytes(const DecodeLayout& L, int dtype, int k) {
+    const size_t n_px = static_cast<size_t>(L.H) * L.W;
+    if (k < kOutTs) return n_px * L.fields[k].elem_size;
+    if (k == kOutTs) return L.W * 8ull;
+    if (k == kOutMid) return L.W * 2ull;
+    if (k == kOutStatus) return L.W * 4ull;
+    return is_xyz(k) ? n_px * 3 * (dtype == OB_F64 ? 8 : 4) : n_px * 4;
+}
+
+// output k of an ob_decode_io, or of frame 0 of an ob_decode_batch; null: not requested
+template <typename IO>
+static void* io_out(const DecodeLayout& L, const IO& io, int k) {
+    if (k < kOutTs) return k < static_cast<int>(L.n_fields) ? io.fields[k] : nullptr;
+    if (k == kOutTs) return io.timestamp;
+    if (k == kOutMid) return io.measurement_id;
+    if (k == kOutStatus) return io.status;
+    const int r = (k - kOutReturns) / 2;
+    return is_xyz(k) ? io.xyz[r] : io.range_destaggered[r];
+}
+
+// bytes from a batch frame's output k to the next frame's
+static size_t batch_stride(const ob_decode_batch& b, int k) {
+    if (k < kOutTs) return b.field_frame_stride[k];
+    if (k == kOutTs) return b.timestamp_frame_stride;
+    if (k == kOutMid) return b.measurement_id_frame_stride;
+    if (k == kOutStatus) return b.status_frame_stride;
+    return is_xyz(k) ? b.xyz_frame_stride : b.rd_frame_stride;
+}
+
+static void set_out(DecodeFrame& f, int k, void* p) {
+    const int r = (k - kOutReturns) / 2;
+    if (k < kOutTs) f.fields[k] = p;
+    else if (k == kOutTs) f.timestamp = static_cast<uint64_t*>(p);
+    else if (k == kOutMid) f.measurement_id = static_cast<uint16_t*>(p);
+    else if (k == kOutStatus) f.status = static_cast<uint32_t*>(p);
+    else if (is_xyz(k)) f.xyz[r] = p;
+    else f.rd[r] = static_cast<uint32_t*>(p);
+}
+
+// A LUT of a decode call as the kernels see it
+struct CallLut {
+    const void* dir{nullptr};
+    const void* off{nullptr};
+    const void* maps{nullptr};  // TMA descriptors for the pipelined kernel, or null
+    const void* an{nullptr};    // LUT-free mode, or null
+};
+
+// One decode call: its checked arguments, and the launch-level facts every frame of its table folds into
+struct DecodeCall {
+    const DecodeLayout* L;
+    int device;
+    const ob_lut* lut;         // call-level LUT (nullable) ...
+    CallLut call_lut;          // ... as the kernels see it
+    int dtype{OB_F32};         // the one dtype of every LUT of the call
+    int n_luts{0};
+    std::vector<uint16_t> sh;  // shift table reduced to [0, W); empty: no shifts
+    bool vec_ok{true}, frame_luts_have_maps{true}, any_xyz{false};
+};
+
+static ob_status same_device(const ob_decoder* dec, ob_stream* s) {
+    if (stream_device(s) != dec->device) return fail(OB_INVALID_ARGUMENT, "decoder and stream are on different devices");
+    return OB_OK;
+}
+
+// Checks a LUT of the call, call-level or per-frame: every LUT of one launch has the decoder's shape, the call's
+// device and one dtype, because the kernel is instantiated for one dtype and XYZ outputs are sized by it
+static ob_status take_lut(DecodeCall& c, const ob_lut* lut, CallLut* out) {
+    const LutView v = lut_view(lut);
+    if (v.h != c.L->H || v.w != c.L->W) return fail(OB_INVALID_ARGUMENT, "unexpected image dimensions");
+    if (v.device != c.device) return fail(OB_INVALID_ARGUMENT, "lut and stream are on different devices");
+    if (c.n_luts++ > 0 && v.dtype != c.dtype)
+        return fail(OB_INVALID_ARGUMENT,
+                    c.lut ? "per-frame lut dtype differs from the call-level lut" : "per-frame lut dtype differs");
+    c.dtype = v.dtype;
+    if (!al16(v.dir) || !al16(v.off)) c.vec_ok = false;
+    *out = CallLut{v.dir, v.off, maps_for(*c.L, c.device, v.dir, v.off, v.dtype), v.an};
+    return OB_OK;
+}
+
+// The start of every decode call: device, call-level LUT and shift table
+static ob_status begin_call(DecodeCall& c, const ob_decoder* dec, ob_stream* s, const ob_lut* lut,
+                            const int32_t* shifts, size_t n_shifts) {
+    ob_status rs = same_device(dec, s);
+    if (rs == OB_OK) rs = require_device(dec->device);
+    if (rs != OB_OK) return rs;
+    const DecodeLayout& L = dec->L;
+    c.L = &L;
+    c.device = dec->device;
+    c.lut = lut;
+    if (lut && (rs = take_lut(c, lut, &c.call_lut)) != OB_OK) return rs;
+    if (shifts) {
+        if (n_shifts != L.H) return fail(OB_INVALID_ARGUMENT, "image height does not match shifts size");
+        if (L.H > static_cast<uint32_t>(kMaxRows))
+            return fail(OB_INVALID_ARGUMENT, "fused destagger supports at most 512 rows");
+        reduce_shifts(shifts, L.H, L.W, 0, c.sh);
+    }
+    return OB_OK;
+}
+
+// XYZ needs a LUT, destaggered range a shift table
+static ob_status check_fused(const DecodeCall& c, bool has_lut, void* const xyz[], uint32_t* const rd[]) {
+    for (int r = 0; r < OB_MAX_RETURNS; ++r) {
+        if (xyz[r] && !has_lut) return fail(OB_INVALID_ARGUMENT, "xyz output requested without a lut");
+        if (rd[r] && c.sh.empty()) return fail(OB_INVALID_ARGUMENT, "image height does not match shifts size");
+    }
+    return OB_OK;
+}
+
+// Sets a frame's flag bits and its own LUT (null: the call-level one) once its packets, column map and outputs are
+// in place, and folds the frame into the launch-level facts
+static void finish_frame(DecodeCall& c, DecodeFrame& f, bool bulk_ok, const CallLut* lut) {
+    bool all_fields = c.L->n_fields > 0;
+    for (uint32_t k = 0; k < c.L->n_fields; ++k) all_fields = all_fields && f.fields[k] != nullptr;
+    f.flags = (f.col_src ? 0u : kFrameIdentityMap) | (bulk_ok ? kFrameBulkPackets : 0u) |
+              (all_fields ? kFrameAllFields : 0u);
+    if (lut) {
+        f.lut_dir = lut->dir;
+        f.lut_off = lut->off;
+        f.lut_maps = lut->maps;
+        f.lut_an = lut->an;
+        if (!lut->maps && !lut->an) c.frame_luts_have_maps = false;
+    }
+    for (int r = 0; r < OB_MAX_RETURNS; ++r) {
+        if (!f.xyz[r]) continue;
+        c.any_xyz = true;
+        if (!al16(f.xyz[r])) c.vec_ok = false;
+    }
+}
+
+// xyz_base / xyz_frame_stride: the XYZ outputs of a uniformly strided batch (frame f at base + f * stride)
+static cudaError_t launch(const DecodeCall& c, const void* frames_dev, size_t n_frames, cudaStream_t st,
+                          const void* const* xyz_base = nullptr, unsigned long long xyz_frame_stride = 0) {
+    DecodeLaunch a;
+    a.layout_host = c.L;
+    a.frames_dev = static_cast<const DecodeFrame*>(frames_dev);
+    a.n_frames = static_cast<uint32_t>(n_frames);
+    a.lut_dir = c.call_lut.dir;
+    a.lut_off = c.call_lut.off;
+    a.lut_dtype = c.dtype;
+    a.shift_host = c.sh.empty() ? nullptr : c.sh.data();
+    a.vec_ok = c.vec_ok;
+    a.lut_maps = c.call_lut.maps;
+    a.lut_an = c.call_lut.an;
+    a.frame_luts_have_maps = c.frame_luts_have_maps;
+    a.any_xyz = c.any_xyz;
+    if (xyz_base) {
+        a.xyz_base[0] = xyz_base[0];
+        a.xyz_base[1] = xyz_base[1];
+        a.xyz_frame_stride = xyz_frame_stride;
+    }
+    return launch_decode(a, c.device, st);
+}
+
+// ob_decode_frames and ob_decode_batch_run: the table goes through the stream's cached copy, host outputs come
+// back from their staging after the launch
+static ob_status run_table(const DecodeCall& c, ob_stream* s, std::vector<DecodeFrame>& hf, Staging& stg,
+                           const void* const* xyz_base = nullptr, unsigned long long xyz_frame_stride = 0) {
+    group_by_lut(hf);
+    const void* fdev = nullptr;
+    cudaError_t e = stream_table(s, 0, hf.data(), hf.size() * sizeof(DecodeFrame), &fdev);
+    if (e != cudaSuccess) return fail_cuda(e, "frame table upload");
+    e = launch(c, fdev, hf.size(), stream_handle(s), xyz_base, xyz_frame_stride);
+    if (e != cudaSuccess) return fail_cuda(e, "decode launch");
+    e = stg.flush();
+    if (e != cudaSuccess) return fail_cuda(e, "decode D2H");
+    return OB_OK;
 }
 
 extern "C" {
@@ -110,34 +289,12 @@ ob_status ob_decode_frames(const ob_decoder* dec, const ob_decode_io* frames, si
                            const ob_lut* lut, const int32_t* shifts, size_t n_shifts, ob_stream* s) {
     if (!dec || !s || (n_frames && !frames)) return fail(OB_INVALID_ARGUMENT, "null pointer");
     if (n_frames == 0) return OB_OK;
-    const DecodeLayout& L = dec->L;
-    const int device = stream_device(s);
-    if (device != dec->device) return fail(OB_INVALID_ARGUMENT, "decoder and stream are on different devices");
-    ob_status rs = require_device(device);
+    DecodeCall c;
+    ob_status rs = begin_call(c, dec, s, lut, shifts, n_shifts);
     if (rs != OB_OK) return rs;
-    const void *ldir = nullptr, *loff = nullptr;
-    int ldtype = OB_F32;
-    if (lut) {
-        size_t lh, lw;
-        int ldev;
-        lut_view(lut, &ldir, &loff, &ldtype, &lh, &lw, &ldev);
-        if (lh != L.H || lw != L.W) return fail(OB_INVALID_ARGUMENT, "unexpected image dimensions");
-        if (ldev != device) return fail(OB_INVALID_ARGUMENT, "lut and stream are on different devices");
-    }
-    std::vector<uint16_t> sh;
-    if (shifts) {
-        if (n_shifts != L.H) return fail(OB_INVALID_ARGUMENT, "image height does not match shifts size");
-        if (L.H > static_cast<uint32_t>(kMaxRows))
-            return fail(OB_INVALID_ARGUMENT, "fused destagger supports at most 512 rows");
-        reduce_shifts(shifts, L.H, L.W, 0, sh);
-    }
-    const size_t n_px = static_cast<size_t>(L.H) * L.W;
-    cudaStream_t st = stream_handle(s);
-    Staging stg(st);
+    const DecodeLayout& L = dec->L;
+    Staging stg(stream_handle(s));
     std::vector<DecodeFrame> hf(n_frames);
-    bool vec_ok = true, frame_maps_ok = true, any_xyz = false;
-    auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
-    if (lut && (!al16(ldir) || !al16(loff))) vec_ok = false;
     for (size_t i = 0; i < n_frames; ++i) {
         const ob_decode_io& io = frames[i];
         DecodeFrame& f = hf[i];
@@ -145,7 +302,10 @@ ob_status ob_decode_frames(const ob_decoder* dec, const ob_decode_io* frames, si
         if (io.n_slots > 0 && !io.packets) return fail(OB_INVALID_ARGUMENT, "null packet buffer");
         if (io.n_slots > 0 && io.packet_stride < L.packet_size)
             return fail(OB_INVALID_ARGUMENT, "packet_stride smaller than the lidar packet size");
-        if (io.n_slots > (1u << 20)) return fail(OB_INVALID_ARGUMENT, "too many packet slots");
+        if (io.n_slots > kMaxSlots) return fail(OB_INVALID_ARGUMENT, "too many packet slots");
+        CallLut frame_lut;
+        if (io.lut && (rs = take_lut(c, io.lut, &frame_lut)) != OB_OK) return rs;
+        if ((rs = check_fused(c, lut || io.lut, io.xyz, io.range_destaggered)) != OB_OK) return rs;
         const void* d = nullptr;
         cudaError_t e = cudaSuccess;
         if (io.n_slots > 0) {
@@ -155,241 +315,76 @@ ob_status ob_decode_frames(const ob_decoder* dec, const ob_decode_io* frames, si
         f.packets = static_cast<const uint8_t*>(d);
         f.packet_stride = io.packet_stride;
         f.n_slots = static_cast<uint32_t>(io.n_slots);
-        f.flags = 0;
-        if (!io.col_src) f.flags |= 1u;
-        if (d && al16(d) && io.packet_stride % 16 == 0 && L.packet_size % 16 == 0) f.flags |= 2u;
         if (io.col_src) {
             e = stg.in(io.col_src, static_cast<size_t>(L.W) * 4, &d);
             if (e != cudaSuccess) return fail_cuda(e, "stage column map");
             f.col_src = static_cast<const int32_t*>(d);
         }
-        void* o = nullptr;
-        for (uint32_t k = 0; k < L.n_fields; ++k) {
-            if (!io.fields[k]) continue;
-            e = stg.out(io.fields[k], n_px * L.fields[k].elem_size, &o);
-            if (e != cudaSuccess) return fail_cuda(e, "stage field output");
-            f.fields[k] = o;
+        for (int k = 0; k < kOuts; ++k) {
+            void* user = io_out(L, io, k);
+            if (!user) continue;
+            void* o = nullptr;
+            e = stg.out(user, out_bytes(L, c.dtype, k), &o);
+            if (e != cudaSuccess) return fail_cuda(e, "stage outputs");
+            set_out(f, k, o);
         }
-        {
-            bool allf = L.n_fields > 0;
-            for (uint32_t k = 0; k < L.n_fields; ++k) allf = allf && f.fields[k] != nullptr;
-            if (allf) f.flags |= 4u;  // every decoder field has an output image
-        }
-        if (io.timestamp) {
-            e = stg.out(io.timestamp, static_cast<size_t>(L.W) * 8, &o);
-            if (e != cudaSuccess) return fail_cuda(e, "stage timestamp");
-            f.timestamp = static_cast<uint64_t*>(o);
-        }
-        if (io.measurement_id) {
-            e = stg.out(io.measurement_id, static_cast<size_t>(L.W) * 2, &o);
-            if (e != cudaSuccess) return fail_cuda(e, "stage measurement_id");
-            f.measurement_id = static_cast<uint16_t*>(o);
-        }
-        if (io.status) {
-            e = stg.out(io.status, static_cast<size_t>(L.W) * 4, &o);
-            if (e != cudaSuccess) return fail_cuda(e, "stage status");
-            f.status = static_cast<uint32_t*>(o);
-        }
-        if (io.lut) {
-            const void *fd = nullptr, *fo = nullptr;
-            int fdt, fdev;
-            size_t fh, fw;
-            lut_view(io.lut, &fd, &fo, &fdt, &fh, &fw, &fdev);
-            if (fh != L.H || fw != L.W) return fail(OB_INVALID_ARGUMENT, "unexpected image dimensions");
-            if (fdev != device) return fail(OB_INVALID_ARGUMENT, "lut and stream are on different devices");
-            if (lut && fdt != ldtype) return fail(OB_INVALID_ARGUMENT, "per-frame lut dtype differs from the call-level lut");
-            if (!lut) ldtype = fdt;
-            f.lut_dir = fd;
-            f.lut_off = fo;
-            f.lut_maps = maps_for(L, device, fd, fo, fdt);
-            f.lut_an = lut_analytic(io.lut);
-            if (!f.lut_maps && !f.lut_an) frame_maps_ok = false;
-            if (!al16(fd) || !al16(fo)) vec_ok = false;
-        }
-        for (int r = 0; r < OB_MAX_RETURNS; ++r) {
-            if (io.xyz[r]) {
-                if (!lut && !io.lut) return fail(OB_INVALID_ARGUMENT, "xyz output requested without a lut");
-                e = stg.out(io.xyz[r], n_px * 3 * (ldtype == OB_F64 ? 8 : 4), &o);
-                if (e != cudaSuccess) return fail_cuda(e, "stage xyz");
-                f.xyz[r] = o;
-                any_xyz = true;
-                if (!al16(o)) vec_ok = false;
-            }
-            if (io.range_destaggered[r]) {
-                if (!shifts) return fail(OB_INVALID_ARGUMENT, "image height does not match shifts size");
-                e = stg.out(io.range_destaggered[r], n_px * 4, &o);
-                if (e != cudaSuccess) return fail_cuda(e, "stage range_destaggered");
-                f.rd[r] = static_cast<uint32_t*>(o);
-            }
-        }
+        const bool bulk_ok = f.packets && al16(f.packets) && io.packet_stride % 16 == 0 && L.packet_size % 16 == 0;
+        finish_frame(c, f, bulk_ok, io.lut ? &frame_lut : nullptr);
     }
-    group_by_lut(hf);
-    const void* fdev = nullptr;
-    cudaError_t e = stream_table(s, 0, hf.data(), n_frames * sizeof(DecodeFrame), &fdev);
-    if (e != cudaSuccess) return fail_cuda(e, "frame table upload");
-    DecodeLaunch a;
-    a.layout_host = &L;
-    a.frames_dev = static_cast<const DecodeFrame*>(fdev);
-    a.n_frames = static_cast<uint32_t>(n_frames);
-    a.lut_dir = ldir;
-    a.lut_off = loff;
-    a.lut_dtype = ldtype;
-    a.shift_host = shifts ? sh.data() : nullptr;
-    a.vec_ok = vec_ok;
-    a.lut_maps = maps_for(L, device, ldir, loff, ldtype);
-    a.lut_an = lut ? lut_analytic(lut) : nullptr;
-    a.frame_luts_have_maps = frame_maps_ok;
-    a.any_xyz = any_xyz;
-    e = launch_decode(a, device, st);
-    if (e != cudaSuccess) return fail_cuda(e, "decode launch");
-    e = stg.flush();
-    if (e != cudaSuccess) return fail_cuda(e, "decode D2H");
-    return OB_OK;
+    return run_table(c, s, hf, stg);
 }
 
 ob_status ob_decode_batch_run(const ob_decoder* dec, const ob_decode_batch* b, const ob_lut* lut,
                               const int32_t* shifts, size_t n_shifts, ob_stream* s) {
     if (!dec || !b || !s) return fail(OB_INVALID_ARGUMENT, "null pointer");
     if (b->n_frames == 0) return OB_OK;
-    const DecodeLayout& L = dec->L;
-    const int device = stream_device(s);
-    if (device != dec->device) return fail(OB_INVALID_ARGUMENT, "decoder and stream are on different devices");
-    ob_status rs = require_device(device);
+    DecodeCall c;
+    ob_status rs = begin_call(c, dec, s, lut, shifts, n_shifts);
     if (rs != OB_OK) return rs;
+    const DecodeLayout& L = dec->L;
     if (!b->packets || b->n_slots == 0) return fail(OB_INVALID_ARGUMENT, "null packet buffer");
     if (b->packet_stride < L.packet_size)
         return fail(OB_INVALID_ARGUMENT, "packet_stride smaller than the lidar packet size");
-    const void *ldir = nullptr, *loff = nullptr;
-    int ldtype = OB_F32;
-    if (lut) {
-        size_t lh, lw;
-        int ldev;
-        lut_view(lut, &ldir, &loff, &ldtype, &lh, &lw, &ldev);
-        if (lh != L.H || lw != L.W) return fail(OB_INVALID_ARGUMENT, "unexpected image dimensions");
-        if (ldev != device) return fail(OB_INVALID_ARGUMENT, "lut and stream are on different devices");
-    }
-    std::vector<uint16_t> sh;
-    if (shifts) {
-        if (n_shifts != L.H) return fail(OB_INVALID_ARGUMENT, "image height does not match shifts size");
-        if (L.H > static_cast<uint32_t>(kMaxRows))
-            return fail(OB_INVALID_ARGUMENT, "fused destagger supports at most 512 rows");
-        reduce_shifts(shifts, L.H, L.W, 0, sh);
-    }
+    if (b->n_slots > kMaxSlots) return fail(OB_INVALID_ARGUMENT, "too many packet slots");
     const size_t F = b->n_frames;
-    const size_t n_px = static_cast<size_t>(L.H) * L.W;
-    cudaStream_t st = stream_handle(s);
-    Staging stg(st);
-    auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
-    auto span = [&](size_t stride, size_t last) { return (F - 1) * stride + last; };
-    bool vec_ok = !lut || (al16(ldir) && al16(loff));
+    std::vector<CallLut> frame_luts(b->frame_luts ? F : 0);
+    for (size_t f = 0; f < frame_luts.size(); ++f) {
+        if (!b->frame_luts[f]) return fail(OB_INVALID_ARGUMENT, "null per-frame lut");
+        if ((rs = take_lut(c, b->frame_luts[f], &frame_luts[f])) != OB_OK) return rs;
+    }
+    if ((rs = check_fused(c, lut || b->frame_luts, b->xyz, b->range_destaggered)) != OB_OK) return rs;
 
+    Staging stg(stream_handle(s));
+    auto span = [&](size_t stride, size_t last) { return (F - 1) * stride + last; };
     const void* dpk = nullptr;
     cudaError_t e = stg.in(b->packets,
                            span(b->packets_frame_stride, (b->n_slots - 1) * b->packet_stride + L.packet_size),
                            &dpk);
     if (e != cudaSuccess) return fail_cuda(e, "stage packets");
-    void* dfields[OB_MAX_FIELDS] = {};
-    for (uint32_t k = 0; k < L.n_fields; ++k) {
-        if (!b->fields[k]) continue;
-        e = stg.out(b->fields[k], span(b->field_frame_stride[k], n_px * L.fields[k].elem_size), &dfields[k]);
-        if (e != cudaSuccess) return fail_cuda(e, "stage field output");
+    void* dout[kOuts] = {};  // frame 0's outputs
+    for (int k = 0; k < kOuts; ++k) {
+        void* user = io_out(L, *b, k);
+        if (!user) continue;
+        e = stg.out(user, span(batch_stride(*b, k), out_bytes(L, c.dtype, k)), &dout[k]);
+        if (e != cudaSuccess) return fail_cuda(e, "stage outputs");
     }
-    void *dts = nullptr, *dmid = nullptr, *dstat = nullptr;
-    if (b->timestamp) e = stg.out(b->timestamp, span(b->timestamp_frame_stride, L.W * 8ull), &dts);
-    if (e == cudaSuccess && b->measurement_id)
-        e = stg.out(b->measurement_id, span(b->measurement_id_frame_stride, L.W * 2ull), &dmid);
-    if (e == cudaSuccess && b->status) e = stg.out(b->status, span(b->status_frame_stride, L.W * 4ull), &dstat);
-    if (e != cudaSuccess) return fail_cuda(e, "stage headers");
-    std::vector<const void*> fl_dir, fl_off;
-    if (b->frame_luts) {
-        fl_dir.resize(F);
-        fl_off.resize(F);
-        for (size_t f = 0; f < F; ++f) {
-            if (!b->frame_luts[f]) return fail(OB_INVALID_ARGUMENT, "null per-frame lut");
-            int fdt, fdev;
-            size_t fh, fw;
-            lut_view(b->frame_luts[f], &fl_dir[f], &fl_off[f], &fdt, &fh, &fw, &fdev);
-            if (fh != L.H || fw != L.W) return fail(OB_INVALID_ARGUMENT, "unexpected image dimensions");
-            if (fdev != device) return fail(OB_INVALID_ARGUMENT, "lut and stream are on different devices");
-            if ((lut || f > 0) && fdt != ldtype)
-                return fail(OB_INVALID_ARGUMENT, "per-frame lut dtype differs");
-            ldtype = fdt;
-            if (!al16(fl_dir[f]) || !al16(fl_off[f])) vec_ok = false;
-        }
-    }
-    const size_t esz2 = ldtype == OB_F64 ? 8 : 4;
-    void* dxyz[OB_MAX_RETURNS] = {};
-    void* drd[OB_MAX_RETURNS] = {};
-    for (int r = 0; r < OB_MAX_RETURNS; ++r) {
-        if (b->xyz[r]) {
-            if (!lut && !b->frame_luts) return fail(OB_INVALID_ARGUMENT, "xyz output requested without a lut");
-            e = stg.out(b->xyz[r], span(b->xyz_frame_stride, n_px * 3 * esz2), &dxyz[r]);
-            if (e != cudaSuccess) return fail_cuda(e, "stage xyz");
-            if (!al16(dxyz[r]) || b->xyz_frame_stride % 16) vec_ok = false;
-        }
-        if (b->range_destaggered[r]) {
-            if (!shifts) return fail(OB_INVALID_ARGUMENT, "image height does not match shifts size");
-            e = stg.out(b->range_destaggered[r], span(b->rd_frame_stride, n_px * 4), &drd[r]);
-            if (e != cudaSuccess) return fail_cuda(e, "stage range_destaggered");
-        }
-    }
-    std::vector<DecodeFrame> hf(F);
-    bool frame_maps_ok = true;
     const bool bulk_ok = al16(dpk) && b->packet_stride % 16 == 0 && L.packet_size % 16 == 0 &&
                          b->packets_frame_stride % 16 == 0;
+    std::vector<DecodeFrame> hf(F);
     for (size_t f = 0; f < F; ++f) {
         DecodeFrame& d = hf[f];
         std::memset(&d, 0, sizeof(d));
         d.packets = static_cast<const uint8_t*>(dpk) + f * b->packets_frame_stride;
         d.packet_stride = b->packet_stride;
         d.n_slots = static_cast<uint32_t>(b->n_slots);
-        d.flags = 1u | (bulk_ok ? 2u : 0u);
-        bool allf = L.n_fields > 0;
-        for (uint32_t k = 0; k < L.n_fields; ++k) {
-            if (dfields[k]) d.fields[k] = static_cast<uint8_t*>(dfields[k]) + f * b->field_frame_stride[k];
-            allf = allf && dfields[k] != nullptr;
-        }
-        if (allf) d.flags |= 4u;  // every decoder field has an output image
-        if (dts) d.timestamp = reinterpret_cast<uint64_t*>(static_cast<uint8_t*>(dts) + f * b->timestamp_frame_stride);
-        if (dmid) d.measurement_id = reinterpret_cast<uint16_t*>(static_cast<uint8_t*>(dmid) + f * b->measurement_id_frame_stride);
-        if (dstat) d.status = reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(dstat) + f * b->status_frame_stride);
-        if (!fl_dir.empty()) {
-            d.lut_dir = fl_dir[f];
-            d.lut_off = fl_off[f];
-            d.lut_maps = maps_for(L, device, fl_dir[f], fl_off[f], ldtype);
-            d.lut_an = lut_analytic(b->frame_luts[f]);
-            if (!d.lut_maps && !d.lut_an) frame_maps_ok = false;
-        }
-        for (int r = 0; r < OB_MAX_RETURNS; ++r) {
-            if (dxyz[r]) d.xyz[r] = static_cast<uint8_t*>(dxyz[r]) + f * b->xyz_frame_stride;
-            if (drd[r]) d.rd[r] = reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(drd[r]) + f * b->rd_frame_stride);
-        }
+        for (int k = 0; k < kOuts; ++k)
+            if (dout[k]) set_out(d, k, static_cast<uint8_t*>(dout[k]) + f * batch_stride(*b, k));
+        finish_frame(c, d, bulk_ok, frame_luts.empty() ? nullptr : &frame_luts[f]);
     }
-    group_by_lut(hf);
-    const void* fdev = nullptr;
-    e = stream_table(s, 0, hf.data(), F * sizeof(DecodeFrame), &fdev);
-    if (e != cudaSuccess) return fail_cuda(e, "frame table upload");
-    DecodeLaunch a;
-    a.layout_host = &L;
-    a.frames_dev = static_cast<const DecodeFrame*>(fdev);
-    a.n_frames = static_cast<uint32_t>(F);
-    a.lut_dir = ldir;
-    a.lut_off = loff;
-    a.lut_dtype = ldtype;
-    a.shift_host = shifts ? sh.data() : nullptr;
-    a.vec_ok = vec_ok;
-    a.lut_maps = maps_for(L, device, ldir, loff, ldtype);
-    a.lut_an = lut ? lut_analytic(lut) : nullptr;
-    a.frame_luts_have_maps = frame_maps_ok;
-    a.any_xyz = dxyz[0] != nullptr || dxyz[1] != nullptr;
-    a.xyz_base[0] = dxyz[0];
-    a.xyz_base[1] = dxyz[1];
-    a.xyz_frame_stride = b->xyz_frame_stride;
-    e = launch_decode(a, device, st);
-    if (e != cudaSuccess) return fail_cuda(e, "decode launch");
-    e = stg.flush();
-    if (e != cudaSuccess) return fail_cuda(e, "decode D2H");
-    return OB_OK;
+    // the frames' XYZ pointers show a stride that breaks alignment only when there are two of them
+    if (c.any_xyz && b->xyz_frame_stride % 16) c.vec_ok = false;
+    const void* xyz_base[OB_MAX_RETURNS] = {hf[0].xyz[0], hf[0].xyz[1]};
+    return run_table(c, s, hf, stg, xyz_base, b->xyz_frame_stride);
 }
 
 
@@ -441,9 +436,9 @@ static cudaError_t job_reserve(ob_decode_job* j, size_t slots) {
 ob_status ob_decode_job_create(const ob_decoder* dec, size_t reserve_slots, ob_stream* s,
                                ob_decode_job** out) {
     if (!dec || !s || !out) return fail(OB_INVALID_ARGUMENT, "null pointer");
-    const int device = stream_device(s);
-    if (device != dec->device) return fail(OB_INVALID_ARGUMENT, "decoder and stream are on different devices");
-    ob_status rs = require_device(device);
+    const int device = dec->device;
+    ob_status rs = same_device(dec, s);
+    if (rs == OB_OK) rs = require_device(device);
     if (rs != OB_OK) return rs;
     std::unique_ptr<ob_decode_job> j(new ob_decode_job);
     j->dec = dec;
@@ -491,7 +486,7 @@ ob_status ob_decode_job_upload(ob_decode_job* j, const uint8_t* src, size_t src_
     const size_t psize = j->dec->L.packet_size;
     if (count > 1 && src_stride < psize)
         return fail(OB_INVALID_ARGUMENT, "packet_stride smaller than the lidar packet size");
-    if (first_slot + count > (1u << 20)) return fail(OB_INVALID_ARGUMENT, "too many packet slots");
+    if (first_slot + count > kMaxSlots) return fail(OB_INVALID_ARGUMENT, "too many packet slots");
     ob_status rs = require_device(j->device);
     if (rs != OB_OK) return rs;
     if (j->busy) {  // the previous frame still reads the slots
@@ -537,65 +532,34 @@ ob_status ob_decode_job_submit(ob_decode_job* j, const ob_decode_io* io, const o
                                const int32_t* shifts, size_t n_shifts) {
     if (!j || !io) return fail(OB_INVALID_ARGUMENT, "null pointer");
     const DecodeLayout& L = j->dec->L;
-    ob_status rs = require_device(j->device);
+    // the frame's own LUT replaces the call-level one for the whole one-frame launch; the two share one dtype
+    DecodeCall c;
+    ob_status rs = begin_call(c, j->dec, j->s, io->lut ? io->lut : lut, shifts, n_shifts);
     if (rs != OB_OK) return rs;
     if (io->n_slots > j->up_slots) return fail(OB_INVALID_ARGUMENT, "n_slots exceeds the uploaded packet slots");
-    const ob_lut* use_lut = io->lut ? io->lut : lut;
-    const void *ldir = nullptr, *loff = nullptr;
-    int ldtype = OB_F32;
-    if (use_lut) {
-        size_t lh, lw;
-        int ldev;
-        lut_view(use_lut, &ldir, &loff, &ldtype, &lh, &lw, &ldev);
-        if (lh != L.H || lw != L.W) return fail(OB_INVALID_ARGUMENT, "unexpected image dimensions");
-        if (ldev != j->device) return fail(OB_INVALID_ARGUMENT, "lut and stream are on different devices");
-    }
-    std::vector<uint16_t> sh;
-    if (shifts) {
-        if (n_shifts != L.H) return fail(OB_INVALID_ARGUMENT, "image height does not match shifts size");
-        if (L.H > static_cast<uint32_t>(kMaxRows))
-            return fail(OB_INVALID_ARGUMENT, "fused destagger supports at most 512 rows");
-        reduce_shifts(shifts, L.H, L.W, 0, sh);
-    }
-    for (int r = 0; r < OB_MAX_RETURNS; ++r) {
-        if (io->xyz[r] && !use_lut) return fail(OB_INVALID_ARGUMENT, "xyz output requested without a lut");
-        if (io->range_destaggered[r] && !shifts)
-            return fail(OB_INVALID_ARGUMENT, "image height does not match shifts size");
-    }
+    if (io->lut && lut && lut_view(lut).dtype != c.dtype)
+        return fail(OB_INVALID_ARGUMENT, "per-frame lut dtype differs from the call-level lut");
+    if ((rs = check_fused(c, io->lut || lut, io->xyz, io->range_destaggered)) != OB_OK) return rs;
     if (j->busy) {  // the previous submission still owns h_frame / h_colsrc / the slab
         rs = ob_decode_job_wait(j);
         if (rs != OB_OK) return rs;
     }
 
     // ---- outputs: device pointers in place, host pointers through the slab + D2H ----
-    const size_t n_px = static_cast<size_t>(L.H) * L.W;
     struct Out {
         void* user;
         size_t bytes;
-        void** slot;  // where the device pointer goes
+        int k;
         bool host;
         size_t off;
     };
-    DecodeFrame f;
-    std::memset(&f, 0, sizeof(f));
-    Out outs[OB_MAX_FIELDS + 3 + 2 * OB_MAX_RETURNS];
+    Out outs[kOuts];
     size_t n_out = 0;
-    void* fld[OB_MAX_FIELDS] = {};
-    void *ts = nullptr, *mid = nullptr, *stt = nullptr, *xyz[OB_MAX_RETURNS] = {}, *rd[OB_MAX_RETURNS] = {};
-    auto add = [&](void* user, size_t bytes, void** slot) {
-        if (user) outs[n_out++] = Out{user, bytes, slot, false, 0};
-    };
-    for (uint32_t k = 0; k < L.n_fields; ++k) add(io->fields[k], n_px * L.fields[k].elem_size, &fld[k]);
-    add(io->timestamp, static_cast<size_t>(L.W) * 8, &ts);
-    add(io->measurement_id, static_cast<size_t>(L.W) * 2, &mid);
-    add(io->status, static_cast<size_t>(L.W) * 4, &stt);
-    for (int r = 0; r < OB_MAX_RETURNS; ++r) {
-        add(io->xyz[r], n_px * 3 * (ldtype == OB_F64 ? 8 : 4), &xyz[r]);
-        add(io->range_destaggered[r], n_px * 4, &rd[r]);
-    }
+    for (int k = 0; k < kOuts; ++k)
+        if (void* user = io_out(L, *io, k)) outs[n_out++] = Out{user, out_bytes(L, c.dtype, k), k, false, 0};
     // host outputs take slab space in ADDRESS order; buffers that are adjacent in host memory
     // (HostBuffer::carve) stay adjacent in the slab, so their D2H is one copy
-    size_t order[OB_MAX_FIELDS + 3 + 2 * OB_MAX_RETURNS];
+    size_t order[kOuts];
     size_t n_host = 0;
     for (size_t i = 0; i < n_out; ++i) {
         outs[i].host = !is_device_ptr(outs[i].user);
@@ -623,57 +587,24 @@ ob_status ob_decode_job_submit(ob_decode_job* j, const ob_decode_io* io, const o
         if (e != cudaSuccess) return fail_cuda(e, "decode job output slab");
         j->out_bytes = need;
     }
-    for (size_t i = 0; i < n_out; ++i) *outs[i].slot = outs[i].host ? j->d_out + outs[i].off : outs[i].user;
-
-    auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
-    bool vec_ok = !use_lut || (al16(ldir) && al16(loff));
+    DecodeFrame f;
+    std::memset(&f, 0, sizeof(f));
+    for (size_t i = 0; i < n_out; ++i) set_out(f, outs[i].k, outs[i].host ? j->d_out + outs[i].off : outs[i].user);
     f.packets = j->d_pk;
     f.packet_stride = j->stride;
     f.n_slots = static_cast<uint32_t>(io->n_slots);
-    f.flags = 0;
-    if (!io->col_src) f.flags |= 1u;
-    if (L.packet_size % 16 == 0) f.flags |= 2u;  // slots are 16-byte aligned by construction
     if (io->col_src) {
         std::memcpy(j->h_colsrc, io->col_src, static_cast<size_t>(L.W) * 4);
         e = cudaMemcpyAsync(j->d_colsrc, j->h_colsrc, static_cast<size_t>(L.W) * 4, cudaMemcpyHostToDevice, j->st);
         if (e != cudaSuccess) return fail_cuda(e, "stage column map");
         f.col_src = j->d_colsrc;
     }
-    {
-        bool allf = L.n_fields > 0;
-        for (uint32_t k = 0; k < L.n_fields; ++k) {
-            f.fields[k] = fld[k];
-            allf = allf && fld[k] != nullptr;
-        }
-        if (allf) f.flags |= 4u;  // every decoder field has an output image
-    }
-    f.timestamp = static_cast<uint64_t*>(ts);
-    f.measurement_id = static_cast<uint16_t*>(mid);
-    f.status = static_cast<uint32_t*>(stt);
-    for (int r = 0; r < OB_MAX_RETURNS; ++r) {
-        f.xyz[r] = xyz[r];
-        f.rd[r] = static_cast<uint32_t*>(rd[r]);
-        if (xyz[r] && !al16(xyz[r])) vec_ok = false;
-    }
+    finish_frame(c, f, L.packet_size % 16 == 0, nullptr);  // slots are 16-byte aligned by construction
     *j->h_frame = f;
     e = cudaMemcpyAsync(j->d_frame, j->h_frame, sizeof(DecodeFrame), cudaMemcpyHostToDevice, j->st);
     if (e != cudaSuccess) return fail_cuda(e, "frame table upload");
-    DecodeLaunch a;
-    a.layout_host = &L;
-    a.frames_dev = j->d_frame;
-    a.n_frames = 1;
-    a.lut_dir = ldir;
-    a.lut_off = loff;
-    a.lut_dtype = ldtype;
-    a.shift_host = shifts ? sh.data() : nullptr;
-    a.vec_ok = vec_ok;
-    a.lut_maps = maps_for(L, j->device, ldir, loff, ldtype);
-    a.lut_an = use_lut ? lut_analytic(use_lut) : nullptr;
-    a.any_xyz = xyz[0] != nullptr || xyz[1] != nullptr;
-    a.xyz_base[0] = xyz[0];  // a one-frame batch
-    a.xyz_base[1] = xyz[1];
-    a.xyz_frame_stride = static_cast<unsigned long long>(n_px) * 3 * (ldtype == OB_F64 ? 8 : 4);
-    e = launch_decode(a, j->device, j->st);
+    const void* xyz_base[OB_MAX_RETURNS] = {f.xyz[0], f.xyz[1]};  // a one-frame batch
+    e = launch(c, j->d_frame, 1, j->st, xyz_base, out_bytes(L, c.dtype, kOutReturns));  // kOutReturns: XYZ of return 0
     if (e != cudaSuccess) return fail_cuda(e, "decode launch");
     for (size_t k = 0; k < n_host;) {  // one D2H per run of outputs contiguous on both sides
         const Out& first = outs[order[k]];
@@ -698,17 +629,18 @@ ob_status ob_encode_frames(const ob_decoder* dec, const ob_encode_io* frames, si
     if (!dec || !s || (n_frames && !frames)) return fail(OB_INVALID_ARGUMENT, "null pointer");
     if (n_frames == 0) return OB_OK;
     const DecodeLayout& L = dec->L;
-    const int device = stream_device(s);
-    if (device != dec->device) return fail(OB_INVALID_ARGUMENT, "decoder and stream are on different devices");
+    const int device = dec->device;
+    ob_status rs = same_device(dec, s);
+    if (rs != OB_OK) return rs;
     if (L.W % L.cpp != 0)
         return fail(OB_INVALID_ARGUMENT, "Mismatch between expected number of packets and PacketFormat.columns_per_packet");
     if (with_crc && (L.packet_size % 4 != 0 || L.packet_size < 8))
         return fail(OB_INVALID_ARGUMENT, "packet size must be a multiple of 4 for the CRC64 footer");
-    ob_status rs = require_device(device);
+    rs = require_device(device);
     if (rs != OB_OK) return rs;
     cudaStream_t st = stream_handle(s);
     Staging stg(st);
-    const size_t n_px = static_cast<size_t>(L.H) * L.W, n_pk = L.W / L.cpp;
+    const size_t n_pk = L.W / L.cpp;
     std::vector<EncodeFrame> hf(n_frames);
     for (size_t i = 0; i < n_frames; ++i) {
         const ob_encode_io& io = frames[i];
@@ -723,15 +655,15 @@ ob_status ob_encode_frames(const ob_decoder* dec, const ob_encode_io* frames, si
         cudaError_t e = cudaSuccess;
         for (uint32_t k = 0; k < L.n_fields && e == cudaSuccess; ++k) {
             if (!io.fields[k]) continue;
-            e = stg.in(io.fields[k], n_px * L.fields[k].elem_size, &d);
+            e = stg.in(io.fields[k], out_bytes(L, OB_F32, k), &d);
             f.fields[k] = d;
         }
         if (e == cudaSuccess && io.timestamp) {
-            e = stg.in(io.timestamp, static_cast<size_t>(L.W) * 8, &d);
+            e = stg.in(io.timestamp, out_bytes(L, OB_F32, kOutTs), &d);
             f.timestamp = static_cast<const uint64_t*>(d);
         }
         if (e == cudaSuccess && io.status) {
-            e = stg.in(io.status, static_cast<size_t>(L.W) * 4, &d);
+            e = stg.in(io.status, out_bytes(L, OB_F32, kOutStatus), &d);
             f.status = static_cast<const uint32_t*>(d);
         }
         if (e == cudaSuccess && io.packet_headers) {

@@ -77,8 +77,8 @@ __global__ void __launch_bounds__(384, 3) decode_kernel(const __grid_constant__ 
         const DecodeFrame& fr = p.frames[f];
         TileCtl& c = ctl[s];
         uint8_t* st = stage0 + static_cast<size_t>(s) * p.stage_bytes;
-        const bool identity = (fr.flags & 1u) != 0;
-        const bool bulk_ok = (fr.flags & 2u) != 0;
+        const bool identity = (fr.flags & kFrameIdentityMap) != 0;
+        const bool bulk_ok = (fr.flags & kFrameBulkPackets) != 0;
         const unsigned n_groups = (tc + L.cpp - 1) / L.cpp;
         // regular tile: identity map, whole packets present -> no per-column bookkeeping
         if (identity && bulk_ok && (tc % L.cpp) == 0 && (j0 + tc) / L.cpp <= fr.n_slots) {
@@ -136,7 +136,8 @@ __global__ void __launch_bounds__(384, 3) decode_kernel(const __grid_constant__ 
         unsigned f, j0, tc;
         tile_of(k, f, j0, tc);
         const DecodeFrame& fr = p.frames[f];
-        if ((fr.flags & 3u) != 3u || (tc % L.cpp) != 0 || (j0 + tc) / L.cpp > fr.n_slots) return;
+        constexpr uint32_t regular = kFrameIdentityMap | kFrameBulkPackets;
+        if ((fr.flags & regular) != regular || (tc % L.cpp) != 0 || (j0 + tc) / L.cpp > fr.n_slots) return;
         const unsigned slot0 = j0 / L.cpp, n_groups = tc / L.cpp;
         const uint64_t pol = keep ? policy_evict_last() : 0;
         for (unsigned g = 0; g < n_groups; ++g) {
@@ -472,7 +473,7 @@ cudaError_t make_decode_params(const DecodeLaunch& a, int device, bool pipe, Dec
         }
     }
     p.prefetch = static_cast<uint32_t>(std::max(0, tn.decode_prefetch));
-    p.vec_ok = (L.W % 4 == 0) ? 1 : 0;  // caller (ob_decode_frames) also checks pointer alignment
+    p.vec_ok = (L.W % 4 == 0) ? 1 : 0;  // the C-ABI glue (DecodeLaunch::vec_ok) also checks pointer alignment
     p.has_shift = a.shift_host != nullptr ? 1 : 0;
     for (int i = 0; i < kMaxRows; ++i)
         p.shift[i] = (a.shift_host != nullptr && i < static_cast<int>(L.H)) ? a.shift_host[i] : 0;

@@ -240,8 +240,8 @@ __global__ void __launch_bounds__(MAXT, 1)
                 pc.mode = xyz_mode(fr);
                 pc.row_ctr[0] = pc.row_ctr[1] = 0u;
             }
-            const bool identity = (fr.flags & 1u) != 0;
-            const bool bulk_ok = (fr.flags & 2u) != 0;
+            const bool identity = (fr.flags & kFrameIdentityMap) != 0;
+            const bool bulk_ok = (fr.flags & kFrameBulkPackets) != 0;
             const unsigned n_groups = tc >> p.cpp_shift;
             if (identity && bulk_ok && (j0 + tc) / L.cpp <= fr.n_slots) {
                 if (lane != 0) mbar_arrive(&pk_full[s]);  // this lane's part of the table entry is written
@@ -446,7 +446,8 @@ __global__ void __launch_bounds__(MAXT, 1)
             unsigned f, j0;
             tile_of(k, f, j0);
             const DecodeFrame& fr = p.frames[f];
-            if ((fr.flags & 3u) != 3u || (j0 + tc) / L.cpp > fr.n_slots) continue;
+            constexpr uint32_t regular = kFrameIdentityMap | kFrameBulkPackets;
+            if ((fr.flags & regular) != regular || (j0 + tc) / L.cpp > fr.n_slots) continue;
             const unsigned slot0 = j0 / L.cpp, n_groups = tc >> p.cpp_shift;
             for (unsigned gi = 0; gi < n_groups; ++gi)
                 bulk_prefetch_l2(fr.packets + static_cast<size_t>(slot0 + gi) * fr.packet_stride, L.packet_size);

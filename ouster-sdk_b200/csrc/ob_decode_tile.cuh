@@ -457,10 +457,9 @@ __device__ __forceinline__ void decode_static_dyn(const uint8_t* px0, bool col_v
     }
 }
 
-// output mode of a tile for the compile-time layouts (see slot_store): frame flag bit 2 = the host found an output
-// image for every field of the decoder
+// output mode of a tile for the compile-time layouts (see slot_store)
 __device__ __forceinline__ int static_output_mode(const DecodeParams& p, const DecodeFrame& fr) {
-    if (p.layout_all == 0 || (fr.flags & 4u) == 0 || p.n_returns == 0) return 0;
+    if (p.layout_all == 0 || (fr.flags & kFrameAllFields) == 0 || p.n_returns == 0) return 0;
     const bool rd0 = fr.rd[0] != nullptr, rd1 = p.n_returns > 1 ? fr.rd[1] != nullptr : rd0;
     if (rd0 && rd1) return 1;
     if (!rd0 && !(p.n_returns > 1 && fr.rd[1] != nullptr)) return 2;

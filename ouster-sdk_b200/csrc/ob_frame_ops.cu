@@ -425,15 +425,12 @@ ob_status ob_frame_mask_fields(const ob_frame_ops_io* io, ob_stream* s) {
         per_frame[fd.frame].push_back(e);
         if (per_frame[fd.frame].size() > 512) return fail(OB_INVALID_ARGUMENT, "too many fields in one frame");
     }
-    const void* ldir = nullptr;
-    const void* loff = nullptr;
-    int ldtype = 0, ldev = 0;
+    LutView lut{};
     if (a.predicate == OB_FRAME_XYZ_RANGE) {
         if (!a.lut) return fail(OB_INVALID_ARGUMENT, "null pointer");
-        size_t lh = 0, lw = 0;
-        lut_view(a.lut, &ldir, &loff, &ldtype, &lh, &lw, &ldev);
-        if (lh != a.h || lw != a.w) return fail(OB_INVALID_ARGUMENT, "Frame dimensions do not match lut.");
-        if (ldev != stream_device(s)) return fail(OB_INVALID_ARGUMENT, "stream and lut are on different devices");
+        lut = lut_view(a.lut);
+        if (lut.h != a.h || lut.w != a.w) return fail(OB_INVALID_ARGUMENT, "Frame dimensions do not match lut.");
+        if (lut.device != stream_device(s)) return fail(OB_INVALID_ARGUMENT, "stream and lut are on different devices");
     }
     ob_status rs = require_device(stream_device(s));
     if (rs != OB_OK) return rs;
@@ -471,7 +468,7 @@ ob_status ob_frame_mask_fields(const ob_frame_ops_io* io, ob_stream* s) {
     if (e != cudaSuccess) return fail_cuda(e, "stage frame fields");
     const void* dposes = nullptr;
     if (a.predicate == OB_FRAME_XYZ_RANGE && a.poses) {
-        e = stg.in(a.poses, size_t(a.n_frames) * a.w * 16 * (ldtype == OB_F64 ? 8 : 4), &dposes);
+        e = stg.in(a.poses, size_t(a.n_frames) * a.w * 16 * (lut.dtype == OB_F64 ? 8 : 4), &dposes);
         if (e != cudaSuccess) return fail_cuda(e, "stage poses");
     }
     std::vector<uint16_t> sh;
@@ -485,12 +482,12 @@ ob_status ob_frame_mask_fields(const ob_frame_ops_io* io, ob_stream* s) {
         p.npx = uint32_t(npx);
         p.pred = a.predicate;
         p.axis = a.axis;
-        p.lut_f64 = ldtype == OB_F64;
+        p.lut_f64 = lut.dtype == OB_F64;
         p.has_poses = dposes != nullptr;
         p.lo = a.lower;
         p.hi = a.upper;
-        p.dir = ldir;
-        p.off = loff;
+        p.dir = lut.dir;
+        p.off = lut.off;
         p.poses = dposes;
         for (size_t r = 0; r < sh.size(); ++r) p.shift[r] = sh[r];
     };

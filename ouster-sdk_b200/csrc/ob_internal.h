@@ -129,11 +129,16 @@ struct DecodeLayout {
     DecodeField fields[OB_MAX_FIELDS];
 };
 
+// DecodeFrame::flags
+constexpr uint32_t kFrameIdentityMap = 1u;  // col_src is null: column j comes from slot j / cpp, column j % cpp
+constexpr uint32_t kFrameBulkPackets = 2u;  // packets, packet_stride and packet_size are 16-byte aligned
+constexpr uint32_t kFrameAllFields = 4u;    // every decoder field has an output image
+
 struct DecodeFrame {  // one per frame of a batched launch, lives in device memory
     const uint8_t* packets;
     unsigned long long packet_stride;
     uint32_t n_slots;
-    uint32_t flags;          // bit0: identity column map
+    uint32_t flags;          // kFrame* bits
     const int32_t* col_src;  // device, W entries (unused when identity)
     void* fields[OB_MAX_FIELDS];
     uint64_t* timestamp;
@@ -158,7 +163,6 @@ struct DecodeLaunch {
     bool vec_ok;                 // LUT / XYZ pointers are 16-byte aligned
     const void* lut_maps{nullptr};  // TMA descriptors of the launch-level LUT (lut_tensor_maps) or null
     const void* lut_an{nullptr};    // launch-level LUT in LUT-free mode: device LutAnalyticT<T>
-    bool all_regular{false};     // every frame: identity column map, bulk-copyable packets, all slots present
     bool frame_luts_have_maps{true};  // every per-frame LUT of the table carries lut_maps
     // XYZ outputs of a uniformly strided batch (frame f at base + f * stride): lets the pipelined kernel store
     // them with tensor copies; null when the frames' XYZ pointers are unrelated
