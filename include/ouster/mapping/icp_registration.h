@@ -1,7 +1,7 @@
 // icp_registration.h -- ICPRegistration and build_linear_system (mirrors
 // ouster_mapping/include/ouster/mapping/icp_registration.h and ouster_mapping/src/icp_registration.cpp; DESIGN f-6).
 // Same names, defaults and public fields; the iterations run on the GPU (ob_icp_align, ob_icp_linear_system,
-// ouster-sdk_b200/csrc/ob_voxel_map.cu) against a device-resident core::VoxelHashMap3d.
+// ouster-sdk_b200/csrc/ob_voxel_map.cu) against a device-resident core::VoxelHashMap3d or core::VoxelHashMapXd.
 //
 // Eigen is absent (as in ouster/core/typedefs.h): Matrix6d / Vector6d are plain row-major arrays with the accessor
 // names the reference's callers use, Correspondences is a vector of (source, target) core::Vector3d pairs.
@@ -12,8 +12,7 @@
 //    bit (DESIGN 4);
 //  * align_points_to_map's pose agrees with a CPU restatement to about 1e-12: device sin/cos are not host libm
 //    (DESIGN 9);
-//  * max_num_threads_ only reads back (the hardware concurrency when 0 is given); it has no effect on the GPU;
-//  * the align_points_to_map overload for VoxelHashMapXd is not provided.
+//  * max_num_threads_ only reads back (the hardware concurrency when 0 is given); it has no effect on the GPU.
 #pragma once
 #include <array>
 #include <thread>
@@ -72,7 +71,8 @@ inline LinearSystem build_linear_system(const Correspondences& correspondences, 
     return out;
 }
 
-/// ICPRegistration (icp_registration.h): point-to-point ICP with a Geman-McClure kernel against a VoxelHashMap3d.
+/// ICPRegistration (icp_registration.h): point-to-point ICP with a Geman-McClure kernel against a VoxelHashMap3d or a
+/// VoxelHashMapXd (which it reads x, y, z of only).
 struct ICPRegistration {
     explicit ICPRegistration(int max_num_iteration = 50, double convergence_criterion = 0.0001,
                              int max_num_threads = 0)
@@ -87,6 +87,22 @@ struct ICPRegistration {
     /// the map; the identity for an empty map.
     core::Matrix4dR align_points_to_map(const std::vector<core::Vector3d>& frame, const core::VoxelHashMap3d& voxel_map,
                                         const double max_distance, const double kernel_scale) const {
+        return align(frame, voxel_map, max_distance, kernel_scale);
+    }
+    /// align_points_to_map(frame, VoxelHashMapXd, max_distance, kernel_scale) (icp_registration.cpp:205-210): the
+    /// same iterations on the map's x, y, z; the pose is the one a VoxelHashMap3d of the same x, y, z gives
+    core::Matrix4dR align_points_to_map(const std::vector<core::Vector3d>& frame, const core::VoxelHashMapXd& voxel_map,
+                                        const double max_distance, const double kernel_scale) const {
+        return align(frame, voxel_map, max_distance, kernel_scale);
+    }
+
+    int max_num_iterations_;
+    double convergence_criterion_;
+    int max_num_threads_;
+
+   private:
+    core::Matrix4dR align(const std::vector<core::Vector3d>& frame, const core::impl::DeviceVoxelMap& voxel_map,
+                          const double max_distance, const double kernel_scale) const {
         core::Matrix4dR pose;
         ob_icp_io io{};
         io.source.dtype = OB_F64;
@@ -100,10 +116,6 @@ struct ICPRegistration {
         core::b200::check(ob_icp_align(voxel_map.handle(), &io, core::b200::thread_stream()));
         return pose;
     }
-
-    int max_num_iterations_;
-    double convergence_criterion_;
-    int max_num_threads_;
 };
 
 }  // namespace mapping

@@ -54,7 +54,7 @@ int ob_abi_version(void);
  * "ob_voxel_io", "ob_point_rows", "ob_voxel_map_cull_io", "ob_voxel_query_io", "ob_icp_io", "ob_icp_system_io",
  * "ob_cloud_align_io", "ob_cloud_nearest_io", "ob_zone_desc", "ob_zone_render_io", "ob_zone_live", "ob_zone_state",
  * "ob_image_params", "ob_image_state", "ob_frame_field", "ob_frame_ops_io", "ob_frame_rows_entry",
- * "ob_frame_rows_io");
+ * "ob_frame_rows_io", "ob_map_rows", "ob_map_field", "ob_map_rows_item");
  * 0 for unknown names.  Lets FFI bindings verify their layout. */
 size_t ob_abi_sizeof(const char* struct_name);
 const char* ob_last_error(void);
@@ -293,7 +293,7 @@ typedef struct ob_point_rows {
     size_t capacity;        /* rows the buffer holds; used with n_device */
 } ob_point_rows;
 
-typedef struct ob_voxel_map ob_voxel_map; /* VoxelHashMap3d: open-addressing table in device memory */
+typedef struct ob_voxel_map ob_voxel_map; /* VoxelHashMap3d / Xd: open-addressing table in device memory */
 
 /* replaces VoxelHashMap3d(voxel_size, max_distance, max_points_per_voxel, min_pts_threshold)
  *          ouster_core/src/voxel_hash_map.cpp:14-41 (min_pts_threshold is stored and unused, as there)
@@ -301,6 +301,15 @@ typedef struct ob_voxel_map ob_voxel_map; /* VoxelHashMap3d: open-addressing tab
  * "voxel_size must be greater than 0", "max_distance must be greater than 0"; then OB_NO_DEVICE without a GPU. */
 ob_status ob_voxel_map_create(double voxel_size, double max_distance, size_t max_points_per_voxel,
                               size_t min_pts_threshold, int device, ob_voxel_map** out);
+/* replaces VoxelHashMapXd(voxel_size, max_distance, max_points_per_voxel, min_pts_threshold, num_attributes)
+ *          voxel_hash_map.h:352-517 with Eigen::VectorXd points (DESIGN f-11): every point is 3 + num_attributes
+ * doubles, x, y, z first.  Voxels, the first_n_point gate, the cull and every search use x, y, z only; the attributes
+ * ride along.  ob_voxel_map_create is this call with num_attributes = 0.  Same errors in the same order, then
+ * "num_attributes too large" above 65535. */
+ob_status ob_voxel_map_create_xd(double voxel_size, double max_distance, size_t max_points_per_voxel,
+                                 size_t min_pts_threshold, size_t num_attributes, int device, ob_voxel_map** out);
+/* VoxelHashMap::point_cols(): 3 + num_attributes, the row width of every rows x cols buffer of this map */
+ob_status ob_voxel_map_cols(const ob_voxel_map* m, size_t* cols);
 ob_status ob_voxel_map_destroy(ob_voxel_map* m);
 /* replaces VoxelHashMap::clear                      voxel_hash_map.h:387-389 */
 ob_status ob_voxel_map_clear(ob_voxel_map* m, ob_stream* s);
@@ -311,14 +320,31 @@ ob_status ob_voxel_map_clear(ob_voxel_map* m, ob_stream* s);
  * 4 x (live + new voxels) slots (DESIGN 4, f-6).  Growth frees the old table, so a CUDA graph that captured
  * ob_icp_align or ob_voxel_map_closest_neighbors on this map must be captured again.  error (OB_RUNTIME_ERROR):
  * "voxel map: a table of N slots (B bytes) does not fit in free device memory"; on any error the map is unchanged
- * and nothing of the batch is inserted. */
+ * and nothing of the batch is inserted.  A map with attributes refuses this call (OB_INVALID_ARGUMENT,
+ * "VoxelHashMap::add_points received unexpected point dimension"): use ob_voxel_map_add_rows. */
 ob_status ob_voxel_map_add_points(ob_voxel_map* m, const ob_point_rows* rows, ob_stream* s);
+
+/* float64 rows x cols, n rows or a device-resident row count clamped to `capacity` (e.g. the n_rows of
+ * ob_frames_to_map_rows).  Host or device memory. */
+typedef struct ob_map_rows {
+    const double* rows;     /* rows x cols */
+    size_t cols;
+    size_t n;               /* row count when n_device is NULL */
+    const size_t* n_device; /* optional device-resident row count */
+    size_t capacity;        /* rows the buffer holds; used with n_device */
+} ob_map_rows;
+/* replaces VoxelHashMap::add_points(Eigen::Ref<const ArrayXXdR>)   voxel_hash_map.h:399-411
+ * As ob_voxel_map_add_points for rows of any map: the gate reads columns 0-2, an admitted row keeps all its columns,
+ * a rejected row's attributes are dropped.  error: cols != 3 + num_attributes gives "VoxelHashMap::add_points
+ * received unexpected point dimension" (OB_INVALID_ARGUMENT). */
+ob_status ob_voxel_map_add_rows(ob_voxel_map* m, const ob_map_rows* rows, ob_stream* s);
 
 /* replaces remove_voxels_far_from_location / extract_voxels_far_from_location   voxel_hash_map.cpp:109-154
  * origin: 3 doubles, host or device (so a device-resident pose can feed it).  Voxels with
  * |v - v_origin|^2 >= (ceil(max_distance / voxel_size) + 1)^2, in wrapping int32 arithmetic as the reference runs on
  * x86, are erased.  n_extracted != NULL also emits their points (creation order, then slot order) into `extracted`
- * (capacity rows x 3 float64; give it at least the map's point count, ob_voxel_map_size): with a host n_extracted the
+ * (capacity rows x cols float64, cols = ob_voxel_map_cols; give it at least the map's point count, ob_voxel_map_size):
+ * with a host n_extracted the
  * call synchronises once, with a device one nothing waits.  error: "output capacity too small" (the voxels are
  * erased regardless). */
 typedef struct ob_voxel_map_cull_io {
@@ -331,7 +357,8 @@ ob_status ob_voxel_map_remove_far(ob_voxel_map* m, const ob_voxel_map_cull_io* i
 
 /* replaces VoxelHashMap::pointcloud / pointcloud_vector   voxel_hash_map.cpp:43-76
  * Voxels in creation order (the reference: tsl::robin_map order, DESIGN 9), inside a voxel in slot order.
- * points: capacity x 3 float64 (NULL: count only); n_out host (one synchronisation) or device (none). */
+ * points: capacity rows x cols float64 (cols = ob_voxel_map_cols; NULL: count only); n_out host (one
+ * synchronisation) or device (none). */
 ob_status ob_voxel_map_point_cloud(const ob_voxel_map* m, double* points, size_t capacity, size_t* n_out,
                                    ob_stream* s);
 /* live voxels and stored points (VoxelHashMap::empty is voxels == 0); synchronises the stream */
@@ -339,8 +366,9 @@ ob_status ob_voxel_map_size(const ob_voxel_map* m, size_t* voxels, size_t* point
 
 /* replaces VoxelHashMap::get_closest_neighbor(query, max_distance_sq), one query per row   voxel_hash_map.cpp:194-247
  * The 27 voxels in VOXEL_SHIFTS order, each pruned by its AABB lower bound, the first strictly smaller squared
- * distance kept; (0, 0, 0) and max_distance_sq when nothing qualifies.  neighbors: rows x 3 float64;
- * distances_sq (optional): rows float64. */
+ * distance kept; cols zeros and max_distance_sq when nothing qualifies.  Queries are x, y, z.  neighbors: rows x cols
+ * float64 (cols = ob_voxel_map_cols: the neighbour's whole point, attributes included); distances_sq (optional): rows
+ * float64. */
 typedef struct ob_voxel_query_io {
     ob_point_rows queries;
     double max_distance_sq; /* the reference's default is DBL_MAX */
@@ -349,7 +377,7 @@ typedef struct ob_voxel_query_io {
 } ob_voxel_query_io;
 ob_status ob_voxel_map_closest_neighbors(const ob_voxel_map* m, const ob_voxel_query_io* io, ob_stream* s);
 
-/* replaces ICPRegistration::align_points_to_map(frame, VoxelHashMap3d, max_distance, kernel_scale)
+/* replaces ICPRegistration::align_points_to_map(frame, VoxelHashMap3d / VoxelHashMapXd, max_distance, kernel_scale)
  *          ouster_mapping/src/icp_registration.cpp (align_points_to_map_impl, data_association, build_linear_system)
  * Every iteration runs on the stream: association fused with applying the previous increment to the source,
  * order-preserving compaction, the linear system in parallel_deterministic_reduce's tree, and one kernel for the
@@ -366,6 +394,33 @@ typedef struct ob_icp_io {
     int32_t* iterations;
 } ob_icp_io;
 ob_status ob_icp_align(const ob_voxel_map* m, const ob_icp_io* io, ob_stream* s);
+
+/* ---- frame -> map rows: the map exporter's per-return step on the device (DESIGN f-11) ----
+ * replaces, for every item (one return of one frame), python/src/ouster/cli/plugins/map_export.py:589-617:
+ *   valid = range > 0; dewarp(xyzlut_double(range), body_to_world)[valid], then every field's pixels [valid] as
+ *   columns, np.concatenate(..., axis=1).astype(float64)
+ * Output rows are [x, y, z | the fields' channels widened to double, in table order], one per pixel with range > 0,
+ * in row-major pixel order of the staggered image, item i's rows after item i-1's.  The XYZ is K1's projection and
+ * pose arithmetic (bit for bit the ob_cloud_io poses result).  ONE kernel launch (decoupled look-back compaction,
+ * as ob_dewarp_frames).  n_rows in host memory: one stream synchronisation, then "output capacity too small" when
+ * more rows than `capacity` pass.  n_rows in DEVICE memory (rows in device memory too): nothing waits, and a count
+ * above `capacity` means the list was cut there.  Fields are not tone-mapped (the exporter's float16 RGB step).
+ * errors: "map rows need a float64 lut", "unknown field type", "field channels must be at least 1",
+ * "cols must be 3 plus the channels of every item's fields", "too many fields" (more than 16 per item). */
+typedef struct ob_map_field {
+    const void* data;  /* h x w x channels pixels, staggered like the range */
+    int32_t type;      /* ChanFieldType tag (chanfield.h): 1..10, or 12 for float16 */
+    uint32_t channels; /* >= 1 */
+} ob_map_field;
+typedef struct ob_map_rows_item {
+    const ob_lut* lut;          /* float64 (xyzlut_double) */
+    const uint32_t* range;      /* h x w, staggered */
+    const double* poses;        /* w x 16: body_to_world (row-major 4x4 per column) */
+    const ob_map_field* fields; /* host table of n_fields entries */
+    size_t n_fields;
+} ob_map_rows_item;
+ob_status ob_frames_to_map_rows(const ob_map_rows_item* items, size_t n_items, double* rows, size_t cols,
+                                size_t capacity, size_t* n_rows, ob_stream* s);
 
 /* replaces build_linear_system(correspondences, kernel_scale)   ouster_mapping/src/icp_registration.cpp
  * source / target: n x 3 float64 pairs (n or a device count clamped to capacity); jtj: 36 doubles row-major (lower

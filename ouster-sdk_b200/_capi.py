@@ -60,6 +60,21 @@ class PointRows(C.Structure):
     _fields_ = [("dtype", C.c_int32), ("points", vp), ("n", sz), ("n_device", vp), ("capacity", sz)]
 
 
+class MapRows(C.Structure):
+    """ob_map_rows"""
+    _fields_ = [("rows", vp), ("cols", sz), ("n", sz), ("n_device", vp), ("capacity", sz)]
+
+
+class MapField(C.Structure):
+    """ob_map_field"""
+    _fields_ = [("data", vp), ("type", C.c_int32), ("channels", u32)]
+
+
+class MapRowsItem(C.Structure):
+    """ob_map_rows_item"""
+    _fields_ = [("lut", vp), ("range", vp), ("poses", vp), ("fields", C.POINTER(MapField)), ("n_fields", sz)]
+
+
 class VoxelMapCullIO(C.Structure):
     _fields_ = [("origin", vp), ("extracted", vp), ("capacity", sz), ("n_extracted", vp)]
 
@@ -246,6 +261,10 @@ _sig("ob_dewarp_frame", i32, vp, C.POINTER(DewarpFrameIO), C.POINTER(sz), vp)
 _sig("ob_normals", i32, i32, C.POINTER(NormalsIO), vp)
 _sig("ob_voxel_downsample", i32, C.POINTER(VoxelIO), vp)
 _sig("ob_voxel_map_create", i32, C.c_double, C.c_double, sz, sz, i32, C.POINTER(vp))
+_sig("ob_voxel_map_create_xd", i32, C.c_double, C.c_double, sz, sz, sz, i32, C.POINTER(vp))
+_sig("ob_voxel_map_cols", i32, vp, C.POINTER(sz))
+_sig("ob_voxel_map_add_rows", i32, vp, C.POINTER(MapRows), vp)
+_sig("ob_frames_to_map_rows", i32, C.POINTER(MapRowsItem), sz, vp, sz, sz, vp, vp)
 _sig("ob_voxel_map_destroy", i32, vp)
 _sig("ob_voxel_map_clear", i32, vp, vp)
 _sig("ob_voxel_map_add_points", i32, vp, C.POINTER(PointRows), vp)

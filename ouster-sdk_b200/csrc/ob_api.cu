@@ -344,6 +344,9 @@ size_t ob_abi_sizeof(const char* name) {
     if (n == "ob_frame_ops_io") return sizeof(ob_frame_ops_io);
     if (n == "ob_frame_rows_entry") return sizeof(ob_frame_rows_entry);
     if (n == "ob_frame_rows_io") return sizeof(ob_frame_rows_io);
+    if (n == "ob_map_rows") return sizeof(ob_map_rows);
+    if (n == "ob_map_field") return sizeof(ob_map_field);
+    if (n == "ob_map_rows_item") return sizeof(ob_map_rows_item);
     return 0;
 }
 

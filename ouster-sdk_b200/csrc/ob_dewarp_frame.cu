@@ -25,37 +25,12 @@
 #include <algorithm>
 
 #include "ob_internal.h"
+#include "ob_lookback.cuh"
+#include "ob_project.cuh"
 
 namespace ob {
 
 constexpr int kSlabRows = 16;
-
-__device__ __forceinline__ float k3_project(uint32_t r, float d, float o) {
-    return r == 0 ? 0.0f : __fadd_rn(__fmul_rn(static_cast<float>(r), d), o);
-}
-__device__ __forceinline__ double k3_project(uint32_t r, double d, double o) {
-    return r == 0 ? 0.0 : __dadd_rn(__dmul_rn(static_cast<double>(r), d), o);
-}
-__device__ __forceinline__ float k3_pose_row(const float* m, float x, float y, float z) {
-    return __fadd_rn(__fadd_rn(__fmul_rn(m[0], x), __fadd_rn(__fmul_rn(m[1], y), __fmul_rn(m[2], z))), m[3]);
-}
-__device__ __forceinline__ double k3_pose_row(const double* m, double x, double y, double z) {
-    return __dadd_rn(__dadd_rn(__dmul_rn(m[0], x), __dadd_rn(__dmul_rn(m[1], y), __dmul_rn(m[2], z))), m[3]);
-}
-
-__device__ __forceinline__ uint32_t ld_acquire_u32(const uint32_t* p) {
-    uint32_t v;
-    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ void st_release_u32(uint32_t* p, uint32_t v) {
-    asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ unsigned long long warp_sum_u64(unsigned long long v) {
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
-    return v;
-}
 
 // Scratch of one launch (zeroed by the launcher): ticket, then per logical CTA a state word
 // (0 = nothing yet, 1 = aggregate published, 2 = inclusive prefix published) and the two values.
@@ -140,42 +115,7 @@ __global__ void __launch_bounds__(256) k3_fused_kernel(const K3Frame* __restrict
         }
         s_coloff[lane] = on ? incl - mine : 0xffffffffu;
         const unsigned long long aggregate = __shfl_sync(0xffffffffu, incl, 31);
-        if (lane == 0) {
-            if (bid == 0) {
-                sc.incl[0] = aggregate;
-                st_release_u32(&sc.state[0], 2u);
-            } else {
-                sc.agg[bid] = aggregate;
-                st_release_u32(&sc.state[bid], 1u);
-            }
-        }
-        unsigned long long excl = 0;
-        if (bid > 0) {
-            int p = static_cast<int>(bid) - 1;
-            for (;;) {
-                const int idx = p - static_cast<int>(lane);
-                uint32_t st = 2u;  // positions before CTA 0 behave like a published prefix of zero
-                unsigned long long v = 0;
-                if (idx >= 0) {
-                    do {
-                        st = ld_acquire_u32(&sc.state[idx]);
-                    } while (st == 0u);
-                    v = __ldcg(st == 2u ? &sc.incl[idx] : &sc.agg[idx]);
-                }
-                const unsigned pm = __ballot_sync(0xffffffffu, st == 2u);
-                if (pm != 0u) {  // nearest predecessor with an inclusive prefix closes the chain
-                    const unsigned fl = __ffs(pm) - 1u;
-                    excl += warp_sum_u64(lane <= fl ? v : 0ull);
-                    break;
-                }
-                excl += warp_sum_u64(v);
-                p -= 32;
-            }
-            if (lane == 0) {
-                sc.incl[bid] = excl + aggregate;
-                st_release_u32(&sc.state[bid], 2u);
-            }
-        }
+        const unsigned long long excl = lookback_exclusive(Lookback{sc.state, sc.agg, sc.incl}, bid, aggregate, lane);
         if (lane == 0) {
             s_excl = excl;
             if (cg + 1 == fr.n_cg) sc.frame_end[f] = excl + aggregate;
@@ -202,13 +142,13 @@ __global__ void __launch_bounds__(256) k3_fused_kernel(const K3Frame* __restrict
             const uint32_t r = fr.range[px];
             if (r >= min_r && r <= max_r) {
                 if (w < capacity) {
-                    const T x = k3_project(r, dir[px * 3], off[px * 3]);
-                    const T y = k3_project(r, dir[px * 3 + 1], off[px * 3 + 1]);
-                    const T z = k3_project(r, dir[px * 3 + 2], off[px * 3 + 2]);
+                    const T x = project(r, dir[px * 3], off[px * 3]);
+                    const T y = project(r, dir[px * 3 + 1], off[px * 3 + 1]);
+                    const T z = project(r, dir[px * 3 + 2], off[px * 3 + 2]);
                     T* o = points + w * 3;
-                    o[0] = k3_pose_row(m, x, y, z);
-                    o[1] = k3_pose_row(m + 4, x, y, z);
-                    o[2] = k3_pose_row(m + 8, x, y, z);
+                    o[0] = pose_row(m, x, y, z);
+                    o[1] = pose_row(m + 4, x, y, z);
+                    o[2] = pose_row(m + 8, x, y, z);
                     if (frame_idx != nullptr) frame_idx[w] = fr.index;
                     if (col_idx != nullptr) col_idx[w] = col;
                     if (ts_out != nullptr) ts_out[w] = ts;

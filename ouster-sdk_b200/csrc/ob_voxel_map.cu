@@ -14,6 +14,11 @@
 // max_points_per_voxel double3 points.  Erased voxels become tombstones: queries and inserts probe past them, and
 // they are dropped when the table is rebuilt (DESIGN 9).
 //
+// VoxelHashMapXd (DESIGN f-11) is the same table with num_attributes (A) doubles per point in a separate array of
+// cap x max_points_per_voxel x A, allocated only when A > 0: the spatial part stays in the double3 array, so the gate,
+// the cull and the searches read exactly what they read for VoxelHashMap3d (A = 0), and only insertion, the rehash,
+// emission and the closest-neighbour output touch the attributes.
+//
 // add_points keys and stable-sorts the batch by voxel (the downsampling pipeline's keys, sort and first-appearance
 // numbering, ob_voxel_common.cuh), then one thread per distinct voxel finds or claims its slot and runs the
 // first_n_point gate over the voxel's rows in input order, seeded with the points the bucket already holds -- the
@@ -52,6 +57,8 @@ struct ob_voxel_map {
     unsigned long long* stamp;   // cap
     uint32_t* cnt;               // cap
     double* pts;                 // cap x max_pts x 3
+    size_t na;                   // attributes per point (VoxelHashMapXd; 0 for VoxelHashMap3d)
+    double* attr;                // cap x max_pts x na, null when na == 0
     unsigned long long* ctr;     // device counters, see Ctr
     size_t occupied_bound;       // host upper bound of live + tombstone slots
 };
@@ -71,10 +78,22 @@ struct Table {
     uint32_t* cnt;
     double* pts;
     unsigned max_pts;
+    double* attr;  // max_pts x na per slot, null when na == 0
+    unsigned na;
 };
 
 Table table_of(const ob_voxel_map* m) {
-    return Table{m->cap, m->key, m->state, m->stamp, m->cnt, m->pts, static_cast<unsigned>(m->max_pts)};
+    return Table{m->cap,  m->key, m->state, m->stamp, m->cnt, m->pts, static_cast<unsigned>(m->max_pts),
+                 m->attr, static_cast<unsigned>(m->na)};
+}
+
+// columns 0-2 of row `row` of a rows x cols input
+template <typename T>
+__device__ __forceinline__ void load_xyz(const void* base, size_t row, unsigned cols, double* v) {
+    const T* p = static_cast<const T*>(base) + row * cols;
+    v[0] = static_cast<double>(p[0]);
+    v[1] = static_cast<double>(p[1]);
+    v[2] = static_cast<double>(p[2]);
 }
 
 __device__ __forceinline__ unsigned slot_hash(int32_t x, int32_t y, int32_t z, unsigned mask) {
@@ -131,23 +150,24 @@ __device__ int find_or_claim(const Table& t, int32_t x, int32_t y, int32_t z, un
 
 // ---- add_points ----
 template <typename T>
-__global__ void vm_key_kernel(Rows r, double inv, VKey* keys, uint32_t* seq) {
+__global__ void vm_key_kernel(Rows r, unsigned cols, double inv, VKey* keys, uint32_t* seq) {
     const unsigned t = tid_global();
     if (t >= r.cap) return;
     VKey k{1u, 0, 0, 0};
     if (t < rows_n(r)) {
         double v[3];
-        load3<T>(r.p, t, v);
+        load_xyz<T>(r.p, t, cols, v);
         k = VKey{0u, voxel_coord(mul(v[0], inv)), voxel_coord(mul(v[1], inv)), voxel_coord(mul(v[2], inv))};
     }
     keys[t] = k;
     seq[t] = t;
 }
 
-// one thread per distinct voxel of the batch (first-appearance rank r)
+// one thread per distinct voxel of the batch (first-appearance rank r); rows are cols = 3 + t.na wide, the gate reads
+// columns 0-2 and an admitted row's attributes follow it into the slot
 template <typename T>
-__global__ void vm_insert_kernel(Rows r, Table t, unsigned long long* ctr, const VKey* sk, const uint32_t* sseq,
-                                 const uint32_t* vrank, const uint32_t* seg_start, double res_sq) {
+__global__ void vm_insert_kernel(Rows r, unsigned cols, Table t, unsigned long long* ctr, const VKey* sk,
+                                 const uint32_t* sseq, const uint32_t* vrank, const uint32_t* seg_start, double res_sq) {
     const unsigned rank = tid_global();
     if (rank >= r.cap || rank >= vrank[r.cap - 1]) return;
     const unsigned start = seg_start[rank];
@@ -172,7 +192,7 @@ __global__ void vm_insert_kernel(Rows r, Table t, unsigned long long* ctr, const
     unsigned fill = before;
     for (unsigned q = start; q < end && fill < t.max_pts; ++q) {  // first_n_point, voxel_hash_map.h:287-301
         double v[3];
-        load3<T>(r.p, sseq[q], v);
+        load_xyz<T>(r.p, sseq[q], cols, v);
         bool near = false;
         for (unsigned j = 0; j < fill && !near; ++j)
             near = within_resolution(b[3 * j], b[3 * j + 1], b[3 * j + 2], v[0], v[1], v[2], res_sq);
@@ -180,6 +200,11 @@ __global__ void vm_insert_kernel(Rows r, Table t, unsigned long long* ctr, const
             b[3 * fill] = v[0];
             b[3 * fill + 1] = v[1];
             b[3 * fill + 2] = v[2];
+            if (t.na) {
+                const T* src = static_cast<const T*>(r.p) + static_cast<size_t>(sseq[q]) * cols + 3;
+                double* a = t.attr + (static_cast<size_t>(slot) * t.max_pts + fill) * t.na;
+                for (unsigned c = 0; c < t.na; ++c) a[c] = static_cast<double>(src[c]);
+            }
             ++fill;
         }
     }
@@ -206,6 +231,8 @@ __global__ void vm_rehash_kernel(Table o, Table t) {
     t.cnt[j] = o.cnt[i];
     const size_t w = static_cast<size_t>(o.max_pts) * 3;
     for (size_t c = 0; c < static_cast<size_t>(o.cnt[i]) * 3; ++c) t.pts[j * w + c] = o.pts[i * w + c];
+    const size_t wa = static_cast<size_t>(o.max_pts) * o.na;
+    for (size_t c = 0; c < static_cast<size_t>(o.cnt[i]) * o.na; ++c) t.attr[j * wa + c] = o.attr[i * wa + c];
     t.state[j] = kLive;
 }
 
@@ -256,8 +283,12 @@ __global__ void vm_emit_kernel(Table t, const unsigned long long* skeys, const u
     const unsigned c = t.cnt[s];
     const unsigned long long base = off[p] - c;
     const double* b = t.pts + static_cast<size_t>(s) * t.max_pts * 3;
-    for (unsigned k = 0; k < c && base + k < capacity; ++k)
-        for (int d = 0; d < 3; ++d) out[(base + k) * 3 + d] = b[3 * k + d];
+    const double* a = t.attr + static_cast<size_t>(s) * t.max_pts * t.na;
+    const unsigned cols = 3 + t.na;
+    for (unsigned k = 0; k < c && base + k < capacity; ++k) {
+        for (int d = 0; d < 3; ++d) out[(base + k) * cols + d] = b[3 * k + d];
+        for (unsigned d = 0; d < t.na; ++d) out[(base + k) * cols + 3 + d] = a[k * t.na + d];
+    }
 }
 
 // ---- get_closest_neighbor (voxel_hash_map.cpp:194-247) ----
@@ -268,11 +299,15 @@ __constant__ int8_t kShift[27][3] = {
 };
 
 // nearest point to q with squared distance < max_d2, visiting the 27 voxels in VOXEL_SHIFTS order and pruning each by
-// its AABB lower bound; (0,0,0) and max_d2 when nothing qualifies
-__device__ double closest(const Table& t, double inv, double vs, const double* q, double max_d2, double* nb) {
+// its AABB lower bound; (0,0,0) and max_d2 when nothing qualifies.  kAt: *at = the point's index in the attribute
+// array (slot * max_pts + k), or -1
+template <bool kAt = false>
+__device__ double closest(const Table& t, double inv, double vs, const double* q, double max_d2, double* nb,
+                          long long* at = nullptr) {
     const int32_t v[3] = {voxel_coord(mul(q[0], inv)), voxel_coord(mul(q[1], inv)), voxel_coord(mul(q[2], inv))};
     double best = max_d2;
     nb[0] = nb[1] = nb[2] = 0.0;
+    if (kAt) *at = -1;
     for (int s = 0; s < 27; ++s) {
         int32_t w[3];
         double lb = 0.0;
@@ -300,22 +335,30 @@ __device__ double closest(const Table& t, double inv, double vs, const double* q
                 nb[0] = b[3 * k];
                 nb[1] = b[3 * k + 1];
                 nb[2] = b[3 * k + 2];
+                if (kAt) *at = static_cast<long long>(slot) * t.max_pts + k;
             }
         }
     }
     return best;
 }
 
-template <typename T>
+// kAttr: the map has attributes, a neighbour row is 3 + t.na wide (zeros when nothing qualifies,
+// PointDefaultValue::make(point_cols())); without, the search does not track where the neighbour lives
+template <typename T, bool kAttr>
 __global__ void vm_closest_kernel(Rows r, Table t, double inv, double vs, double max_d2, double* nb, double* d2) {
     const unsigned i = tid_global();
     if (i >= r.cap || i >= rows_n(r)) return;
     double q[3], p[3];
     load3<T>(r.p, i, q);
-    const double best = closest(t, inv, vs, q, max_d2, p);
-    nb[3 * i] = p[0];
-    nb[3 * i + 1] = p[1];
-    nb[3 * i + 2] = p[2];
+    long long at = -1;
+    const double best = closest<kAttr>(t, inv, vs, q, max_d2, p, &at);
+    const unsigned cols = kAttr ? 3 + t.na : 3;
+    double* o = nb + static_cast<size_t>(i) * cols;
+    o[0] = p[0];
+    o[1] = p[1];
+    o[2] = p[2];
+    if (kAttr)
+        for (unsigned d = 0; d < t.na; ++d) o[3 + d] = at >= 0 ? t.attr[static_cast<size_t>(at) * t.na + d] : 0.0;
     if (d2) d2[i] = best;
 }
 
@@ -663,15 +706,17 @@ void free_table(ob_voxel_map* m) {
     cudaFree(m->stamp);
     cudaFree(m->cnt);
     cudaFree(m->pts);
+    cudaFree(m->attr);
     m->key = nullptr;
     m->state = nullptr;
     m->stamp = nullptr;
     m->cnt = nullptr;
     m->pts = nullptr;
+    m->attr = nullptr;
     m->cap = 0;
 }
 
-size_t table_bytes(size_t cap, size_t max_pts) { return cap * (12 + 4 + 8 + 4 + 24 * max_pts); }
+size_t table_bytes(size_t cap, size_t max_pts, size_t na) { return cap * (12 + 4 + 8 + 4 + (24 + 8 * na) * max_pts); }
 
 // a new, empty table in `t` (only its arrays and cap); on failure everything allocated here is freed again
 cudaError_t alloc_table(ob_voxel_map* t, unsigned cap, cudaStream_t st) {
@@ -680,12 +725,14 @@ cudaError_t alloc_table(ob_voxel_map* t, unsigned cap, cudaStream_t st) {
     t->stamp = nullptr;
     t->cnt = nullptr;
     t->pts = nullptr;
+    t->attr = nullptr;
     t->cap = cap;
     cudaError_t e = cudaMalloc(&t->key, cap * 12ull);
     if (e == cudaSuccess) e = cudaMalloc(&t->state, cap * 4ull);
     if (e == cudaSuccess) e = cudaMalloc(&t->stamp, cap * 8ull);
     if (e == cudaSuccess) e = cudaMalloc(&t->cnt, cap * 4ull);
     if (e == cudaSuccess) e = cudaMalloc(&t->pts, cap * t->max_pts * 24ull);
+    if (e == cudaSuccess && t->na) e = cudaMalloc(&t->attr, cap * t->max_pts * t->na * 8ull);
     if (e == cudaSuccess) e = cudaMemsetAsync(t->state, 0, cap * 4ull, st);
     if (e != cudaSuccess) {
         cudaGetLastError();
@@ -721,9 +768,9 @@ ob_status reserve(ob_voxel_map* m, size_t rows, const uint32_t* nv_dev, cudaStre
     size_t free_b = 0, total_b = 0;
     e = cudaMemGetInfo(&free_b, &total_b);
     if (e != cudaSuccess) return fail_cuda(e, "voxel map allocation");
-    if (cap > (1ull << 31) || table_bytes(cap, m->max_pts) > free_b)
+    if (cap > (1ull << 31) || table_bytes(cap, m->max_pts, m->na) > free_b)
         return fail(OB_RUNTIME_ERROR, "voxel map: a table of " + std::to_string(cap) + " slots (" +
-                                          std::to_string(table_bytes(cap, m->max_pts)) +
+                                          std::to_string(table_bytes(cap, m->max_pts, m->na)) +
                                           " bytes) does not fit in free device memory");
     ob_voxel_map nt = *m;
     e = alloc_table(&nt, static_cast<unsigned>(cap), st);
@@ -748,6 +795,7 @@ ob_status reserve(ob_voxel_map* m, size_t rows, const uint32_t* nv_dev, cudaStre
     m->stamp = nt.stamp;
     m->cnt = nt.cnt;
     m->pts = nt.pts;
+    m->attr = nt.attr;
     m->occupied_bound = live;
     return OB_OK;
 }
@@ -759,7 +807,7 @@ struct AddBatch {
 };
 
 template <typename T>
-cudaError_t sort_batch(const ob_voxel_map* m, Rows r, Staging& stg, cudaStream_t st, AddBatch* b) {
+cudaError_t sort_batch(const ob_voxel_map* m, Rows r, unsigned cols, Staging& stg, cudaStream_t st, AddBatch* b) {
     const unsigned cap = r.cap;
     const unsigned nb = blocks_for(cap);
     VKey* keys;
@@ -781,7 +829,7 @@ cudaError_t sort_batch(const ob_voxel_map* m, Rows r, Staging& stg, cudaStream_t
     void* tmp = nullptr;
     if (e == cudaSuccess) e = stg.scratch(tmp_bytes, &tmp);
     if (e != cudaSuccess) return e;
-    vm_key_kernel<T><<<nb, 256, 0, st>>>(r, m->inv, keys, seq);
+    vm_key_kernel<T><<<nb, 256, 0, st>>>(r, cols, m->inv, keys, seq);
     e = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, b->sk, seq, b->sseq, static_cast<int>(cap),
                                         VKeyDecomposer{}, 0, kKeyBits, st);
     if (e != cudaSuccess) return e;
@@ -796,9 +844,9 @@ cudaError_t sort_batch(const ob_voxel_map* m, Rows r, Staging& stg, cudaStream_t
 
 // the second half: every distinct voxel of the batch into the table
 template <typename T>
-cudaError_t insert_batch(ob_voxel_map* m, Rows r, const AddBatch& b, cudaStream_t st) {
-    vm_insert_kernel<T><<<blocks_for(r.cap), 256, 0, st>>>(r, table_of(m), m->ctr, b.sk, b.sseq, b.vrank, b.seg_start,
-                                                            m->res_sq);
+cudaError_t insert_batch(ob_voxel_map* m, Rows r, unsigned cols, const AddBatch& b, cudaStream_t st) {
+    vm_insert_kernel<T><<<blocks_for(r.cap), 256, 0, st>>>(r, cols, table_of(m), m->ctr, b.sk, b.sseq, b.vrank,
+                                                            b.seg_start, m->res_sq);
     vm_advance_stamp_kernel<<<1, 1, 0, st>>>(r.cap, b.vrank, m->ctr);
     count_launch(2);
     count_launch_of(OB_FAM_VOXEL_MAP, 2);
@@ -848,9 +896,10 @@ ob_status emit_rows(const ob_voxel_map* m, const uint32_t* sel, Staging& stg, cu
     const bool dev_count = is_device_ptr(n_out);
     const bool host_out = out && !is_device_ptr(out);
     if (dev_count && host_out) return fail(OB_INVALID_ARGUMENT, "a device-side count needs device outputs");
+    const size_t row_bytes = (3 + m->na) * 8;
     double* dout = out;
     cudaError_t e = cudaSuccess;
-    if (host_out && capacity) e = scratch(stg, capacity * 24, &dout);
+    if (host_out && capacity) e = scratch(stg, capacity * row_bytes, &dout);
     unsigned long long* dn = reinterpret_cast<unsigned long long*>(n_out);
     if (e == cudaSuccess && !dev_count) e = scratch(stg, 8, &dn);
     if (e == cudaSuccess) e = run_emit(m, sel, stg, st, dout, out ? capacity : 0, dn);
@@ -860,7 +909,7 @@ ob_status emit_rows(const ob_voxel_map* m, const uint32_t* sel, Staging& stg, cu
     e = cudaMemcpyAsync(&total, dn, 8, cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     if (e == cudaSuccess && host_out && total)
-        e = cudaMemcpyAsync(out, dout, std::min<size_t>(total, capacity) * 24, cudaMemcpyDeviceToHost, st);
+        e = cudaMemcpyAsync(out, dout, std::min<size_t>(total, capacity) * row_bytes, cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess && host_out) e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail_cuda(e, what);
     *n_out = static_cast<size_t>(total);
@@ -878,18 +927,40 @@ int32_t cull_threshold(double max_distance, double inv) {
 // leaf values of the deterministic-reduce tree for up to `cap` pairs
 unsigned tree_slots(size_t cap) { return 1u << tree_depth(cap); }
 
+// sort, make room, insert: the body of ob_voxel_map_add_points / _add_rows for staged rows of `cols` columns
+ob_status add_batch(ob_voxel_map* m, Rows r, unsigned cols, bool f64, Staging& stg, cudaStream_t st) {
+    AddBatch b{};
+    cudaError_t e = f64 ? sort_batch<double>(m, r, cols, stg, st, &b) : sort_batch<float>(m, r, cols, stg, st, &b);
+    if (e != cudaSuccess) return fail_cuda(e, "voxel map add_points");
+    size_t added = 0;
+    ob_status rs = reserve(m, r.cap, b.vrank + r.cap - 1, st, &added);
+    if (rs != OB_OK) return rs;  // nothing inserted; the map is as it was
+    e = f64 ? insert_batch<double>(m, r, cols, b, st) : insert_batch<float>(m, r, cols, b, st);
+    if (e != cudaSuccess) return fail_cuda(e, "voxel map add_points");
+    m->occupied_bound += added;
+    return OB_OK;
+}
+
+const char* const kDimensionError = "VoxelHashMap::add_points received unexpected point dimension";
+
 }  // namespace
 
 extern "C" {
 
 ob_status ob_voxel_map_create(double voxel_size, double max_distance, size_t max_points_per_voxel,
                               size_t min_pts_threshold, int device, ob_voxel_map** out) {
+    return ob_voxel_map_create_xd(voxel_size, max_distance, max_points_per_voxel, min_pts_threshold, 0, device, out);
+}
+
+ob_status ob_voxel_map_create_xd(double voxel_size, double max_distance, size_t max_points_per_voxel,
+                                 size_t min_pts_threshold, size_t num_attributes, int device, ob_voxel_map** out) {
     if (!out) return fail(OB_INVALID_ARGUMENT, "null output pointer");
     // the constructor's checks in its order (voxel_hash_map.cpp:23-31)
     if (max_points_per_voxel == 0) return fail(OB_INVALID_ARGUMENT, "max_points_per_voxel must be greater than 0");
     if (voxel_size <= 0) return fail(OB_INVALID_ARGUMENT, "voxel_size must be greater than 0");
     if (max_distance <= 0) return fail(OB_INVALID_ARGUMENT, "max_distance must be greater than 0");
     if (max_points_per_voxel > 0xffffu) return fail(OB_INVALID_ARGUMENT, "max_points_per_voxel too large");
+    if (num_attributes > 0xffffu) return fail(OB_INVALID_ARGUMENT, "num_attributes too large");
     ob_status rs = require_device(device);
     if (rs != OB_OK) return rs;
     ob_voxel_map* m = new ob_voxel_map{};
@@ -898,6 +969,7 @@ ob_status ob_voxel_map_create(double voxel_size, double max_distance, size_t max
     m->max_distance = max_distance;
     m->max_pts = max_points_per_voxel;
     m->min_pts = min_pts_threshold;
+    m->na = num_attributes;
     m->res_sq = voxel_size * voxel_size / static_cast<double>(max_points_per_voxel);  // :38
     m->inv = 1.0 / voxel_size;                                                          // :39
     cudaError_t e = cudaMalloc(&m->ctr, C_WORDS * 8);
@@ -934,8 +1006,15 @@ ob_status ob_voxel_map_clear(ob_voxel_map* m, ob_stream* s) {
     return OB_OK;
 }
 
+ob_status ob_voxel_map_cols(const ob_voxel_map* m, size_t* cols) {
+    if (!m || !cols) return fail(OB_INVALID_ARGUMENT, "null pointer");
+    *cols = 3 + m->na;
+    return OB_OK;
+}
+
 ob_status ob_voxel_map_add_points(ob_voxel_map* m, const ob_point_rows* rows, ob_stream* s) {
     if (!m || !rows || !s) return fail(OB_INVALID_ARGUMENT, "null pointer");
+    if (m->na) return fail(OB_INVALID_ARGUMENT, kDimensionError);
     ob_status rs = require_device(m->device);
     if (rs != OB_OK) return rs;
     cudaStream_t st = stream_handle(s);
@@ -943,17 +1022,27 @@ ob_status ob_voxel_map_add_points(ob_voxel_map* m, const ob_point_rows* rows, ob
     Rows r{};
     rs = stage_rows(rows, stg, &r, "stage voxel map rows");
     if (rs != OB_OK || r.cap == 0) return rs;
-    const bool f64 = rows->dtype == OB_F64;
-    AddBatch b{};
-    cudaError_t e = f64 ? sort_batch<double>(m, r, stg, st, &b) : sort_batch<float>(m, r, stg, st, &b);
-    if (e != cudaSuccess) return fail_cuda(e, "voxel map add_points");
-    size_t added = 0;
-    rs = reserve(m, r.cap, b.vrank + r.cap - 1, st, &added);
-    if (rs != OB_OK) return rs;  // nothing inserted; the map is as it was
-    e = f64 ? insert_batch<double>(m, r, b, st) : insert_batch<float>(m, r, b, st);
-    if (e != cudaSuccess) return fail_cuda(e, "voxel map add_points");
-    m->occupied_bound += added;
-    return OB_OK;
+    return add_batch(m, r, 3, rows->dtype == OB_F64, stg, st);
+}
+
+ob_status ob_voxel_map_add_rows(ob_voxel_map* m, const ob_map_rows* rows, ob_stream* s) {
+    if (!m || !rows || !s) return fail(OB_INVALID_ARGUMENT, "null pointer");
+    if (rows->cols != 3 + m->na) return fail(OB_INVALID_ARGUMENT, kDimensionError);
+    ob_status rs = require_device(m->device);
+    if (rs != OB_OK) return rs;
+    const bool dev_n = rows->n_device != nullptr;
+    const size_t cap = dev_n ? rows->capacity : rows->n;
+    if (cap > 0x7fffffffu) return fail(OB_INVALID_ARGUMENT, "too many points in one call");
+    if (dev_n && !is_device_ptr(rows->n_device)) return fail(OB_INVALID_ARGUMENT, "n_device must be device memory");
+    if (cap && !rows->rows) return fail(OB_INVALID_ARGUMENT, "null rows buffer");
+    if (cap == 0) return OB_OK;
+    cudaStream_t st = stream_handle(s);
+    Staging stg(st);
+    const void* d = nullptr;
+    cudaError_t e = stg.in(rows->rows, cap * rows->cols * 8, &d);
+    if (e != cudaSuccess) return fail_cuda(e, "stage voxel map rows");
+    const Rows r{d, reinterpret_cast<const unsigned long long*>(rows->n_device), rows->n, static_cast<unsigned>(cap)};
+    return add_batch(m, r, static_cast<unsigned>(rows->cols), true, stg, st);
 }
 
 ob_status ob_voxel_map_remove_far(ob_voxel_map* m, const ob_voxel_map_cull_io* io, ob_stream* s) {
@@ -1035,16 +1124,15 @@ ob_status ob_voxel_map_closest_neighbors(const ob_voxel_map* m, const ob_voxel_q
     if (rs != OB_OK || r.cap == 0) return rs;
     if (!io->neighbors) return fail(OB_INVALID_ARGUMENT, "null neighbors buffer");
     void *nb = nullptr, *d2 = nullptr;
-    cudaError_t e = stg.out(io->neighbors, r.cap * 24ull, &nb);
+    cudaError_t e = stg.out(io->neighbors, r.cap * (3 + m->na) * 8ull, &nb);
     if (e == cudaSuccess) e = stg.out(io->distances_sq, r.cap * 8ull, &d2);
     if (e != cudaSuccess) return fail_cuda(e, "stage neighbors");
     const Table t = table_of(m);
-    if (io->queries.dtype == OB_F64)
-        vm_closest_kernel<double><<<blocks_for(r.cap), 256, 0, st>>>(r, t, m->inv, m->voxel_size, io->max_distance_sq,
-                                                                      static_cast<double*>(nb), static_cast<double*>(d2));
-    else
-        vm_closest_kernel<float><<<blocks_for(r.cap), 256, 0, st>>>(r, t, m->inv, m->voxel_size, io->max_distance_sq,
-                                                                     static_cast<double*>(nb), static_cast<double*>(d2));
+    const bool f64 = io->queries.dtype == OB_F64, attr = m->na != 0;
+    auto kern = f64 ? (attr ? vm_closest_kernel<double, true> : vm_closest_kernel<double, false>)
+                    : (attr ? vm_closest_kernel<float, true> : vm_closest_kernel<float, false>);
+    kern<<<blocks_for(r.cap), 256, 0, st>>>(r, t, m->inv, m->voxel_size, io->max_distance_sq, static_cast<double*>(nb),
+                                            static_cast<double*>(d2));
     count_launch();
     count_launch_of(OB_FAM_VOXEL_MAP);
     e = cudaGetLastError();

@@ -264,6 +264,10 @@ class DeviceLidarScan:
         identical bits; `.view(torch.uint16)` etc. where torch has the type)."""
         return self._fields[name]
 
+    def field_dtype(self, name):
+        """The field's numpy dtype in the reference (e.g. uint16 for a field held in an int16 tensor)."""
+        return self.host.field(name).dtype
+
     # headers, as on LidarScan
     timestamp = property(lambda self: self.host.timestamp)
     measurement_id = property(lambda self: self.host.measurement_id)
@@ -350,12 +354,18 @@ def _rows3(points, msg="add_points expects an Nx3 array"):
     return p
 
 
-class VoxelHashMap3d:
-    """core.VoxelHashMap3d: first_n_point voxel map, held in device memory.  point_cloud() and
-    extract_voxels_far_from_location() list voxels in creation order (the reference: hash-map order, DESIGN 9)."""
+def _point_xd(point):
+    """x, y, z of a (3 + attributes)-element point (VoxelHashMapXd reads the spatial part only)."""
+    d = _dev(point)
+    p = d.double().reshape(-1) if d is not None else np.ascontiguousarray(point, np.float64).reshape(-1)
+    if p.shape[0] < 3:
+        raise ValueError("VoxelHashMap method expects a (3+attributes)-element point")
+    return p[:3]
 
-    def __init__(self, voxel_size=0.1, max_distance=100.0, max_points_per_voxel=20, min_pts_threshold=1):
-        self._m = _c.VoxelMap(voxel_size, max_distance, max_points_per_voxel, min_pts_threshold)
+
+class _VoxelHashMap:
+    """What VoxelHashMap3d and VoxelHashMapXd share (bind_voxel_hash_map_common, processing.cpp:396-470); the
+    subclasses say how a point and a batch of rows are read."""
 
     @property
     def empty(self):
@@ -371,28 +381,72 @@ class VoxelHashMap3d:
         self._m.clear()
 
     def add_points(self, points):
-        self._m.add_points(_rows3(points))
+        self._m.add_points(self._rows(points))
 
     def point_cloud(self):
         return self._m.point_cloud()
 
     def remove_voxels_far_from_location(self, point):
-        self._m.remove_far(_point3(point))
+        self._m.remove_far(self._point(point))
 
     def extract_voxels_far_from_location(self, point):
-        return self._m.remove_far(_point3(point), extract=True)
+        return self._m.remove_far(self._point(point), extract=True)
 
     def get_closest_neighbor(self, point, max_distance_sq=DBL_MAX):
-        """(closest point [3] float64, squared distance); ((0, 0, 0), max_distance_sq) when nothing qualifies."""
-        p = _point3(point)
+        """(closest point [cols] float64, squared distance); (zeros, max_distance_sq) when nothing qualifies."""
+        p = self._point(point)
         nb, d2 = self._m.closest_neighbors(p.reshape(1, 3), max_distance_sq)
         if _c._is_torch(nb):
             nb, d2 = nb.cpu().numpy(), d2.cpu().numpy()
         return nb[0], float(d2[0])
 
+
+class VoxelHashMap3d(_VoxelHashMap):
+    """core.VoxelHashMap3d: first_n_point voxel map, held in device memory.  point_cloud() and
+    extract_voxels_far_from_location() list voxels in creation order (the reference: hash-map order, DESIGN 9)."""
+
+    def __init__(self, voxel_size=0.1, max_distance=100.0, max_points_per_voxel=20, min_pts_threshold=1):
+        self._m = _c.VoxelMap(voxel_size, max_distance, max_points_per_voxel, min_pts_threshold)
+
+    _point = staticmethod(_point3)
+    _rows = staticmethod(_rows3)
+
     def get_closest_neighbors(self, points, max_distance_sq=DBL_MAX):
         """Batched get_closest_neighbor: (points [n, 3], squared distances [n]); CUDA tensors in, CUDA tensors out."""
         return self._m.closest_neighbors(_rows3(points, "VoxelHashMap method expects a 3-element point"),
+                                         max_distance_sq)
+
+
+class VoxelHashMapXd(_VoxelHashMap):
+    """core.VoxelHashMapXd (processing.cpp:1058-1067): the first_n_point map with num_attributes doubles after x, y, z
+    in every point, held in device memory (DESIGN f-11).  Voxels, the gate and the searches use x, y, z; rows come out
+    3 + num_attributes wide, in creation order."""
+
+    def __init__(self, voxel_size=0.1, max_distance=100.0, max_points_per_voxel=20, min_pts_threshold=1,
+                 num_attributes=0):
+        self._m = _c.VoxelMap(voxel_size, max_distance, max_points_per_voxel, min_pts_threshold,
+                              num_attributes=num_attributes)
+
+    _point = staticmethod(_point_xd)
+
+    def add_points(self, points):
+        """Rows of 3 + num_attributes columns; even with no attributes this is the rows call, whose width error is
+        the reference's"""
+        self._m.add_rows(self._rows(points))
+
+    @staticmethod
+    def _rows(points):
+        d = _dev(points)
+        p = d if d is not None else np.ascontiguousarray(points, np.float64)
+        if len(p.shape) != 2 or p.shape[1] < 3:
+            raise ValueError("add_points expects at least Nx(3+num_attributes) columns")
+        return p
+
+    def get_closest_neighbors(self, points, max_distance_sq=DBL_MAX):
+        """Batched get_closest_neighbor on the first three columns of `points`: (rows [n, 3 + num_attributes],
+        squared distances [n]); CUDA tensors in, CUDA tensors out."""
+        p = self._rows(points)
+        return self._m.closest_neighbors(p[:, :3] if _c._is_torch(p) else np.ascontiguousarray(p[:, :3]),
                                          max_distance_sq)
 
 
@@ -408,7 +462,7 @@ class ICPRegistration:
 
     def align_points_to_map(self, frame, voxel_map, max_distance, kernel_scale):
         """4x4 float64 correction that moves `frame` onto the map (a CUDA tensor for a CUDA-tensor frame)."""
-        m = voxel_map._m if isinstance(voxel_map, VoxelHashMap3d) else voxel_map
+        m = voxel_map._m if isinstance(voxel_map, _VoxelHashMap) else voxel_map
         pose, _ = _c.icp_align(m, _rows3(frame), max_distance, kernel_scale, self.max_num_iterations,
                                self.convergence_criterion)
         return pose

@@ -299,6 +299,23 @@ vp, vit = ob.icp_align(gm, om.point_cloud() + 0.02, 1.0, 0.5, 10)
 wp, wit = oi.align_points_to_map(om.point_cloud() + 0.02, om, 1.0, 0.5, 10)
 assert vit == wit and np.abs(vp - wp).max() <= 1e-12
 print("voxel map / icp ok")
+# voxel map with attributes (growth, cull with extraction, neighbours with attributes) and the frame -> map-row ingest
+from tests import voxel_map_xd_reference as xr
+gx, xx = ob.VoxelMap(0.5, 3.0, 3, num_attributes=2), xr.VoxelHashMapXd(0.5, 3.0, 3, num_attributes=2)
+for k in range(3):
+    xrows = np.hstack([rs.normal(k, 2.0, (1500, 3)), rs.normal(0, 1.0, (1500, 2))])
+    gx.add_points(xrows)
+    xx.add_points(xrows)
+    assert np.array_equal(gx.remove_far([k, 0, 0], extract=True), xx.extract_voxels_far_from_location([k, 0, 0]))
+assert all(np.array_equal(a, b) for a, b in zip(gx.closest_neighbors(vq, 1.0), xx.get_closest_neighbors(vq, 1.0)))
+mh, mw = 16, 64
+mr = (rs.integers(0, 5000, (mh, mw)) * (rs.random((mh, mw)) > 0.2)).astype(np.uint32)
+md = rs.normal(0, 1.0, (mh * mw, 3))
+mlut = ob.XYZLutT.from_arrays(md, np.zeros_like(md), mh, mw)
+mitem = {"range": mr, "poses": np.repeat(np.eye(4)[None], mw, 0), "direction": md, "offset": np.zeros_like(md),
+         "fields": [rs.integers(0, 255, (mh, mw)).astype(np.uint8), rs.normal(0, 1, (mh, mw, 3)).astype(np.float16)]}
+assert np.array_equal(ob.map_rows([dict(mitem, lut=mlut)] * 2), xr.map_rows([mitem] * 2))
+print("voxel map xd / map rows ok")
 # cloud-to-cloud ICP: nearest with NaN / 1e300 rows and bad normals, both aligns (f32 and f64)
 from oracle import align as oa
 rs = np.random.default_rng(12)
