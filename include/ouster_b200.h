@@ -155,11 +155,13 @@ ob_status ob_dewarp(ob_dtype dtype, const void* points, const void* poses, size_
  * (body_to_world cast to the LUT dtype) -- the reference's order and arithmetic, without
  * materialising the full cloud first (the fusion its own note at dewarp_impl.h:27-29 asks for).
  * ONE kernel launch (count, decoupled look-back scan and emit fused; the count is a device-side word).
- * n_points in host memory: the call returns after the count is known (one stream synchronisation; host
- * outputs are final on return, device outputs after ob_stream_sync) and raises
- * "output capacity too small" when more than `capacity` points pass the filter.
+ * n_points in host memory: the call waits for the count and, when outputs are in host memory, then for their
+ * points (host outputs are final on return, device outputs after ob_stream_sync); it raises
+ * "output capacity too small" when more than `capacity` points pass the filter, with *n_points left 0 and the
+ * host outputs untouched.
  * n_points in DEVICE memory (8 bytes; all outputs in device memory): nothing waits for the GPU, the count is
- * written in stream order next to the points, and a count above `capacity` means the list was cut there.
+ * written in stream order next to the points, and a count above `capacity` means the list was cut there.  A host
+ * output with a device n_points is refused before anything is launched, with the count 0.
  */
 typedef struct ob_dewarp_frame_io {
     const uint32_t* range;       /* h x w, staggered (the RANGE field) */
@@ -249,8 +251,9 @@ ob_status ob_normals(ob_dtype dtype, const ob_normals_io* io, ob_stream* s);
  * input before any check; POINT_NORMAL skips rows with a non-finite point or normal or a normal of norm <= 1e-12.
  * Row count: n (host) or, when n_device is set, a device word read in stream order (values above `capacity` are
  * clamped; work is launched for `capacity` rows, parameters are checked whenever capacity > 0).  n_out may be
- * host memory (the call synchronises once and host outputs are final on return) or device memory (nothing waits;
- * all outputs must then be device memory).  Output buffers hold `capacity` (or n) rows.
+ * host memory (the call waits for the count, then for the rows of host outputs, which are final on return) or
+ * device memory (nothing waits; all outputs must then be device memory).  Output buffers hold `capacity` (or n)
+ * rows.
  * errors (OB_INVALID_ARGUMENT, the reference's std::invalid_argument texts): "max_points_per_voxel must be greater
  * than 0" (checked first), "voxel_size must be greater than 0", "voxel_downsample_xd: frame must have at least 3
  * columns", "voxel_downsample_with_normals expects Nx3 inputs", "voxel_downsample_with_normals voxel_size must be > 0".
@@ -344,9 +347,11 @@ ob_status ob_voxel_map_add_rows(ob_voxel_map* m, const ob_map_rows* rows, ob_str
  * |v - v_origin|^2 >= (ceil(max_distance / voxel_size) + 1)^2, in wrapping int32 arithmetic as the reference runs on
  * x86, are erased.  n_extracted != NULL also emits their points (creation order, then slot order) into `extracted`
  * (capacity rows x cols float64, cols = ob_voxel_map_cols; give it at least the map's point count, ob_voxel_map_size):
- * with a host n_extracted the
- * call synchronises once, with a device one nothing waits.  error: "output capacity too small" (the voxels are
- * erased regardless). */
+ * with a host n_extracted the call waits for the count and, for a host `extracted`, then for the rows; more rows
+ * than `capacity` fail "output capacity too small" (the voxels are erased regardless) with *n_extracted left 0 and
+ * `extracted` untouched.  With a device n_extracted nothing waits, rows past `capacity` are cut and the count is the
+ * true total; a host `extracted` is then refused before the cull, leaving the map unchanged.  extracted == NULL
+ * counts only. */
 typedef struct ob_voxel_map_cull_io {
     const double* origin;
     double* extracted;
@@ -357,8 +362,8 @@ ob_status ob_voxel_map_remove_far(ob_voxel_map* m, const ob_voxel_map_cull_io* i
 
 /* replaces VoxelHashMap::pointcloud / pointcloud_vector   voxel_hash_map.cpp:43-76
  * Voxels in creation order (the reference: tsl::robin_map order, DESIGN 9), inside a voxel in slot order.
- * points: capacity rows x cols float64 (cols = ob_voxel_map_cols; NULL: count only); n_out host (one
- * synchronisation) or device (none). */
+ * points: capacity rows x cols float64 (cols = ob_voxel_map_cols; NULL: count only); n_out host or device, with
+ * the capacity rule of ob_voxel_map_remove_far's extraction (a count-only call never exceeds it). */
 ob_status ob_voxel_map_point_cloud(const ob_voxel_map* m, double* points, size_t capacity, size_t* n_out,
                                    ob_stream* s);
 /* live voxels and stored points (VoxelHashMap::empty is voxels == 0); synchronises the stream */
@@ -402,9 +407,9 @@ ob_status ob_icp_align(const ob_voxel_map* m, const ob_icp_io* io, ob_stream* s)
  * Output rows are [x, y, z | the fields' channels widened to double, in table order], one per pixel with range > 0,
  * in row-major pixel order of the staggered image, item i's rows after item i-1's.  The XYZ is K1's projection and
  * pose arithmetic (bit for bit the ob_cloud_io poses result).  ONE kernel launch (decoupled look-back compaction,
- * as ob_dewarp_frames).  n_rows in host memory: one stream synchronisation, then "output capacity too small" when
- * more rows than `capacity` pass.  n_rows in DEVICE memory (rows in device memory too): nothing waits, and a count
- * above `capacity` means the list was cut there.  Fields are not tone-mapped (the exporter's float16 RGB step).
+ * as ob_dewarp_frames).  n_rows in host memory: the call waits for the count, then for host rows; "output capacity
+ * too small" when more rows than `capacity` pass (n_rows left 0, rows untouched).  n_rows in DEVICE memory (rows in
+ * device memory too): nothing waits, and a count above `capacity` means the list was cut there.  Fields are not tone-mapped (the exporter's float16 RGB step).
  * errors: "map rows need a float64 lut", "unknown field type", "field channels must be at least 1",
  * "cols must be 3 plus the channels of every item's fields", "too many fields" (more than 16 per item). */
 typedef struct ob_map_field {

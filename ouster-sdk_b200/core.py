@@ -531,8 +531,7 @@ def voxel_downsample(points, voxel_size, mode="shuffle_first", normals=None, max
         if tuple(nrm.shape) != (rows, 3) or cols != 3:
             raise ValueError("voxel_downsample_with_normals expects Nx3 inputs" if cols != 3 or nrm.shape[-1] != 3
                              else "voxel_downsample_with_normals points/normals size mismatch")
-    if n is not None and not (_is_torch(points) and points.is_cuda):
-        raise ValueError("a device-side row count needs device inputs")
+    n_dev = None if n is None else _device_rows(n, points)
     out_cols = 3 if m == _capi.OB_VOXEL_POINT_NORMAL else cols
     out = _empty(points, (rows, out_cols), np.float64)
     out_n = _empty(points, (rows, 3), np.float64) if nrm is not None else None
@@ -545,11 +544,8 @@ def voxel_downsample(points, voxel_size, mode="shuffle_first", normals=None, max
     io.points_out, io.normals_out, io.indices_out = _ptr(out), _ptr(out_n), _ptr(idx)
     head = (out, out_n, idx) if nrm is not None else (out, idx)
     if n is not None:
-        import torch
-        if not (_is_torch(n) and n.is_cuda and n.dtype == torch.int64 and n.numel() == 1):
-            raise ValueError("n must be a CUDA int64 tensor with one element")
-        count = torch.zeros(1, dtype=torch.int64, device=points.device)
-        io.n_device, io.capacity, io.n_out = n.data_ptr(), rows, count.data_ptr()
+        count = _device_count(points)
+        io.n_device, io.capacity, io.n_out = n_dev, rows, count.data_ptr()
         check(lib.ob_voxel_downsample(C.byref(io), _stream_for(points, stream, device).h))
         return head + (count,)
     cnt = C.c_size_t(0)
@@ -562,45 +558,42 @@ def voxel_downsample(points, voxel_size, mode="shuffle_first", normals=None, max
 DBL_MAX = float(np.finfo(np.float64).max)
 
 
-def _point_rows(points, n=None, what="add_points expects an Nx3 array"):
-    """(PointRows, kept array) for [rows, 3] float32 / float64 points (numpy or torch); n: optional CUDA int64 [1]
+def _device_rows(n, data):
+    """Address of a device-resident row count n (a CUDA int64 tensor of one element) for the rows in `data`, which
+    must then be a CUDA tensor too."""
+    import torch
+    if not (_is_torch(n) and n.is_cuda and n.dtype == torch.int64 and n.numel() == 1):
+        raise ValueError("n must be a CUDA int64 tensor with one element")
+    if not (_is_torch(data) and data.is_cuda):
+        raise ValueError("a device-side row count needs device inputs")
+    return n.data_ptr()
+
+
+def _device_count(like):
+    """A zeroed CUDA int64 [1] on `like`'s device: the count word of a call that returns a device-side count."""
+    import torch
+    return torch.zeros(1, dtype=torch.int64, device=like.device)
+
+
+def _point_rows(points, n=None, what="add_points expects an Nx3 array", cols=3):
+    """(row argument, kept array): an ob_point_rows (PointRows) for [rows, 3] float32 / float64 points, or with
+    cols=None an ob_map_rows (MapRows) for float64 [rows, any cols]; numpy or torch.  n: optional CUDA int64 [1]
     device-resident row count, then `points` holds `capacity` rows."""
-    from ._capi import PointRows
-    points = _contig(points, floats=True)
-    if len(points.shape) != 2 or points.shape[1] != 3:
+    from ._capi import MapRows, PointRows
+    points = _contig(points, floats=True) if cols else _contig(points, np.float64)
+    if len(points.shape) != 2 or (cols and points.shape[1] != cols):
         raise ValueError(what)
-    r = PointRows()
-    r.dtype = _capi.OB_F64 if _np_dtype(points) == np.float64 else _capi.OB_F32
-    r.points = _ptr(points)
+    if cols:
+        r = PointRows()
+        r.dtype = _capi.OB_F64 if _np_dtype(points) == np.float64 else _capi.OB_F32
+        r.points = _ptr(points)
+    else:
+        r = MapRows()
+        r.rows, r.cols = _ptr(points), int(points.shape[1])
     if n is None:
         r.n = int(points.shape[0])
     else:
-        import torch
-        if not (_is_torch(n) and n.is_cuda and n.dtype == torch.int64 and n.numel() == 1):
-            raise ValueError("n must be a CUDA int64 tensor with one element")
-        if not (_is_torch(points) and points.is_cuda):
-            raise ValueError("a device-side row count needs device inputs")
-        r.n_device, r.capacity = n.data_ptr(), int(points.shape[0])
-    return r, points
-
-
-def _map_rows_arg(points, n=None):
-    """(MapRows, kept float64 array) for [rows, cols] points (numpy or torch); n as for _point_rows."""
-    from ._capi import MapRows
-    points = _contig(points, np.float64)
-    if len(points.shape) != 2:
-        raise ValueError("add_points expects at least Nx(3+num_attributes) columns")
-    r = MapRows()
-    r.rows, r.cols = _ptr(points), int(points.shape[1])
-    if n is None:
-        r.n = int(points.shape[0])
-    else:
-        import torch
-        if not (_is_torch(n) and n.is_cuda and n.dtype == torch.int64 and n.numel() == 1):
-            raise ValueError("n must be a CUDA int64 tensor with one element")
-        if not (_is_torch(points) and points.is_cuda):
-            raise ValueError("a device-side row count needs device inputs")
-        r.n_device, r.capacity = n.data_ptr(), int(points.shape[0])
+        r.n_device, r.capacity = _device_rows(n, points), int(points.shape[0])
     return r, points
 
 
@@ -652,7 +645,7 @@ class VoxelMap(_Handle):
     def add_rows(self, rows, n=None, stream=None):
         """VoxelHashMap::add_points(ArrayXXdR): float64 [rows, cols]; raises ValueError("VoxelHashMap::add_points
         received unexpected point dimension") for another width."""
-        r, keep = _map_rows_arg(rows, n)
+        r, keep = _point_rows(rows, n, "add_points expects at least Nx(3+num_attributes) columns", cols=None)
         check(lib.ob_voxel_map_add_rows(self._h, C.byref(r), _stream_for(keep, stream, self.device).h))
 
     def remove_far(self, origin, extract=False, stream=None):
@@ -804,8 +797,7 @@ def map_rows(items, capacity=None, device_count=None, stream=None):
     out = _empty(ref, (cap, cols), np.float64)
     st = _stream_for(ref, stream, getattr(live[0]["lut"], "_lut", live[0]["lut"]).device)
     if device_count:
-        import torch
-        n = torch.zeros(1, dtype=torch.int64, device=ref.device)
+        n = _device_count(ref)
         check(lib.ob_frames_to_map_rows(ios, len(live), _ptr(out), cols, cap, n.data_ptr(), st.h))
         return out, n
     cnt = C.c_size_t(0)

@@ -814,8 +814,8 @@ ob_status ob_cloud_align(const ob_cloud_align_io* io, ob_stream* s) {
     // the reference's checks in its order (align_clouds.cpp:1593-1595, 1731-1747)
     if (!std::isfinite(io->max_corr_dist) || io->max_corr_dist <= 0.0)
         return fail(OB_INVALID_ARGUMENT, "max_corr_dist must be finite and greater than zero");
-    const size_t src_rows = io->source.n_device ? io->source.capacity : io->source.n;
-    const size_t tgt_rows = io->target.n_device ? io->target.capacity : io->target.n;
+    const size_t src_rows = row_capacity(io->source.n, io->source.n_device, io->source.capacity);
+    const size_t tgt_rows = row_capacity(io->target.n, io->target.n_device, io->target.capacity);
     if (plane) {
         if (!std::isfinite(io->max_normal_angle_deg) || io->max_normal_angle_deg < 0.0 || io->max_normal_angle_deg > 180.0)
             return fail(OB_INVALID_ARGUMENT, "max_normal_angle_deg must be finite and in [0, 180]");
@@ -844,21 +844,17 @@ ob_status ob_cloud_align(const ob_cloud_align_io* io, ob_stream* s) {
         if (e == cudaSuccess) e = stg.in(io->target_normals, tr.cap * 3 * esz, &tnrm);
     }
     if (e == cudaSuccess && io->initial_guess) e = stg.in(io->initial_guess, 16 * 8, &guess);
-    const bool dev_pose = is_device_ptr(io->pose);
-    const bool dev_it = io->iterations == nullptr || is_device_ptr(io->iterations);
-    double* pose = io->pose;
-    int32_t* iters = io->iterations;
-    if (e == cudaSuccess && !dev_pose) e = scratch(stg, 16 * 8, &pose);
-    if (e == cudaSuccess && !dev_it) e = scratch(stg, 4, &iters);
+    void *pose = nullptr, *iters = nullptr;
+    if (e == cudaSuccess) e = stg.out(io->pose, 16 * 8, &pose);
+    if (e == cudaSuccess) e = stg.out(io->iterations, 4, &iters);
     if (e != cudaSuccess) return fail_cuda(e, "stage cloud align");
-    rs = io->source.dtype == OB_F64
-             ? run_align<double>(io, sr, tr, snrm, tnrm, static_cast<const double*>(guess), stg, st, pose, iters)
-             : run_align<float>(io, sr, tr, snrm, tnrm, static_cast<const double*>(guess), stg, st, pose, iters);
+    const double* g = static_cast<const double*>(guess);
+    double* p = static_cast<double*>(pose);
+    int32_t* it = static_cast<int32_t*>(iters);
+    rs = io->source.dtype == OB_F64 ? run_align<double>(io, sr, tr, snrm, tnrm, g, stg, st, p, it)
+                                    : run_align<float>(io, sr, tr, snrm, tnrm, g, stg, st, p, it);
     if (rs != OB_OK) return rs;
-    if (dev_pose && dev_it) return OB_OK;  // nothing waits for the GPU
-    if (!dev_pose) e = cudaMemcpyAsync(io->pose, pose, 16 * 8, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess && !dev_it) e = cudaMemcpyAsync(io->iterations, iters, 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    e = stg.finish();  // host pose / iterations: one wait; device ones: nothing waits for the GPU
     if (e != cudaSuccess) return fail_cuda(e, "cloud align result");
     return OB_OK;
 }
@@ -898,8 +894,7 @@ ob_status ob_cloud_nearest(const ob_cloud_nearest_io* io, ob_stream* s) {
     count_launch(launches);
     count_launch_of(OB_FAM_ALIGN, launches);
     if (e == cudaSuccess) e = cudaGetLastError();
-    if (e == cudaSuccess) e = stg.flush();
-    if (e == cudaSuccess && !is_device_ptr(io->indices)) e = cudaStreamSynchronize(st);
+    if (e == cudaSuccess) e = stg.finish();
     if (e != cudaSuccess) return fail_cuda(e, "cloud nearest");
     return OB_OK;
 }

@@ -213,6 +213,83 @@ cudaError_t Staging::flush() {
     return cudaSuccess;
 }
 
+cudaError_t Staging::finish() {
+    const bool wait = !pending_.empty();
+    cudaError_t e = flush();
+    if (e == cudaSuccess && wait) e = cudaStreamSynchronize(st_);
+    return e;
+}
+
+CountedRows::CountedRows(size_t* n, size_t capacity, Staging& stg, cudaStream_t st, const char* what)
+    : n_(n), cap_(capacity), stg_(stg), st_(st), what_(what), dev_(is_device_ptr(n)) {
+    if (n && !dev_) *n = 0;
+}
+
+ob_status CountedRows::zero() {
+    if (!dev_ || zeroed_) return OB_OK;
+    cudaError_t e = cudaMemsetAsync(n_, 0, sizeof(size_t), st_);
+    if (e != cudaSuccess) return fail_cuda(e, what_);
+    zeroed_ = true;
+    return OB_OK;
+}
+
+ob_status CountedRows::refuse(std::initializer_list<const void*> arrays, const char* msg) {
+    if (!dev_) return OB_OK;
+    for (const void* p : arrays)
+        if (p && !is_device_ptr(p)) {
+            ob_status rs = zero();
+            return rs != OB_OK ? rs : fail(OB_INVALID_ARGUMENT, msg);
+        }
+    return OB_OK;
+}
+
+cudaError_t CountedRows::array(void* p, size_t row_bytes, void** dev) {
+    *dev = p;
+    if (!p || is_device_ptr(p)) return cudaSuccess;
+    cudaError_t e = stg_.scratch(cap_ * row_bytes, dev);
+    if (e == cudaSuccess) host_.push_back({p, *dev, row_bytes});
+    return e;
+}
+
+cudaError_t CountedRows::word(unsigned long long** w) {
+    *w = reinterpret_cast<unsigned long long*>(n_);
+    if (dev_) return cudaSuccess;
+    void* d = nullptr;
+    cudaError_t e = stg_.scratch(8, &d);
+    *w = static_cast<unsigned long long*>(d);
+    return e;
+}
+
+ob_status CountedRows::finish(const unsigned long long* end) {
+    if (dev_) {
+        if (end == reinterpret_cast<const unsigned long long*>(n_)) return OB_OK;  // the kernel wrote it in place
+        cudaError_t e = cudaMemcpyAsync(n_, end, 8, cudaMemcpyDeviceToDevice, st_);
+        return e == cudaSuccess ? OB_OK : fail_cuda(e, what_);
+    }
+    unsigned long long total = 0;
+    ob_status rs = read(end, 1, &total);
+    return rs != OB_OK ? rs : deliver(total);
+}
+
+ob_status CountedRows::read(const unsigned long long* ends, size_t k, unsigned long long* host) {
+    cudaError_t e = cudaMemcpyAsync(host, ends, k * 8, cudaMemcpyDeviceToHost, st_);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st_);
+    return e == cudaSuccess ? OB_OK : fail_cuda(e, what_);
+}
+
+ob_status CountedRows::deliver(unsigned long long total) {
+    if (total > cap_) return fail(OB_INVALID_ARGUMENT, "output capacity too small");
+    cudaError_t e = cudaSuccess;
+    if (total && !host_.empty()) {
+        for (const HostArray& a : host_)
+            if (e == cudaSuccess) e = cudaMemcpyAsync(a.host, a.dev, total * a.row_bytes, cudaMemcpyDeviceToHost, st_);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st_);
+    }
+    if (e != cudaSuccess) return fail_cuda(e, what_);
+    *n_ = static_cast<size_t>(total);
+    return OB_OK;
+}
+
 ob_status require_device(int device) {
     int n = 0;
     cudaError_t e = cudaGetDeviceCount(&n);
@@ -787,11 +864,10 @@ ob_status ob_dewarp(ob_dtype dtype, const void* points, const void* poses, size_
 }
 
 // Shared driver of ob_dewarp_frame / ob_dewarp_frames: frame table upload, ONE kernel launch, then the
-// device-side counts.  Results for device outputs are complete in stream order; the only host wait is the
-// one a host-memory result needs anyway.
+// count (the per-frame ends of the look-back scan) through `res`.
 static ob_status run_dewarp(std::vector<K3Frame>& hf, int dtype, uint32_t min_r, uint32_t max_r, void* points,
                             size_t capacity, uint32_t* frame_idx, uint32_t* col_idx, uint64_t* timestamps_out,
-                            size_t* counts, size_t* n_points, Staging& stg, ob_stream* s) {
+                            size_t* counts, CountedRows& res, Staging& stg, ob_stream* s) {
     unsigned n_blocks = 0, max_slabs = 0;
     for (K3Frame& f : hf) {
         f.first_block = n_blocks;
@@ -799,64 +875,30 @@ static ob_status run_dewarp(std::vector<K3Frame>& hf, int dtype, uint32_t min_r,
         max_slabs = std::max(max_slabs, f.n_slabs);
     }
     const size_t esz = dtype_size(dtype);
-    void *fdev = nullptr, *scan = nullptr, *o = nullptr;
+    void *fdev = nullptr, *scan = nullptr;
     cudaError_t e = stg.scratch(hf.size() * sizeof(K3Frame), &fdev);
     if (e == cudaSuccess) e = stg.scratch(dewarp_scan_scratch_bytes(n_blocks, static_cast<unsigned>(hf.size())), &scan);
     if (e == cudaSuccess) e = cudaMemcpyAsync(fdev, hf.data(), hf.size() * sizeof(K3Frame), cudaMemcpyHostToDevice, s->st);
     if (e != cudaSuccess) return fail_cuda(e, "frame table upload");
-    // outputs: device pointers in place, host pointers through device scratch of `capacity` points
-    const bool host_out = !is_device_ptr(points);
-    void* dpts = points;
-    uint32_t *dfi = frame_idx, *dci = col_idx;
-    uint64_t* dts = timestamps_out;
-    if (host_out) {
-        e = stg.scratch(std::max<size_t>(1, capacity) * 3 * esz, &o);
-        dpts = o;
-        if (e == cudaSuccess && frame_idx) {
-            e = stg.scratch(std::max<size_t>(1, capacity) * 4, &o);
-            dfi = static_cast<uint32_t*>(o);
-        }
-        if (e == cudaSuccess && col_idx) {
-            e = stg.scratch(std::max<size_t>(1, capacity) * 4, &o);
-            dci = static_cast<uint32_t*>(o);
-        }
-        if (e == cudaSuccess && timestamps_out) {
-            e = stg.scratch(std::max<size_t>(1, capacity) * 8, &o);
-            dts = static_cast<uint64_t*>(o);
-        }
-        if (e != cudaSuccess) return fail_cuda(e, "stage dewarp outputs");
-    }
+    void* dpts = nullptr;
+    uint32_t *dfi = nullptr, *dci = nullptr;
+    uint64_t* dts = nullptr;
+    e = res.array(points, 3 * esz, &dpts);
+    if (e == cudaSuccess) e = res.array(frame_idx, 4, &dfi);
+    if (e == cudaSuccess) e = res.array(col_idx, 4, &dci);
+    if (e == cudaSuccess) e = res.array(timestamps_out, 8, &dts);
+    if (e != cudaSuccess) return fail_cuda(e, "stage dewarp outputs");
     const unsigned long long* fend = nullptr;
     e = launch_dewarp_fused(static_cast<const K3Frame*>(fdev), static_cast<unsigned>(hf.size()), n_blocks, max_slabs,
                             min_r, max_r, dtype, scan, dpts, dfi, dci, dts, capacity, &fend, s->st);
     if (e != cudaSuccess) return fail_cuda(e, "dewarp launch");
-    if (is_device_ptr(n_points)) {
-        // fully asynchronous form: the count stays on the device next to the points (a count above
-        // `capacity` means the list was cut at `capacity` points; no error can be raised from here)
-        if (host_out || counts) return fail(OB_INVALID_ARGUMENT, "a device-side count needs device outputs and no per-frame counts");
-        e = cudaMemcpyAsync(n_points, fend + (hf.size() - 1), 8, cudaMemcpyDeviceToDevice, s->st);
-        if (e != cudaSuccess) return fail_cuda(e, "dewarp count");
-        return OB_OK;
-    }
+    if (res.on_device()) return res.finish(fend + (hf.size() - 1));
     std::vector<unsigned long long> ends(hf.size());
-    e = cudaMemcpyAsync(ends.data(), fend, hf.size() * 8, cudaMemcpyDeviceToHost, s->st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(s->st);
-    if (e != cudaSuccess) return fail_cuda(e, "dewarp count");
-    const unsigned long long total = ends.back();
+    ob_status rs = res.read(fend, hf.size(), ends.data());
+    if (rs != OB_OK) return rs;
     if (counts)
         for (size_t k = 0; k < hf.size(); ++k) counts[hf[k].index] = static_cast<size_t>(ends[k] - (k ? ends[k - 1] : 0ull));
-    if (total > capacity) return fail(OB_INVALID_ARGUMENT, "output capacity too small");
-    if (host_out && total) {
-        e = cudaMemcpyAsync(points, dpts, total * 3 * esz, cudaMemcpyDeviceToHost, s->st);
-        if (e == cudaSuccess && frame_idx) e = cudaMemcpyAsync(frame_idx, dfi, total * 4, cudaMemcpyDeviceToHost, s->st);
-        if (e == cudaSuccess && col_idx) e = cudaMemcpyAsync(col_idx, dci, total * 4, cudaMemcpyDeviceToHost, s->st);
-        if (e == cudaSuccess && timestamps_out)
-            e = cudaMemcpyAsync(timestamps_out, dts, total * 8, cudaMemcpyDeviceToHost, s->st);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(s->st);
-        if (e != cudaSuccess) return fail_cuda(e, "dewarp D2H");
-    }
-    *n_points = static_cast<size_t>(total);
-    return OB_OK;
+    return res.deliver(ends.back());
 }
 
 static ob_status stage_k3_frame(const ob_lut* lut, const uint32_t* range, const double* poses, const uint32_t* status,
@@ -895,20 +937,15 @@ static bool range_window(double min_range, double max_range, uint32_t* min_r, ui
     return true;
 }
 
-static ob_status zero_count(size_t* n_points, ob_stream* s) {
-    if (is_device_ptr(n_points)) {
-        cudaError_t e = cudaMemsetAsync(n_points, 0, 8, s->st);
-        return e == cudaSuccess ? OB_OK : fail_cuda(e, "dewarp count");
-    }
-    *n_points = 0;
-    return OB_OK;
-}
+static const char* const kDewarpMixed = "a device-side count needs device outputs and no per-frame counts";
 
 ob_status ob_dewarp_frame(const ob_lut* lut, const ob_dewarp_frame_io* io, size_t* n_points, ob_stream* s) {
     if (!lut || !io || !n_points || !s) return fail(OB_INVALID_ARGUMENT, "null pointer");
     ob_status rs = require_device(s->device);
     if (rs != OB_OK) return rs;
-    rs = zero_count(n_points, s);
+    Staging stg(s->st);
+    CountedRows res(n_points, io->capacity, stg, s->st, "dewarp count");
+    rs = res.zero();
     if (rs != OB_OK) return rs;
     if (!io->range || !io->poses || !io->status || !io->points)
         return fail(OB_INVALID_ARGUMENT, "null range / poses / status / points");
@@ -918,12 +955,13 @@ ob_status ob_dewarp_frame(const ob_lut* lut, const ob_dewarp_frame_io* io, size_
     uint32_t min_r, max_r;
     if (!range_window(io->min_range, io->max_range, &min_r, &max_r)) return OB_OK;
     if (lut->h == 0 || lut->w == 0) return OB_OK;
-    Staging stg(s->st);
+    rs = res.refuse({io->points, io->col_idx, io->timestamps_out}, kDewarpMixed);
+    if (rs != OB_OK) return rs;
     std::vector<K3Frame> hf(1);
     rs = stage_k3_frame(lut, io->range, io->poses, io->status, io->timestamps, io->timestamps_out != nullptr, 0, stg, &hf[0]);
     if (rs != OB_OK) return rs;
     return run_dewarp(hf, lut->dtype, min_r, max_r, io->points, io->capacity, nullptr, io->col_idx, io->timestamps_out,
-                      nullptr, n_points, stg, s);
+                      nullptr, res, stg, s);
 }
 
 ob_status ob_dewarp_frames(const ob_dewarp_frames_io* frames, size_t n_frames, double min_range, double max_range,
@@ -932,7 +970,9 @@ ob_status ob_dewarp_frames(const ob_dewarp_frames_io* frames, size_t n_frames, d
     if (!s || !n_points || (n_frames && !frames)) return fail(OB_INVALID_ARGUMENT, "null pointer");
     ob_status rs = require_device(s->device);
     if (rs != OB_OK) return rs;
-    rs = zero_count(n_points, s);
+    Staging stg(s->st);
+    CountedRows res(n_points, capacity, stg, s->st, "dewarp count");
+    rs = res.zero();
     if (rs != OB_OK) return rs;
     if (counts) std::fill(counts, counts + n_frames, static_cast<size_t>(0));
     if (n_frames == 0) return OB_OK;
@@ -940,9 +980,7 @@ ob_status ob_dewarp_frames(const ob_dewarp_frames_io* frames, size_t n_frames, d
     uint32_t min_r, max_r;
     if (!range_window(min_range, max_range, &min_r, &max_r)) return OB_OK;
     int dtype = -1;
-    Staging stg(s->st);
-    std::vector<K3Frame> hf;
-    hf.reserve(n_frames);
+    std::vector<size_t> live;  // frames with pixels, checked before any is staged
     for (size_t i = 0; i < n_frames; ++i) {
         const ob_dewarp_frames_io& io = frames[i];
         if (!io.lut) continue;  // FrameSet::valid_indices(): empty slots of the set are skipped
@@ -953,16 +991,20 @@ ob_status ob_dewarp_frames(const ob_dewarp_frames_io* frames, size_t n_frames, d
         if (lut->device != s->device) return fail(OB_INVALID_ARGUMENT, "lut and stream are on different devices");
         if (dtype < 0) dtype = lut->dtype;
         if (lut->dtype != dtype) return fail(OB_INVALID_ARGUMENT, "the luts of a set must share one dtype");
-        if (lut->h == 0 || lut->w == 0) continue;
-        K3Frame f;
-        rs = stage_k3_frame(lut, io.range, io.poses, io.status, io.timestamps, timestamps_out != nullptr,
-                            static_cast<unsigned>(i), stg, &f);
-        if (rs != OB_OK) return rs;
-        hf.push_back(f);
+        if (lut->h != 0 && lut->w != 0) live.push_back(i);
     }
-    if (hf.empty()) return OB_OK;
-    return run_dewarp(hf, dtype, min_r, max_r, points, capacity, frame_idx, col_idx, timestamps_out, counts, n_points,
-                      stg, s);
+    if (live.empty()) return OB_OK;
+    rs = res.refuse({points, frame_idx, col_idx, timestamps_out, counts}, kDewarpMixed);
+    if (rs != OB_OK) return rs;
+    std::vector<K3Frame> hf(live.size());
+    for (size_t k = 0; k < live.size(); ++k) {
+        const ob_dewarp_frames_io& io = frames[live[k]];
+        rs = stage_k3_frame(io.lut, io.range, io.poses, io.status, io.timestamps, timestamps_out != nullptr,
+                            static_cast<unsigned>(live[k]), stg, &hf[k]);
+        if (rs != OB_OK) return rs;
+    }
+    return run_dewarp(hf, dtype, min_r, max_r, points, capacity, frame_idx, col_idx, timestamps_out, counts, res, stg,
+                      s);
 }
 
 ob_status ob_destagger(size_t elem_size, size_t k, const void* img, const int32_t* shifts,

@@ -1,5 +1,6 @@
 // ob_api_common.h -- helpers shared by the C-ABI translation units.
 #pragma once
+#include <initializer_list>
 #include <string>
 #include <vector>
 
@@ -27,6 +28,9 @@ class Staging {
     cudaError_t inout(void* p, size_t bytes, void** dev);
     cudaError_t scratch(size_t bytes, void** dev);
     cudaError_t flush();
+    // flush(), then wait for the stream if that issued a D2H: host results are final on return, and a call whose
+    // outputs are all device memory waits for nothing (and stays capturable in a CUDA graph)
+    cudaError_t finish();
 
    private:
     struct Pending {
@@ -37,6 +41,54 @@ class Staging {
     cudaStream_t st_;
     std::vector<void*> scratch_;
     std::vector<Pending> pending_;
+};
+
+// A result whose length the GPU decides: rows in one or more arrays plus their count, each in host or device memory.
+//  - The count reads 0 until the call succeeds: a host count is zeroed here, a device count by zero() (or by the
+//    kernel that writes it).
+//  - A device count needs every array in device memory; refuse() turns a host array away (count 0) before anything
+//    is staged or launched.
+//  - array(): a device array is written in place, a host array through scratch of `capacity` rows, a null array is
+//    not written (count only).
+//  - finish(): with a device count nothing waits, rows past `capacity` are cut and the count is the true total.  With
+//    a host count the call waits for the count; more rows than `capacity` fail "output capacity too small" with the
+//    count left 0 and the host rows untouched; otherwise it waits again for the rows of the host arrays.
+class CountedRows {
+   public:
+    static constexpr size_t kCountOnly = ~static_cast<size_t>(0);  // capacity of a call that writes no rows
+    CountedRows(size_t* n, size_t capacity, Staging& stg, cudaStream_t st, const char* what);
+    bool on_device() const { return dev_; }
+    ob_status zero();
+    ob_status refuse(std::initializer_list<const void*> arrays, const char* msg);
+    cudaError_t array(void* p, size_t row_bytes, void** dev);
+    template <typename T>
+    cudaError_t array(T* p, size_t row_bytes, T** dev) {
+        void* d = nullptr;
+        cudaError_t e = array(static_cast<void*>(p), row_bytes, &d);
+        *dev = static_cast<T*>(d);
+        return e;
+    }
+    // the device word the kernel writes the count to: the caller's device count, or scratch
+    cudaError_t word(unsigned long long** w);
+    // after the launch; `end`: the device word holding the count
+    ob_status finish(const unsigned long long* end);
+    // finish() in two steps for a host count: read k device words (the last is the count) with one wait, then deliver
+    ob_status read(const unsigned long long* ends, size_t k, unsigned long long* host);
+    ob_status deliver(unsigned long long total);
+
+   private:
+    struct HostArray {
+        void* host;
+        void* dev;
+        size_t row_bytes;
+    };
+    size_t* n_;
+    size_t cap_;
+    Staging& stg_;
+    cudaStream_t st_;
+    const char* what_;
+    bool dev_, zeroed_ = false;
+    std::vector<HostArray> host_;
 };
 
 // accessors for the opaque handles (defined in ob_api.cu)

@@ -130,15 +130,6 @@ __global__ void __launch_bounds__(kMrThreads) map_rows_kernel(const MrItem* __re
 // scratch: [ticket + pad : 16 B][state u32 x nb, padded to 8][agg u64 x nb][incl u64 x nb][item_end u64 x ni]
 size_t state_bytes(unsigned nb) { return 16 + ((static_cast<size_t>(nb) * 4 + 7) & ~static_cast<size_t>(7)); }
 
-ob_status zero_rows(size_t* n_rows, cudaStream_t st) {
-    if (is_device_ptr(n_rows)) {
-        cudaError_t e = cudaMemsetAsync(n_rows, 0, 8, st);
-        return e == cudaSuccess ? OB_OK : fail_cuda(e, "map rows count");
-    }
-    *n_rows = 0;
-    return OB_OK;
-}
-
 }  // namespace
 }  // namespace ob
 
@@ -151,11 +142,11 @@ extern "C" ob_status ob_frames_to_map_rows(const ob_map_rows_item* items, size_t
     ob_status rs = require_device(device);
     if (rs != OB_OK) return rs;
     const cudaStream_t st = stream_handle(s);
-    rs = zero_rows(n_rows, st);
+    Staging stg(st);
+    CountedRows res(n_rows, capacity, stg, st, "map rows count");
+    rs = res.zero();
+    if (rs == OB_OK) rs = res.refuse({rows}, "a device-side count needs device outputs");
     if (rs != OB_OK) return rs;
-    const bool dev_count = is_device_ptr(n_rows);
-    const bool host_out = rows && !is_device_ptr(rows);
-    if (dev_count && host_out) return fail(OB_INVALID_ARGUMENT, "a device-side count needs device outputs");
     // every check before anything is staged
     for (size_t i = 0; i < n_items; ++i) {
         const ob_map_rows_item& io = items[i];
@@ -176,7 +167,6 @@ extern "C" ob_status ob_frames_to_map_rows(const ob_map_rows_item* items, size_t
         if (c != cols) return fail(OB_INVALID_ARGUMENT, "cols must be 3 plus the channels of every item's fields");
     }
     if (capacity && !rows) return fail(OB_INVALID_ARGUMENT, "null rows buffer");
-    Staging stg(st);
     std::vector<MrItem> hi;
     unsigned nb = 0;
     for (size_t i = 0; i < n_items; ++i) {
@@ -213,12 +203,8 @@ extern "C" ob_status ob_frames_to_map_rows(const ob_map_rows_item* items, size_t
     if (e == cudaSuccess) e = stg.scratch(state_bytes(nb) + static_cast<size_t>(nb) * 16 + ni * 8ull, &scan);
     if (e == cudaSuccess) e = cudaMemcpyAsync(tab, hi.data(), hi.size() * sizeof(MrItem), cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(scan, 0, state_bytes(nb), st);  // ticket + state words
-    double* dout = rows;
-    if (e == cudaSuccess && host_out && capacity) {
-        void* o = nullptr;
-        e = stg.scratch(capacity * cols * 8, &o);
-        dout = static_cast<double*>(o);
-    }
+    double* dout = nullptr;
+    if (e == cudaSuccess) e = res.array(rows, cols * 8, &dout);
     if (e != cudaSuccess) return fail_cuda(e, "stage map rows");
     uint8_t* b = static_cast<uint8_t*>(scan);
     Lookback lb;
@@ -232,20 +218,5 @@ extern "C" ob_status ob_frames_to_map_rows(const ob_map_rows_item* items, size_t
     count_launch_of(OB_FAM_VOXEL_MAP);
     e = cudaGetLastError();
     if (e != cudaSuccess) return fail_cuda(e, "map rows launch");
-    if (dev_count) {
-        e = cudaMemcpyAsync(n_rows, item_end + (ni - 1), 8, cudaMemcpyDeviceToDevice, st);
-        return e == cudaSuccess ? OB_OK : fail_cuda(e, "map rows count");
-    }
-    unsigned long long total = 0;
-    e = cudaMemcpyAsync(&total, item_end + (ni - 1), 8, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) return fail_cuda(e, "map rows count");
-    if (total > capacity) return fail(OB_INVALID_ARGUMENT, "output capacity too small");
-    if (host_out && total) {
-        e = cudaMemcpyAsync(rows, dout, total * cols * 8, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        if (e != cudaSuccess) return fail_cuda(e, "map rows D2H");
-    }
-    *n_rows = static_cast<size_t>(total);
-    return OB_OK;
+    return res.finish(item_end + (ni - 1));
 }

@@ -32,21 +32,32 @@ __device__ __forceinline__ void load3(const void* base, size_t row, double* v) {
 // ---- host side ----
 bool dtype_ok(int32_t d) { return d == OB_F32 || d == OB_F64; }
 
-// validate an ob_point_rows and stage it: host rows go through scratch; the row capacity is returned
+// rows an input's buffers hold: n, or `capacity` with a device-resident count
+size_t row_capacity(size_t n, const void* n_device, size_t capacity) { return n_device ? capacity : n; }
+
+// the count fields of Rows for an input row count (n, or the device word n_device clamped to `capacity`):
+// at most 2^31-1 rows per call (else `too_many`), and n_device must be device memory
+ob_status count_rows(size_t n, const void* n_device, size_t capacity, Rows* r,
+                     const char* too_many = "too many points in one call") {
+    const size_t cap = row_capacity(n, n_device, capacity);
+    if (cap > 0x7fffffffu) return fail(OB_INVALID_ARGUMENT, too_many);
+    if (n_device && !is_device_ptr(n_device)) return fail(OB_INVALID_ARGUMENT, "n_device must be device memory");
+    r->n_dev = static_cast<const unsigned long long*>(n_device);
+    r->n_host = n;
+    r->cap = static_cast<unsigned>(cap);
+    return OB_OK;
+}
+
+// validate an ob_point_rows and stage it: host rows go through scratch
 ob_status stage_rows(const ob_point_rows* in, Staging& stg, Rows* r, const char* what) {
     if (!dtype_ok(in->dtype)) return fail(OB_INVALID_ARGUMENT, "unknown dtype");
-    const bool dev_n = in->n_device != nullptr;
-    const size_t cap = dev_n ? in->capacity : in->n;
-    if (cap > 0x7fffffffu) return fail(OB_INVALID_ARGUMENT, "too many points in one call");
-    if (dev_n && !is_device_ptr(in->n_device)) return fail(OB_INVALID_ARGUMENT, "n_device must be device memory");
-    if (cap && !in->points) return fail(OB_INVALID_ARGUMENT, "null points buffer");
+    ob_status rs = count_rows(in->n, in->n_device, in->capacity, r);
+    if (rs != OB_OK) return rs;
+    if (r->cap && !in->points) return fail(OB_INVALID_ARGUMENT, "null points buffer");
     const void* d = nullptr;
-    cudaError_t e = stg.in(in->points, cap * 3 * (in->dtype == OB_F64 ? 8 : 4), &d);
+    cudaError_t e = stg.in(in->points, r->cap * 3ull * (in->dtype == OB_F64 ? 8 : 4), &d);
     if (e != cudaSuccess) return fail_cuda(e, what);
     r->p = d;
-    r->n_dev = reinterpret_cast<const unsigned long long*>(in->n_device);
-    r->n_host = in->n;
-    r->cap = static_cast<unsigned>(cap);
     return OB_OK;
 }
 

@@ -29,6 +29,7 @@
 #include <type_traits>
 
 #include "ob_api_common.h"
+#include "ob_rows.cuh"
 #include "ob_voxel_common.cuh"
 
 namespace ob {
@@ -546,15 +547,6 @@ cudaError_t run_voxel(VoxelParams p, Staging& stg, cudaStream_t st, double* out,
     return cudaGetLastError();
 }
 
-ob_status zero_voxel_count(size_t* n_out, cudaStream_t st) {
-    if (is_device_ptr(n_out)) {
-        cudaError_t e = cudaMemsetAsync(n_out, 0, sizeof(size_t), st);
-        return e == cudaSuccess ? OB_OK : fail_cuda(e, "voxel count");
-    }
-    *n_out = 0;
-    return OB_OK;
-}
-
 }  // namespace
 
 extern "C" ob_status ob_voxel_downsample(const ob_voxel_io* io, ob_stream* s) {
@@ -567,8 +559,7 @@ extern "C" ob_status ob_voxel_downsample(const ob_voxel_io* io, ob_stream* s) {
         if (io->cols != 3) return fail(OB_INVALID_ARGUMENT, "voxel_downsample_with_normals expects Nx3 inputs");
         if (!(io->voxel_size > 0.0)) return fail(OB_INVALID_ARGUMENT, "voxel_downsample_with_normals voxel_size must be > 0");
     }
-    const bool dev_n = io->n_device != nullptr;
-    const size_t cap = dev_n ? io->capacity : io->n;
+    const size_t cap = row_capacity(io->n, io->n_device, io->capacity);
     if (cap != 0) {  // an empty frame returns before any other check
         if (mode == OB_VOXEL_SHUFFLE_FIRST && io->cols != 3) return fail(OB_INVALID_ARGUMENT, "voxel_downsample: points must be Nx3");
         if (mode != OB_VOXEL_POINT_NORMAL && io->cols < 3)
@@ -582,16 +573,20 @@ extern "C" ob_status ob_voxel_downsample(const ob_voxel_io* io, ob_stream* s) {
     ob_status rs = require_device(device);
     if (rs != OB_OK) return rs;
     cudaStream_t st = stream_handle(s);
-    rs = zero_voxel_count(io->n_out, st);
+    Staging stg(st);
+    CountedRows res(io->n_out, cap, stg, st, "voxel count");  // outputs hold `cap` rows: never too small
+    rs = res.zero();
+    if (rs != OB_OK || cap == 0) return rs;
+    if (io->cols > 0xffffu) return fail(OB_INVALID_ARGUMENT, "too many points in one call");
+    Rows r{};
+    rs = count_rows(io->n, io->n_device, io->capacity, &r);
     if (rs != OB_OK) return rs;
-    if (cap == 0) return OB_OK;
-    if (cap > 0x7fffffffu || io->cols > 0xffffu) return fail(OB_INVALID_ARGUMENT, "too many points in one call");
     if (!io->points || !io->points_out) return fail(OB_INVALID_ARGUMENT, "null points buffer");
     if (mode == OB_VOXEL_POINT_NORMAL && !io->normals) return fail(OB_INVALID_ARGUMENT, "null normals buffer");
-    if (dev_n && !is_device_ptr(io->n_device)) return fail(OB_INVALID_ARGUMENT, "n_device must be device memory");
+    rs = res.refuse({io->points_out, io->normals_out, io->indices_out}, "a device-side count needs device outputs");
+    if (rs != OB_OK) return rs;
     const size_t esz = io->dtype == OB_F64 ? 8 : 4;
     const size_t cols = io->cols, out_cols = mode == OB_VOXEL_POINT_NORMAL ? 3 : cols;
-    Staging stg(st);
     VoxelParams p{};
     const void* d = nullptr;
     cudaError_t e = stg.in(io->points, cap * cols * esz, &d);
@@ -601,9 +596,9 @@ extern "C" ob_status ob_voxel_downsample(const ob_voxel_io* io, ob_stream* s) {
         p.normals = d;
     }
     if (e != cudaSuccess) return fail_cuda(e, "stage voxel inputs");
-    p.n_dev = reinterpret_cast<const unsigned long long*>(io->n_device);
-    p.n_host = io->n;
-    p.cap = static_cast<unsigned>(cap);
+    p.n_dev = r.n_dev;
+    p.n_host = r.n_host;
+    p.cap = r.cap;
     p.cols = static_cast<unsigned>(cols);
     p.mode = mode;
     p.inv = 1.0 / io->voxel_size;  // VoxelHashMap::inv_voxel_size_, voxel_hash_map.cpp:40 / :290
@@ -619,51 +614,16 @@ extern "C" ob_status ob_voxel_downsample(const ob_voxel_io* io, ob_stream* s) {
         p.min_pts = io->min_pts_threshold;
         p.res_sq = io->voxel_size * io->voxel_size / static_cast<double>(io->max_points_per_voxel);  // :39
     }
-    // outputs: device pointers in place, host pointers through scratch of `cap` rows
-    const bool host_out = !is_device_ptr(io->points_out);
-    const bool dev_count = is_device_ptr(io->n_out);
-    if (dev_count && (host_out || (io->normals_out && !is_device_ptr(io->normals_out)) ||
-                      (io->indices_out && !is_device_ptr(io->indices_out))))
-        return fail(OB_INVALID_ARGUMENT, "a device-side count needs device outputs");
-    double* dpts = io->points_out;
-    double* dnrm = mode == OB_VOXEL_POINT_NORMAL ? io->normals_out : nullptr;
-    uint32_t* didx = io->indices_out;
-    void* o = nullptr;
-    if (host_out) {
-        e = stg.scratch(cap * out_cols * 8, &o);
-        dpts = static_cast<double*>(o);
-    }
-    if (e == cudaSuccess && dnrm && !is_device_ptr(dnrm)) {
-        e = stg.scratch(cap * 3 * 8, &o);
-        dnrm = static_cast<double*>(o);
-    }
-    if (e == cudaSuccess && didx && !is_device_ptr(didx)) {
-        e = stg.scratch(cap * 4, &o);
-        didx = static_cast<uint32_t*>(o);
-    }
-    unsigned long long* dcount = reinterpret_cast<unsigned long long*>(io->n_out);
-    if (e == cudaSuccess && !dev_count) {
-        e = stg.scratch(8, &o);
-        dcount = static_cast<unsigned long long*>(o);
-    }
+    double *dpts = nullptr, *dnrm = nullptr;
+    uint32_t* didx = nullptr;
+    unsigned long long* dcount = nullptr;
+    e = res.array(io->points_out, out_cols * 8, &dpts);
+    if (e == cudaSuccess && mode == OB_VOXEL_POINT_NORMAL) e = res.array(io->normals_out, 3 * 8, &dnrm);
+    if (e == cudaSuccess) e = res.array(io->indices_out, 4, &didx);
+    if (e == cudaSuccess) e = res.word(&dcount);
     if (e != cudaSuccess) return fail_cuda(e, "stage voxel outputs");
     e = io->dtype == OB_F64 ? run_voxel<double>(p, stg, st, dpts, dnrm, didx, dcount)
                             : run_voxel<float>(p, stg, st, dpts, dnrm, didx, dcount);
     if (e != cudaSuccess) return fail_cuda(e, "voxel downsample launch");
-    if (dev_count) return OB_OK;  // fully asynchronous: the count stays on the device next to the rows
-    unsigned long long total = 0;
-    e = cudaMemcpyAsync(&total, dcount, 8, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) return fail_cuda(e, "voxel count");
-    if (total) {
-        if (dpts != io->points_out) e = cudaMemcpyAsync(io->points_out, dpts, total * out_cols * 8, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess && dnrm && dnrm != io->normals_out)
-            e = cudaMemcpyAsync(io->normals_out, dnrm, total * 3 * 8, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess && didx && didx != io->indices_out)
-            e = cudaMemcpyAsync(io->indices_out, didx, total * 4, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        if (e != cudaSuccess) return fail_cuda(e, "voxel D2H");
-    }
-    *io->n_out = static_cast<size_t>(total);
-    return OB_OK;
+    return res.finish(dcount);
 }

@@ -890,32 +890,19 @@ cudaError_t run_emit(const ob_voxel_map* m, const uint32_t* sel, Staging& stg, c
     return cudaGetLastError();
 }
 
-// rows written to `out` (host or device) with the count to `n_out` (host: one synchronisation; device: none)
+// rows of the selected voxels of a non-empty map into `out` (null: count only), the count through `res`
 ob_status emit_rows(const ob_voxel_map* m, const uint32_t* sel, Staging& stg, cudaStream_t st, double* out,
-                    size_t capacity, size_t* n_out, const char* what) {
-    const bool dev_count = is_device_ptr(n_out);
-    const bool host_out = out && !is_device_ptr(out);
-    if (dev_count && host_out) return fail(OB_INVALID_ARGUMENT, "a device-side count needs device outputs");
-    const size_t row_bytes = (3 + m->na) * 8;
-    double* dout = out;
-    cudaError_t e = cudaSuccess;
-    if (host_out && capacity) e = scratch(stg, capacity * row_bytes, &dout);
-    unsigned long long* dn = reinterpret_cast<unsigned long long*>(n_out);
-    if (e == cudaSuccess && !dev_count) e = scratch(stg, 8, &dn);
+                    size_t capacity, CountedRows& res, const char* what) {
+    double* dout = nullptr;
+    unsigned long long* dn = nullptr;
+    cudaError_t e = res.array(out, (3 + m->na) * 8, &dout);
+    if (e == cudaSuccess) e = res.word(&dn);
     if (e == cudaSuccess) e = run_emit(m, sel, stg, st, dout, out ? capacity : 0, dn);
     if (e != cudaSuccess) return fail_cuda(e, what);
-    if (dev_count) return OB_OK;
-    unsigned long long total = 0;
-    e = cudaMemcpyAsync(&total, dn, 8, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e == cudaSuccess && host_out && total)
-        e = cudaMemcpyAsync(out, dout, std::min<size_t>(total, capacity) * row_bytes, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess && host_out) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) return fail_cuda(e, what);
-    *n_out = static_cast<size_t>(total);
-    if (out && total > capacity) return fail(OB_INVALID_ARGUMENT, "output capacity too small");
-    return OB_OK;
+    return res.finish(dn);
 }
+
+const char* const kMixedCount = "a device-side count needs device outputs";
 
 // max_voxel_dist_sq of remove_voxels_far_from_location (voxel_hash_map.cpp:112-113) in x86 int32 arithmetic
 int32_t cull_threshold(double max_distance, double inv) {
@@ -1030,18 +1017,15 @@ ob_status ob_voxel_map_add_rows(ob_voxel_map* m, const ob_map_rows* rows, ob_str
     if (rows->cols != 3 + m->na) return fail(OB_INVALID_ARGUMENT, kDimensionError);
     ob_status rs = require_device(m->device);
     if (rs != OB_OK) return rs;
-    const bool dev_n = rows->n_device != nullptr;
-    const size_t cap = dev_n ? rows->capacity : rows->n;
-    if (cap > 0x7fffffffu) return fail(OB_INVALID_ARGUMENT, "too many points in one call");
-    if (dev_n && !is_device_ptr(rows->n_device)) return fail(OB_INVALID_ARGUMENT, "n_device must be device memory");
-    if (cap && !rows->rows) return fail(OB_INVALID_ARGUMENT, "null rows buffer");
-    if (cap == 0) return OB_OK;
+    Rows r{};
+    rs = count_rows(rows->n, rows->n_device, rows->capacity, &r);
+    if (rs != OB_OK) return rs;
+    if (r.cap && !rows->rows) return fail(OB_INVALID_ARGUMENT, "null rows buffer");
+    if (r.cap == 0) return OB_OK;
     cudaStream_t st = stream_handle(s);
     Staging stg(st);
-    const void* d = nullptr;
-    cudaError_t e = stg.in(rows->rows, cap * rows->cols * 8, &d);
+    cudaError_t e = stg.in(rows->rows, r.cap * rows->cols * 8, &r.p);
     if (e != cudaSuccess) return fail_cuda(e, "stage voxel map rows");
-    const Rows r{d, reinterpret_cast<const unsigned long long*>(rows->n_device), rows->n, static_cast<unsigned>(cap)};
     return add_batch(m, r, static_cast<unsigned>(rows->cols), true, stg, st);
 }
 
@@ -1052,33 +1036,30 @@ ob_status ob_voxel_map_remove_far(ob_voxel_map* m, const ob_voxel_map_cull_io* i
     if (rs != OB_OK) return rs;
     cudaStream_t st = stream_handle(s);
     Staging stg(st);
+    const bool extract = io->n_extracted != nullptr;
+    // the kernel writes a device count itself: it is zeroed here only for an empty map or a refused call
+    CountedRows res(io->n_extracted, io->extracted ? io->capacity : CountedRows::kCountOnly, stg, st, "voxel map cull");
     const void* org = nullptr;
     cudaError_t e = stg.in(io->origin, 24, &org);
     if (e != cudaSuccess) return fail_cuda(e, "stage origin");
+    if (!m->cap) return res.zero();
+    if (extract) {  // refused before the cull, so a refused call leaves the map as it was
+        rs = res.refuse({io->extracted}, kMixedCount);
+        if (rs != OB_OK) return rs;
+    }
     uint32_t* removed = nullptr;
-    const bool extract = io->n_extracted != nullptr;
-    if (extract && m->cap) {
+    if (extract) {
         e = scratch(stg, m->cap * 4ull, &removed);
         if (e != cudaSuccess) return fail_cuda(e, "voxel map cull");
     }
-    if (m->cap) {
-        vm_cull_kernel<<<blocks_for(m->cap), 256, 0, st>>>(table_of(m), m->ctr, static_cast<const double*>(org), m->inv,
-                                                            cull_threshold(m->max_distance, m->inv), removed);
-        count_launch();
-        count_launch_of(OB_FAM_VOXEL_MAP);
-        e = cudaGetLastError();
-        if (e != cudaSuccess) return fail_cuda(e, "voxel map cull");
-    }
+    vm_cull_kernel<<<blocks_for(m->cap), 256, 0, st>>>(table_of(m), m->ctr, static_cast<const double*>(org), m->inv,
+                                                        cull_threshold(m->max_distance, m->inv), removed);
+    count_launch();
+    count_launch_of(OB_FAM_VOXEL_MAP);
+    e = cudaGetLastError();
+    if (e != cudaSuccess) return fail_cuda(e, "voxel map cull");
     if (!extract) return OB_OK;
-    if (!m->cap) {
-        if (is_device_ptr(io->n_extracted)) {
-            e = cudaMemsetAsync(io->n_extracted, 0, 8, st);
-            return e == cudaSuccess ? OB_OK : fail_cuda(e, "voxel map cull");
-        }
-        *io->n_extracted = 0;
-        return OB_OK;
-    }
-    return emit_rows(m, removed, stg, st, io->extracted, io->capacity, io->n_extracted, "voxel map extract");
+    return emit_rows(m, removed, stg, st, io->extracted, io->capacity, res, "voxel map extract");
 }
 
 ob_status ob_voxel_map_point_cloud(const ob_voxel_map* m, double* points, size_t capacity, size_t* n_out, ob_stream* s) {
@@ -1087,15 +1068,12 @@ ob_status ob_voxel_map_point_cloud(const ob_voxel_map* m, double* points, size_t
     if (rs != OB_OK) return rs;
     cudaStream_t st = stream_handle(s);
     Staging stg(st);
-    if (!m->cap) {
-        if (is_device_ptr(n_out)) {
-            cudaError_t e = cudaMemsetAsync(n_out, 0, 8, st);
-            return e == cudaSuccess ? OB_OK : fail_cuda(e, "voxel map point cloud");
-        }
-        *n_out = 0;
-        return OB_OK;
-    }
-    return emit_rows(m, nullptr, stg, st, points, capacity, n_out, "voxel map point cloud");
+    // as ob_voxel_map_remove_far: a device count is zeroed only for an empty map or a refused call
+    CountedRows res(n_out, points ? capacity : CountedRows::kCountOnly, stg, st, "voxel map point cloud");
+    if (!m->cap) return res.zero();
+    rs = res.refuse({points}, kMixedCount);
+    if (rs != OB_OK) return rs;
+    return emit_rows(m, nullptr, stg, st, points, capacity, res, "voxel map point cloud");
 }
 
 ob_status ob_voxel_map_size(const ob_voxel_map* m, size_t* voxels, size_t* points, ob_stream* s) {
@@ -1148,10 +1126,10 @@ ob_status ob_icp_linear_system(const ob_icp_system_io* io, ob_stream* s) {
     if (rs != OB_OK) return rs;
     cudaStream_t st = stream_handle(s);
     Staging stg(st);
-    const bool dev_n = io->n_device != nullptr;
-    const size_t cap = dev_n ? io->capacity : io->n;
-    if (cap > 0x7fffffffu) return fail(OB_INVALID_ARGUMENT, "too many pairs in one call");
-    if (dev_n && !is_device_ptr(io->n_device)) return fail(OB_INVALID_ARGUMENT, "n_device must be device memory");
+    Rows r{};
+    rs = count_rows(io->n, io->n_device, io->capacity, &r, "too many pairs in one call");
+    if (rs != OB_OK) return rs;
+    const size_t cap = r.cap;
     if (cap && (!io->source || !io->target)) return fail(OB_INVALID_ARGUMENT, "null pairs buffer");
     const void *src = nullptr, *tgt = nullptr;
     void *jtj = nullptr, *jtr = nullptr;
@@ -1160,7 +1138,7 @@ ob_status ob_icp_linear_system(const ob_icp_system_io* io, ob_stream* s) {
     if (e == cudaSuccess) e = stg.out(io->jtj, 36 * 8, &jtj);
     if (e == cudaSuccess) e = stg.out(io->jtr, 6 * 8, &jtr);
     // a host count travels by value as the clamp (cap == n), a device count is read by the kernels
-    const unsigned long long* n = reinterpret_cast<const unsigned long long*>(io->n_device);
+    const unsigned long long* n = r.n_dev;
     const unsigned slots = tree_slots(cap);
     double* val = nullptr;
     if (e == cudaSuccess) e = scratch(stg, slots * kSys * 8ull, &val);
@@ -1171,8 +1149,7 @@ ob_status ob_icp_linear_system(const ob_icp_system_io* io, ob_stream* s) {
     count_launch(2);
     count_launch_of(OB_FAM_ICP, 2);
     e = cudaGetLastError();
-    if (e == cudaSuccess) e = stg.flush();
-    if (e == cudaSuccess && (!is_device_ptr(io->jtj) || !is_device_ptr(io->jtr))) e = cudaStreamSynchronize(st);
+    if (e == cudaSuccess) e = stg.finish();
     if (e != cudaSuccess) return fail_cuda(e, "icp linear system");
     return OB_OK;
 }
@@ -1186,14 +1163,11 @@ ob_status ob_icp_align(const ob_voxel_map* m, const ob_icp_io* io, ob_stream* s)
     Rows r{};
     rs = stage_rows(&io->source, stg, &r, "stage icp source");
     if (rs != OB_OK) return rs;
-    const bool dev_pose = is_device_ptr(io->pose);
-    const bool dev_it = io->iterations == nullptr || is_device_ptr(io->iterations);
-    double* pose = io->pose;
-    int32_t* iters = io->iterations;
+    void *pose = nullptr, *iters = nullptr;
     IcpState* state = nullptr;
     cudaError_t e = scratch(stg, sizeof(IcpState), &state);
-    if (e == cudaSuccess && !dev_pose) e = scratch(stg, 16 * 8, &pose);
-    if (e == cudaSuccess && !dev_it) e = scratch(stg, 4, &iters);
+    if (e == cudaSuccess) e = stg.out(io->pose, 16 * 8, &pose);
+    if (e == cudaSuccess) e = stg.out(io->iterations, 4, &iters);
     const unsigned cap = std::max(r.cap, 1u);
     const unsigned nb = (cap + kAssocThreads - 1) / kAssocThreads;
     const unsigned slots = tree_slots(cap);
@@ -1221,15 +1195,12 @@ ob_status ob_icp_align(const ob_voxel_map* m, const ob_icp_io* io, ob_stream* s)
         icp_solve_kernel<<<1, kTreeThreads, 0, st>>>(val, crit_sq, state);
         launches += 4;
     }
-    icp_finish_kernel<<<1, 1, 0, st>>>(state, pose, iters);
+    icp_finish_kernel<<<1, 1, 0, st>>>(state, static_cast<double*>(pose), static_cast<int32_t*>(iters));
     count_launch(launches);
     count_launch_of(OB_FAM_ICP, launches);
     e = cudaGetLastError();
     if (e != cudaSuccess) return fail_cuda(e, "icp launch");
-    if (dev_pose && dev_it) return OB_OK;  // nothing waits for the GPU
-    if (!dev_pose) e = cudaMemcpyAsync(io->pose, pose, 16 * 8, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess && !dev_it) e = cudaMemcpyAsync(io->iterations, iters, 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    e = stg.finish();  // host pose / iterations: one wait; device ones: nothing waits for the GPU
     if (e != cudaSuccess) return fail_cuda(e, "icp result");
     return OB_OK;
 }
