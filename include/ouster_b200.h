@@ -54,7 +54,8 @@ int ob_abi_version(void);
  * "ob_voxel_io", "ob_point_rows", "ob_voxel_map_cull_io", "ob_voxel_query_io", "ob_icp_io", "ob_icp_system_io",
  * "ob_cloud_align_io", "ob_cloud_nearest_io", "ob_zone_desc", "ob_zone_render_io", "ob_zone_live", "ob_zone_state",
  * "ob_image_params", "ob_image_state", "ob_frame_field", "ob_frame_ops_io", "ob_frame_rows_entry",
- * "ob_frame_rows_io", "ob_map_rows", "ob_map_field", "ob_map_rows_item");
+ * "ob_frame_rows_io", "ob_map_rows", "ob_map_field", "ob_map_rows_item", "ob_interp_pose_io",
+ * "ob_frame_poses_item");
  * 0 for unknown names.  Lets FFI bindings verify their layout. */
 size_t ob_abi_sizeof(const char* struct_name);
 const char* ob_last_error(void);
@@ -63,7 +64,8 @@ int ob_device_count(void);
 /* kernels launched by this library since load (all threads); the bench's gpu_launches claim */
 uint64_t ob_kernel_launch_count(void);
 /* launches of one named kernel family since load: "decode_pipe" (pipelined K2), "decode" (K2, any
- * kernel), "cloud" (K1), "normals", "voxel", "voxel_map", "icp", "align", "zone", "image", "frame_ops"; 0 for unknown names.  Lets tests assert which code path ran. */
+ * kernel), "cloud" (K1), "normals", "voxel", "voxel_map", "icp", "align", "zone", "image", "frame_ops",
+ * "pose"; 0 for unknown names.  Lets tests assert which code path ran. */
 uint64_t ob_kernel_launch_count_of(const char* name);
 /* tuning hook (launch geometry and code-path selection only, never results): cloud_tw, cloud_stages,
  * cloud_threads (compute threads; a copy warp is added), cloud_ctas_per_sm, cloud_store_lag,
@@ -144,6 +146,75 @@ ob_status ob_destagger(size_t elem_size, size_t k, const void* img, const int32_
  */
 ob_status ob_dewarp(ob_dtype dtype, const void* points, const void* poses, size_t n_points,
                     size_t n_poses, void* out, ob_stream* s);
+
+/* ---- pose interpolation (DESIGN f-12) ----
+ * replaces core::interp_pose(x_interp, t0, x0, t1, x1)      ouster_core/include/ouster/core/pose_util.h:316-326
+ *          core::interp_pose(x_interp, x_known, poses_known) and the MatrixX16R<float | double> overload
+ *                                                            pose_util.h:360-434 (impl::interp_pose, :243-286)
+ *          python interp_pose / interp_pose_float            python/src/cpp/client/processing.cpp:241-338
+ * Between knots k[i] < k[i+1] the pose at x is a * exp((x - k[i]) * (1 / (k[i+1] - k[i])) * log(a^-1 b)), a and b
+ * the knots' poses; x is split into segments by the reference's lower_bound walk on any input, the part after the
+ * last knot takes the last segment, and x - k[i] is taken in the x dtype before it is widened.
+ * x_interp, x_known: float64 or int64 (x_dtype); poses_known m x 16 and poses n x 16 of pose_dtype (row-major 4x4):
+ * OB_F64 is interp_pose, OB_F32 is interp_pose_float (the known poses are widened, each result rounded once).
+ * two_pose = 1: interp_pose(x, t0, x0, t1, x1) with x_known = {t0, t1} (m == 2): no knot-order check, and the zero
+ * duration check runs even for n == 0.
+ * Errors, OB_INVALID_ARGUMENT with the reference's texts, in the reference's order: "Not enough evaluation poses for
+ * interpolation" (m < 2, on the host), then as the walk meets them "input x_known values are not monotonically
+ * increasing or values repeated", "Cannot interpolate with zero duration between poses" (|t1 - t0| < epsilon of the x
+ * dtype: never for int64) and "x_interp values must be monotonically increasing: <x[j]> < <x[j-1]>" (std::to_string).
+ * NaN compares false, so it never fails a check.  A failing call writes no pose.
+ * error == NULL: the call waits for the check and fails with the text; with host outputs it waits again for them.
+ * error = 3 int64 in DEVICE memory (poses must then be device memory too): nothing waits, the words (kind
+ * ob_pose_error, index, 0) are written in stream order and the call can be captured in a CUDA graph.
+ * Launches (family "pose"): three, one when n == 0.  Pointers may be host or device memory. */
+typedef enum ob_pose_x_dtype { OB_POSE_X_F64 = 0, OB_POSE_X_I64 = 1 } ob_pose_x_dtype;
+typedef enum ob_pose_error {
+    OB_POSE_OK = 0,
+    OB_POSE_KNOT_ORDER = 1,    /* index: i, with x_known[i] >= x_known[i + 1] */
+    OB_POSE_ZERO_DURATION = 2, /* index: the segment */
+    OB_POSE_DESCENT = 3        /* index: j, with x[j] < x[j - 1] (in ob_frames_interp_pose: the column) */
+} ob_pose_error;
+typedef struct ob_interp_pose_io {
+    const void* x_interp; /* n values of x_dtype */
+    size_t n;
+    const void* x_known;  /* m values of x_dtype */
+    size_t m;
+    int x_dtype;          /* ob_pose_x_dtype */
+    int pose_dtype;       /* ob_dtype */
+    int two_pose;
+    int pad;
+    const void* poses_known; /* m x 16 */
+    void* poses;             /* n x 16 */
+    int64_t* error;          /* NULL, or 3 words of device memory */
+} ob_interp_pose_io;
+ob_status ob_interp_pose(const ob_interp_pose_io* io, ob_stream* s);
+
+/* replaces mapping::ConstantVelocityDeskewMethod::update over a FrameSet     ouster_mapping/src/deskew_method.cpp:55-71
+ *          mapping::impl::interp_pose(frame, t0, x0, t1, x1)                 deskew_method.cpp:29-37
+ *          impl::init_valid_column_poses(frame_set, pose)  (x1 == NULL)      ouster_mapping/src/slam_util.cpp:129-140
+ * For every frame of the set in slot order (timestamps == NULL marks an empty slot): the valid columns
+ * (status & 1) get the pose at double(timestamp) * 1e-9 between (t0, x0) and (t1, x1); other columns keep their
+ * bytes.  x1 == NULL: every valid column gets x0.  x0 / x1: 16 doubles, host or device memory (e.g. a device pose of
+ * ob_icp_align).  Errors in the reference's order: "Cannot interpolate with zero duration between poses" is known
+ * on the host and fails the call before anything runs when the set has a frame; a decreasing valid timestamp in a
+ * frame fails "x_interp values must be monotonically increasing: ..." with the frames before it written and that
+ * frame and the later ones untouched.  error: as for ob_interp_pose (kind, column, slot); host poses are fine with
+ * it, since every frame's poses are copied in and out whole.
+ * Launches (family "pose"): two (a check block per frame, then the write), one with x1 == NULL, none for a set
+ * without columns.  Buffers may be host or device memory.
+ * CUDA graphs: with device buffers and a device error word the call can be captured once it has run on the stream
+ * with the same frames.  The frame table lives in the ob_stream and is rewritten in place by the next call on that
+ * stream with a different set, so a graph captured earlier then reads that set: after such a call, capture the
+ * graph again (or give each graph its own ob_stream). */
+typedef struct ob_frame_poses_item {
+    const uint64_t* timestamps; /* w: LidarFrame::timestamp; NULL: empty slot */
+    const uint32_t* status;     /* w: LidarFrame::status */
+    double* poses;              /* w x 16: LidarFrame::body_to_world */
+    size_t w;
+} ob_frame_poses_item;
+ob_status ob_frames_interp_pose(const ob_frame_poses_item* frames, size_t n_frames, double t0, const double* x0,
+                                double t1, const double* x1, int64_t* error, ob_stream* s);
 
 /* ---- range image -> world-frame point list (projection + pose + range filter + compaction) ----
  * replaces dewarp<T>(const LidarFrame&, const XYZLutT<T>&, min_range, max_range)

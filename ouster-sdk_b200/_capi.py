@@ -75,6 +75,20 @@ class MapRowsItem(C.Structure):
     _fields_ = [("lut", vp), ("range", vp), ("poses", vp), ("fields", C.POINTER(MapField)), ("n_fields", sz)]
 
 
+class InterpPoseIO(C.Structure):
+    """ob_interp_pose_io"""
+    _fields_ = [("x_interp", vp), ("n", sz), ("x_known", vp), ("m", sz), ("x_dtype", i32), ("pose_dtype", i32),
+                ("two_pose", i32), ("pad", i32), ("poses_known", vp), ("poses", vp), ("error", vp)]
+
+
+class FramePosesItem(C.Structure):
+    """ob_frame_poses_item"""
+    _fields_ = [("timestamps", vp), ("status", vp), ("poses", vp), ("w", sz)]
+
+
+OB_POSE_OK, OB_POSE_KNOT_ORDER, OB_POSE_ZERO_DURATION, OB_POSE_DESCENT = range(4)
+
+
 class VoxelMapCullIO(C.Structure):
     _fields_ = [("origin", vp), ("extracted", vp), ("capacity", sz), ("n_extracted", vp)]
 
@@ -266,6 +280,8 @@ _sig("ob_voxel_map_cols", i32, vp, C.POINTER(sz))
 _sig("ob_voxel_map_add_rows", i32, vp, C.POINTER(MapRows), vp)
 _sig("ob_frames_to_map_rows", i32, C.POINTER(MapRowsItem), sz, vp, sz, sz, vp, vp)
 _sig("ob_voxel_map_destroy", i32, vp)
+_sig("ob_interp_pose", i32, C.POINTER(InterpPoseIO), vp)
+_sig("ob_frames_interp_pose", i32, C.POINTER(FramePosesItem), sz, C.c_double, vp, C.c_double, vp, vp, vp)
 _sig("ob_voxel_map_clear", i32, vp, vp)
 _sig("ob_voxel_map_add_points", i32, vp, C.POINTER(PointRows), vp)
 _sig("ob_voxel_map_remove_far", i32, vp, C.POINTER(VoxelMapCullIO), vp)

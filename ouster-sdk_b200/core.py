@@ -962,6 +962,69 @@ def dewarp_frames(frames, min_range=0.0, max_range=float("inf"), provenance=Fals
     return pts[:k]
 
 
+def interp_pose(x_interp, x_known, poses_known, two_pose=False, error=None, out=None, stream=None, device=0):
+    """ob_interp_pose: x_interp (n,) and x_known (m,) of float64 or int64 (an integer x is read as int64, anything
+    else as float64), poses_known (m, 4, 4) of float32 or float64 -> (n, 4, 4) of the poses' dtype, numpy in and
+    out, or CUDA tensors on their device.  two_pose: x_known = (t0, t1), the interp_pose(x, t0, x0, t1, x1) form.
+    error: a device int64 tensor of 3 words (kind, index, 0) written in stream order; nothing waits, and a failing
+    call leaves `out` unwritten.  Without it, errors raise ValueError with the reference's texts."""
+    def xconv(a):
+        if _is_torch(a):
+            import torch
+            return a.contiguous() if a.dtype in (torch.int64, torch.float64) else \
+                a.to(torch.int64 if not a.is_floating_point() else torch.float64).contiguous()
+        a = np.asarray(a)
+        return np.ascontiguousarray(a, np.int64 if a.dtype.kind in "iu" else np.float64)
+    x, k = xconv(x_interp).reshape(-1), xconv(x_known).reshape(-1)
+    if _np_dtype(x) != _np_dtype(k):
+        raise ValueError("x_interp and x_known must have one dtype")
+    pk = _contig(poses_known, floats=True)
+    n, m = _numel(x), _numel(k)
+    if _numel(pk) != m * 16:
+        raise ValueError("x_known and poses_known sizes are not matching")
+    pdt = _np_dtype(pk)
+    if out is None:
+        out = _empty(x if (_is_torch(x) and x.is_cuda) else pk, (n, 4, 4), pdt)
+    io = _capi.InterpPoseIO()
+    io.x_interp, io.n, io.x_known, io.m = _ptr(x), n, _ptr(k), m
+    io.x_dtype = 1 if _np_dtype(x) == np.int64 else 0
+    io.pose_dtype = _capi.OB_F64 if pdt == np.float64 else _capi.OB_F32
+    io.two_pose, io.poses_known, io.poses, io.error = int(two_pose), _ptr(pk), _ptr(out), _ptr(error)
+    st = _stream_for(x, stream, device)
+    check(lib.ob_interp_pose(C.byref(io), st.h))
+    return out
+
+
+def frames_interp_pose(frames, t0, x0, t1=None, x1=None, error=None, stream=None, device=0):
+    """ob_frames_interp_pose: ConstantVelocityDeskewMethod::update over a frame set.  `frames`: one entry per slot,
+    None for an empty slot, else (timestamps (W,) uint64, status (W,) uint32, poses (W, 4, 4) float64, written in
+    place) -- numpy arrays or CUDA tensors, e.g. the column headers core.Decoder.decode writes (uint64 / uint32 data
+    in int64 / int32 tensors).  x0 / x1: 4 x 4 float64, host or device; x1 None: every valid column gets x0.
+    error: optional device int64 tensor of 3 words (kind, column, slot); nothing waits with device buffers."""
+    items = (_capi.FramePosesItem * max(len(frames), 1))()
+    keep, ref = [], None
+    for i, fr in enumerate(frames):
+        if fr is None:
+            continue
+        ts, stt, poses = fr
+        w = _numel(ts)
+        if _numel(stt) != w or _numel(poses) != w * 16:
+            raise ValueError("timestamps, status and poses must be [W], [W] and [W, 4, 4]")
+        if _is_torch(poses):
+            assert poses.is_contiguous(), "poses must be contiguous: they are written in place"
+        else:
+            assert poses.dtype == np.float64 and poses.flags["C_CONTIGUOUS"], "poses must be C-contiguous float64"
+        ts, stt = _contig(ts, np.uint64), _contig(stt, np.uint32)
+        keep += [ts, stt]
+        ref = ref if ref is not None else poses
+        items[i].timestamps, items[i].status, items[i].poses, items[i].w = _ptr(ts), _ptr(stt), _ptr(poses), w
+    a0 = _contig(x0, np.float64)
+    a1 = None if x1 is None else _contig(x1, np.float64)
+    st = _stream_for(ref if ref is not None else a0, stream, device)
+    check(lib.ob_frames_interp_pose(items, len(frames), float(t0), _ptr(a0), float(t1 if t1 is not None else 0.0),
+                                    _ptr(a1), _ptr(error), st.h))
+
+
 def transform(points, pose, out=None, stream=None, device=0):
     """transform(points (..., 3), pose (4, 4)): one pose for every point (pose_util.h:118-131)."""
     pose = pose if _is_torch(pose) else np.ascontiguousarray(pose, _np_dtype(points)).reshape(1, 16)

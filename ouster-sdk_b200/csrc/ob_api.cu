@@ -19,7 +19,7 @@ static std::atomic<uint64_t> g_launches{0};
 static std::atomic<uint64_t> g_family[OB_FAM_COUNT];
 static const char* const kFamilies[OB_FAM_COUNT] = {"decode_pipe", "decode", "cloud", "normals", "voxel",
                                                     "voxel_map", "icp", "align", "zone", "image",
-                                                    "frame_ops"};
+                                                    "frame_ops", "pose"};
 
 void count_launch(uint64_t n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 void count_launch_of(int family, uint64_t n) {
@@ -333,7 +333,7 @@ struct ob_stream {
         void* dev{nullptr};
         size_t cap{0};
         std::vector<uint8_t> host;
-    } tables[2];
+    } tables[3];
 };
 
 struct ob_lut {
@@ -356,7 +356,7 @@ LutView lut_view(const ob_lut* lut) {
 cudaStream_t stream_handle(ob_stream* s) { return s->st; }
 
 cudaError_t stream_table(ob_stream* s, int which, const void* host, size_t bytes, const void** dev) {
-    ob_stream::Table& t = s->tables[which & 1];
+    ob_stream::Table& t = s->tables[which];
     if (t.dev != nullptr && t.host.size() == bytes && std::memcmp(t.host.data(), host, bytes) == 0) {
         *dev = t.dev;  // identical to what the device already holds
         return cudaSuccess;
@@ -424,6 +424,8 @@ size_t ob_abi_sizeof(const char* name) {
     if (n == "ob_map_rows") return sizeof(ob_map_rows);
     if (n == "ob_map_field") return sizeof(ob_map_field);
     if (n == "ob_map_rows_item") return sizeof(ob_map_rows_item);
+    if (n == "ob_interp_pose_io") return sizeof(ob_interp_pose_io);
+    if (n == "ob_frame_poses_item") return sizeof(ob_frame_poses_item);
     return 0;
 }
 

@@ -102,7 +102,7 @@ struct LutView {
 };
 LutView lut_view(const ob_lut* lut);
 cudaStream_t stream_handle(ob_stream* s);
-// device copy of a small per-launch table (which: 0 decode frames, 1 encode frames), re-uploaded only when
+// device copy of a small per-launch table (which: 0 decode frames, 1 encode frames, 2 pose frames), re-uploaded only when
 // its contents changed since the stream's previous launch of that kind
 cudaError_t stream_table(ob_stream* s, int which, const void* host, size_t bytes, const void** dev);
 int stream_device(ob_stream* s);

@@ -190,7 +190,7 @@ cudaError_t make_decode_params(const DecodeLaunch& a, int device, bool pipe, Dec
 void count_launch(uint64_t n = 1);
 enum { OB_FAM_DECODE_PIPE = 0, OB_FAM_DECODE = 1, OB_FAM_CLOUD = 2, OB_FAM_NORMALS = 3, OB_FAM_VOXEL = 4,
        OB_FAM_VOXEL_MAP = 5, OB_FAM_ICP = 6, OB_FAM_ALIGN = 7, OB_FAM_ZONE = 8, OB_FAM_IMAGE = 9,
-       OB_FAM_FRAME_OPS = 10, OB_FAM_COUNT = 11 };
+       OB_FAM_FRAME_OPS = 10, OB_FAM_POSE = 11, OB_FAM_COUNT = 12 };
 void count_launch_of(int family, uint64_t n = 1);
 
 }  // namespace ob

@@ -8,6 +8,8 @@
 #include <climits>
 #include <cstdint>
 
+#include "ob_se3.cuh"  // mul / add / sub / sqn3
+
 namespace ob {
 namespace {
 
@@ -37,12 +39,6 @@ __device__ __forceinline__ int32_t voxel_coord(double v) {
     if (!(f >= -2147483648.0 && f < 2147483648.0)) return INT_MIN;
     return static_cast<int32_t>(f);
 }
-
-__device__ __forceinline__ double mul(double a, double b) { return __dmul_rn(a, b); }
-__device__ __forceinline__ double add(double a, double b) { return __dadd_rn(a, b); }
-__device__ __forceinline__ double sub(double a, double b) { return __dsub_rn(a, b); }
-// squaredNorm of a 3-vector, (x0*x0 + x1*x1) + x2*x2 as in ob_normals.cu (DESIGN 2)
-__device__ __forceinline__ double sqn3(double a, double b, double c) { return add(add(mul(a, a), mul(b, b)), mul(c, c)); }
 
 // first_n_point's rejection test (voxel_hash_map.h:293-296): a kept point q is within the map resolution of p
 __device__ __forceinline__ bool within_resolution(double qx, double qy, double qz, double px, double py, double pz,

@@ -526,6 +526,118 @@ class AdaptiveThreshold:
 # ouster.sdk.algorithm.point_to_point_align / point_to_plane_align (python/src/cpp/_algorithm.cpp:158-245): numpy in,
 # a (4, 4) float64 numpy array out, as in the reference; CUDA tensors in give a CUDA tensor out with no host wait.
 
+def _interp_pose(x_interp, x_known, poses_known, pose_dtype):
+    """processing.cpp:241-338: shapes (N,) or (N, 1), x as float64, poses (M, 4, 4) converted to pose_dtype."""
+    def xshape(a, name):
+        if len(a.shape) != 1 and (len(a.shape) != 2 or a.shape[1] != 1):
+            raise RuntimeError(f"{name} must have shape (N,) or (N,1)")
+    xshape(x_interp, "x_interp")
+    xshape(x_known, "x_known")
+    if len(poses_known.shape) != 3 or tuple(poses_known.shape[1:]) != (4, 4):
+        raise RuntimeError("poses_known must have shape (M, 4, 4)")
+    if x_known.shape[0] != poses_known.shape[0]:
+        raise RuntimeError("The number of poses in poses_known must match the number of values in x_known")
+    if x_known.shape[0] < 2:
+        raise ValueError("Not enough evaluation poses for interpolation")
+    if _c._is_torch(x_interp):
+        torch = _torch()
+        tdt = torch.float64 if pose_dtype == np.float64 else torch.float32
+        x, k = x_interp.to(torch.float64), x_known.to(x_interp.device, torch.float64)
+        pk = poses_known.to(x_interp.device, tdt)
+    else:
+        x, k = np.asarray(x_interp, np.float64), np.asarray(x_known, np.float64)
+        pk = np.asarray(poses_known, pose_dtype)
+    return _c.interp_pose(x, k, pk)
+
+
+def interp_pose(x_interp, x_known, poses_known):
+    """Interpolate 4x4 poses at x_interp (float64): (N, 4, 4) float64 (processing.cpp:1017-1027).  numpy in and out,
+    or CUDA tensors on their device."""
+    return _interp_pose(x_interp, x_known, poses_known, np.float64)
+
+
+def interp_pose_float(x_interp, x_known, poses_known):
+    """interp_pose with float32 poses: known poses widened, each result rounded once (processing.cpp:1029-1039)."""
+    return _interp_pose(x_interp, x_known, poses_known, np.float32)
+
+
+class DeskewMethod:
+    """mapping::DeskewMethod (deskew_method.h, _mapping_slam.cpp:238-270): keeps the last two registered poses."""
+
+    def __init__(self, infos, initial_pose=None):
+        if len(infos) == 0:
+            raise ValueError("No sensor info provided for slam")
+        self._ts, self._poses = [], []
+        self._initial = np.eye(4) if initial_pose is None else np.array(initial_pose, np.float64).reshape(4, 4)
+
+    def set_last_pose(self, ts, pose):
+        pose = np.asarray(pose, np.float64)
+        if pose.shape != (4, 4):
+            raise RuntimeError("pose must be a (4,4) array representing a transformation matrix")
+        if len(self._ts) >= 2:
+            self._ts.pop(0)
+            self._poses.pop(0)
+        self._ts.append(int(ts) * 1e-9)
+        self._poses.append(pose.copy())
+
+    def finalize_after_registration(self, frames, anchor_timestamp_ns, corrected_anchor_pose):
+        self.set_last_pose(anchor_timestamp_ns, corrected_anchor_pose)
+
+    def update(self, frames):
+        raise NotImplementedError
+
+
+class ConstantVelocityDeskewMethod(DeskewMethod):
+    """ConstantVelocityDeskewMethod::update (deskew_method.cpp:55-71): every valid column of every frame gets the
+    pose at its timestamp on the motion through the last two poses, or the initial pose before there are two.
+    `frames`: a list with None for empty slots, of LidarScan or DeviceLidarScan (whose poses are host-side).
+    One ob_frames_interp_pose call for the whole set."""
+
+    def update(self, frames):
+        items = []
+        for f in frames:
+            if f is None:
+                items.append(None)
+                continue
+            host = f.host if isinstance(f, DeviceLidarScan) else f
+            items.append((host.timestamp, host.status, host.body_to_world))
+        if len(self._ts) < 2:
+            _c.frames_interp_pose(items, 0.0, self._initial)
+        else:
+            _c.frames_interp_pose(items, self._ts[0], self._poses[0], self._ts[-1], self._poses[-1])
+        return frames
+
+
+def _imu_measurements_per_frame(info):
+    """format.imu_measurements_per_packet * format.imu_packets_per_frame (deskew_method.cpp:800-801) of a sensor
+    info object or metadata dict; 0 when the info has no format."""
+    fmt = _sensor_value(info, "format")
+    if fmt is None:
+        return 0
+    return int(_sensor_value(fmt, "imu_measurements_per_packet", 0) or 0) * \
+        int(_sensor_value(fmt, "imu_packets_per_frame", 0) or 0)
+
+
+class DeskewMethodFactory:
+    """DeskewMethodFactory::create (deskew_method.cpp:790-832).  IMU packets are not decoded in this project, so
+    "imu_deskew", and "auto" when a sensor reports IMU measurements, raise instead of deskewing (DESIGN 9)."""
+
+    @staticmethod
+    def create(method_name, infos):
+        if method_name == "none":
+            return None
+        if method_name == "constant_velocity":
+            return ConstantVelocityDeskewMethod(infos)
+        imu_text = "IMU deskew is not supported: IMU packets are not decoded"
+        if method_name == "imu_deskew":
+            raise ValueError(imu_text)
+        if method_name == "auto":
+            if any(_imu_measurements_per_frame(i) > 0 for i in infos):
+                raise ValueError(imu_text)
+            return ConstantVelocityDeskewMethod(infos)
+        raise ValueError("Invalid deskew_method: " + method_name)
+
+
 def point_to_point_align(source_points, target_points, initial_guess=None, max_corr_dist=0.25):
     """source_to_target_transform by point-to-point ICP with MAD-scaled Huber weights (at most 10 iterations);
     initial_guess (identity when None) comes back when fewer than 20 usable points or correspondences exist."""

@@ -389,4 +389,26 @@ fr32 = ob.LidarFrame(si32)
 fr32.field("RANGE")[...] = rf.integers(0, 20000, fr32.field("RANGE").shape)
 ob.frame_ops.filter_xyz(fr32, lut, 2, -0.2, 0.2, dewarp_points=True)
 print("frame ops ok")
+# pose interpolation (f-12): sorted, unsorted and NaN x, both dtypes, an error case, and the frame form
+from oracle import pose as opose  # noqa: E402
+rp = np.random.default_rng(23)
+kp = np.cumsum(rp.random(7) + 0.1)
+pkp = np.stack([opose.posev_exp(np.concatenate([rp.normal(size=3) * 0.3, rp.normal(size=3)])) for _ in kp])
+for xs in (np.sort(rp.uniform(0, kp[-1] + 1, 300)), np.where(rp.random(300) < 0.1, np.nan,
+                                                               np.sort(rp.uniform(0, 9, 300)))):
+    assert np.allclose(ob.core.interp_pose(xs, kp, pkp), opose.interp_pose(xs, kp, pkp), atol=1e-9, equal_nan=True)
+    ob.core.interp_pose(xs, kp, pkp.astype(np.float32))
+xi = np.sort(rp.integers(0, 10**6, 200))
+ob.core.interp_pose(xi, np.array([0, 10**6], np.int64), pkp[:2], two_pose=True)
+try:
+    ob.core.interp_pose(np.array([0.5, 0.2]), kp, pkp)
+    raise AssertionError("descent not reported")
+except ValueError:
+    pass
+tsp = (10**9 + np.arange(100) * 10**6).astype(np.uint64)
+stp = (rp.random(100) < 0.7).astype(np.uint32)
+psp = np.zeros((100, 4, 4))
+ob.core.frames_interp_pose([(tsp, stp, psp), None], 1.0, pkp[0], 1.1, pkp[1])
+ob.core.frames_interp_pose([(tsp, stp, psp)], 0.0, pkp[0])
+print("pose ok")
 print("SANITIZE CASES OK")
