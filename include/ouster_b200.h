@@ -945,7 +945,10 @@ ob_status ob_decode_job_destroy(ob_decode_job* job);
  * with_crc != 0 writes the CRC64 of bytes [0, packet_size - 8) into the last 8 bytes (standard headers,
  * non-LEGACY profiles -- the caller decides, as frame_to_packets does at :512-518).  Every one of the
  * w / columns_per_packet packets is produced; dropping packets "with ts == 0 and no valid column"
- * (:497-500) is the caller's (host-side) choice.  Buffers may be host or device memory.
+ * (:497-500) is the caller's (host-side) choice.  Buffers may be host or device memory; the bytes between
+ * packets (packet_stride > packet_size) are not written.  Fields are set in decoder order, each clearing
+ * its mask's bits first, so where masks overlap the last field wins, as in set_block.  Every field's mask
+ * must lie inside its pixel (offset + bytes up to the mask's top bit <= channel_data_size).
  * errors: "Mismatch between expected number of packets and PacketFormat.columns_per_packet". */
 typedef struct ob_encode_io {
     const void* fields[OB_MAX_FIELDS];

@@ -636,6 +636,15 @@ ob_status ob_encode_frames(const ob_decoder* dec, const ob_encode_io* frames, si
         return fail(OB_INVALID_ARGUMENT, "Mismatch between expected number of packets and PacketFormat.columns_per_packet");
     if (with_crc && (L.packet_size % 4 != 0 || L.packet_size < 8))
         return fail(OB_INVALID_ARGUMENT, "packet size must be a multiple of 4 for the CRC64 footer");
+    // The encoder clears and sets each field's mask in place, one thread per pixel.  That gives the reference's
+    // result only when no mask reaches into a neighbouring pixel's bytes; which pixel the reference writes
+    // last would then decide the overlap, and the encoder does not reproduce that order.
+    for (uint32_t k = 0; k < L.n_fields; ++k) {
+        const uint64_t m = L.fields[k].mask;
+        const uint32_t span = m ? (64u - static_cast<uint32_t>(__builtin_clzll(m)) + 7u) / 8u : 0u;
+        if (static_cast<uint64_t>(L.fields[k].offset) + span > L.channel_data_size)
+            return fail(OB_INVALID_ARGUMENT, "field mask reaches past the pixel's channel data; cannot encode");
+    }
     rs = require_device(device);
     if (rs != OB_OK) return rs;
     cudaStream_t st = stream_handle(s);
@@ -671,8 +680,12 @@ ob_status ob_encode_frames(const ob_decoder* dec, const ob_encode_io* frames, si
             f.packet_headers = static_cast<const uint8_t*>(d);
             f.header_bytes = static_cast<uint32_t>(io.packet_header_bytes);
         }
+        // the kernel writes packet_size bytes of every packet_stride; a host buffer with gaps between packets is
+        // uploaded first so that its copy back leaves the gaps as the caller had them
         void* o = nullptr;
-        if (e == cudaSuccess) e = stg.out(io.packets, (n_pk - 1) * io.packet_stride + L.packet_size, &o);
+        const size_t span = (n_pk - 1) * io.packet_stride + L.packet_size;
+        if (e == cudaSuccess)
+            e = io.packet_stride == L.packet_size ? stg.out(io.packets, span, &o) : stg.inout(io.packets, span, &o);
         if (e != cudaSuccess) return fail_cuda(e, "stage encode buffers");
         f.packets = static_cast<uint8_t*>(o);
         f.packet_stride = io.packet_stride;

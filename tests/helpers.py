@@ -104,11 +104,12 @@ def col_map_from_packets(pf, packets):
     return col_src
 
 
-def random_frame(pf, seed, with_window=True, frame_id=700):
+def random_frame(pf, seed, with_window=True, frame_id=700, extra_fields=()):
     """Random LidarFrame as tests/packet_format_test.cpp:246-266 builds it: every profile field
-    drawn within its value mask, headers iota, status 1."""
+    drawn within its value mask, headers iota, status 1.  extra_fields: [(name, orc type tag)] added to
+    the frame's default fields (and drawn too when the profile carries them)."""
     from oracle import oracle as orc
-    f = orc.Frame(pf, with_window=with_window)
+    f = orc.Frame(pf, with_window=with_window, extra_fields=extra_fields)
     rs = np.random.default_rng(seed)
     w = pf.columns_per_frame
     f.measurement_id[:] = np.arange(w)

@@ -173,20 +173,34 @@ def test_custom_profile_through_batcher(ob):
         assert np.array_equal(fr.field(n), fr2.field(n)), n
 
 
+# the named fields FIVE_WORD_PIXEL's RAW32_WORD1..5 cover (tests/golden/profile_tables.json)
+FIVE_WORD_NAMED_FIELDS = {"FLAGS": np.uint8, "FLAGS2": np.uint8, "NEAR_IR": np.uint16, "RANGE": np.uint32,
+                          "RANGE2": np.uint32, "REFLECTIVITY": np.uint8, "REFLECTIVITY2": np.uint8,
+                          "SIGNAL": np.uint16, "SIGNAL2": np.uint16}
+
+
 @pytest.mark.parametrize("profile,header,h,w", [
     ("RNG19_RFL8_SIG16_NIR16_DUAL", "STANDARD", 128, 1024), ("RNG19_RFL8_SIG16_NIR16", "STANDARD", 64, 512),
     ("RNG15_RFL8_NIR8", "STANDARD", 32, 512), ("LEGACY", "STANDARD", 32, 512),
     ("FUSA_RNG15_RFL8_NIR8_DUAL", "FUSA", 32, 512), ("RNG19_RFL8_SIG16_NIR16_RGB16", "STANDARD", 32, 512),
+    ("FIVE_WORD_PIXEL", "STANDARD", 32, 512), ("RNG15_RFL8_NIR8_DUAL", "STANDARD", 64, 512),
+    ("RNG15_RFL8_WIN8", "STANDARD", 32, 512), ("RNG19_RFL8_SIG16_NIR16_ZONE16", "STANDARD", 32, 512),
+    ("RNG15_RFL8_NIR8_ZONE16", "STANDARD", 32, 512), ("RNG19_RFL8_SIG16_ZONE16_DUAL", "STANDARD", 32, 512),
+    ("RNG19_RFL8_SIG16_NIR16_RGB16_DUAL", "STANDARD", 32, 512),
 ])
 def test_gpu_frame_to_packets_is_byte_identical(ob, profile, header, h, w):
     """K4 (ob_encode_frames): set_block of every field + column headers + CRC64 on the device ==
     the host encoder == the oracle's frame_to_packets (impl/lidar_frame_impl.h:435-531), byte for
-    byte, including invalid columns (no pixel data) and packets that are not emitted at all."""
-    from tests.helpers import oracle_pf, random_frame
+    byte, including invalid columns (no pixel data) and packets that are not emitted at all.
+    FIVE_WORD_PIXEL's frame also carries the named fields its RAW32 words cover, each drawn on its
+    own: where masks overlap, the field set last (PacketFormat order) decides the bits."""
     si = ob.SensorInfo(profile, h, w, 16, header_type=header, fw_rev="v3.2.1")
     masks = {f[0]: f[6] for f in si.fields()}
     rs = np.random.default_rng(99)
     src = ob.LidarFrame(si)
+    if profile == "FIVE_WORD_PIXEL":
+        for name, dt in FIVE_WORD_NAMED_FIELDS.items():
+            src.add_field(name, dt)
     for name in src.fields:
         a = src.field(name)
         a[...] = (rs.integers(0, 1 << 32, size=a.shape, dtype=np.uint64) & np.uint64(masks.get(name, 0xffff))).astype(a.dtype)
@@ -205,5 +219,19 @@ def test_gpu_frame_to_packets_is_byte_identical(ob, profile, header, h, w):
     assert np.array_equal(host_ts, dev_ts)
     assert np.array_equal(host_pk, dev_pk)
     if profile != "LEGACY" and header == "STANDARD":   # the CRC the sensor would have computed
-        for p in dev_pk[:3]:
-            assert int(p[-8:].view(np.uint64)[0]) == si.calculate_crc(p)
+        for p in dev_pk:
+            crc = int(p[-8:].view(np.uint64)[0])
+            assert crc == si.calculate_crc(p) == orc.crc64(p[:-8])
+    if profile == "FIVE_WORD_PIXEL":   # the overlaps really disagree, and the oracle agrees on the outcome
+        opf = oracle_pf(profile, h, w, 16, header)
+        of = orc.Frame(opf, with_window=False,
+                       extra_fields=[(n, orc.NP_TYPE[np.dtype(dt)]) for n, dt in FIVE_WORD_NAMED_FIELDS.items()])
+        assert set(opf.field_names) <= set(src.fields) and set(opf.field_names) <= set(of.field_names)
+        for name in opf.field_names:
+            of.field(name)[...] = src.field(name)
+        of.timestamp[:], of.status[:] = src.timestamp, src.status
+        of.packet_timestamp[:], of.alert_flags[:] = src.packet_timestamp, src.alert_flags
+        of.frame_id = src.frame_id
+        opk, _ = orc.frame_to_packets(of, opf, init_id=77, prod_sn=991)
+        assert np.array_equal(opk, dev_pk)
+        assert np.any(src.field("RANGE") != (src.field("RAW32_WORD1") & np.uint32(0x7ffff)))
