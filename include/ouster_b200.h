@@ -61,11 +61,14 @@ size_t ob_abi_sizeof(const char* struct_name);
 const char* ob_last_error(void);
 /* number of visible CUDA devices (0 without a driver/GPU); never fails */
 int ob_device_count(void);
-/* kernels launched by this library since load (all threads); the bench's gpu_launches claim */
+/* kernels launched by this library since load (all threads), not counting those CUB launches inside its
+ * sorts and scans; the sum of the families below except "decode_pipe".  The bench's gpu_launches claim */
 uint64_t ob_kernel_launch_count(void);
-/* launches of one named kernel family since load: "decode_pipe" (pipelined K2), "decode" (K2, any
- * kernel), "cloud" (K1), "normals", "voxel", "voxel_map", "icp", "align", "zone", "image", "frame_ops",
- * "pose"; 0 for unknown names.  Lets tests assert which code path ran. */
+/* launches of one named kernel family since load: "decode_pipe" (pipelined K2, also counted in "decode"),
+ * "decode" (K2, any kernel), "cloud" (K1), "normals", "voxel", "voxel_map", "icp", "align", "zone", "image",
+ * "frame_ops", "pose", "dewarp" (K3 and the per-column dewarp), "destagger", "lut" (LUT from intrinsics and
+ * its f32 cast), "encode" (K4); 0 for unknown names.  Every launch belongs to exactly one family, so tests
+ * can assert which code path ran. */
 uint64_t ob_kernel_launch_count_of(const char* name);
 /* tuning hook (launch geometry and code-path selection only, never results): cloud_tw, cloud_stages,
  * cloud_threads (compute threads; a copy warp is added), cloud_ctas_per_sm, cloud_store_lag,

@@ -22,7 +22,13 @@ def device_count():
 
 
 def kernel_launch_count(name=None):
-    """Kernels launched since load; `name` restricts the count to one family ("decode_pipe", ...)."""
+    """Kernels launched since load; `name` restricts the count to one family.
+
+    Families: "decode" (K2, any kernel) with its sub-family "decode_pipe" (pipelined K2), "cloud" (K1),
+    "normals", "voxel", "voxel_map", "icp", "align", "zone", "image", "frame_ops", "pose", "dewarp",
+    "destagger", "lut" and "encode" (K4).  Every launch is in exactly one family, so the total is the sum of
+    the families other than "decode_pipe".  Kernels CUB launches inside sorts and scans are not counted.
+    """
     if name is not None:
         return lib.ob_kernel_launch_count_of(name.encode())
     return lib.ob_kernel_launch_count()

@@ -636,8 +636,7 @@ size_t elem_size(int32_t dtype) { return dtype == OB_F64 ? 8 : 4; }
 
 // SpatialHashGrid3D over `t` (with the normal filter when normals != null), built on the stream
 template <typename T>
-cudaError_t build_grid(const Rows& t, const void* normals, double cell_size, Staging& stg, cudaStream_t st, Grid* g,
-                       uint64_t* launches) {
+cudaError_t build_grid(const Rows& t, const void* normals, double cell_size, Staging& stg, cudaStream_t st, Grid* g) {
     const unsigned cap = std::max(t.cap, 1u);
     unsigned slots = 64;
     while (slots < 2 * cap) slots <<= 1;
@@ -673,15 +672,15 @@ cudaError_t build_grid(const Rows& t, const void* normals, double cell_size, Sta
     Rows tc = t;
     tc.cap = cap;  // rows_n() still clamps to the real count; rows past it get the pad bit
     if (t.cap == 0) tc.n_dev = nullptr, tc.n_host = 0;
-    gr_key_kernel<T><<<nb, 256, 0, st>>>(tc, normals, 1.0 / cell_size, keys, seq);
+    launch(OB_FAM_ALIGN, gr_key_kernel<T>, nb, 256, 0, st, tc, normals, 1.0 / cell_size, keys, seq);
     e = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, sk, seq, sseq, static_cast<int>(cap), GKeyDecomposer{}, 0,
                                         kGKeyBits, st);
     if (e != cudaSuccess) return e;
-    gr_head_kernel<<<nb, 256, 0, st>>>(cap, sk, head);
+    launch(OB_FAM_ALIGN, gr_head_kernel, nb, 256, 0, st, cap, sk, head);
     e = cub::DeviceScan::InclusiveSum(tmp, tmp_bytes, head, cid, static_cast<int>(cap), st);
     if (e != cudaSuccess) return e;
-    gr_fill_kernel<T><<<nb, 256, 0, st>>>(cap, t.p, sk, sseq, cid, ckey, cbeg, cend, table, slots - 1, pts, row);
-    *launches += 3;
+    launch(OB_FAM_ALIGN, gr_fill_kernel<T>, nb, 256, 0, st, cap, t.p, sk, sseq, cid, ckey, cbeg, cend, table, slots - 1,
+           pts, row);
     *g = Grid{ckey, cbeg, cend, table, slots - 1, pts, row, 1.0 / cell_size};
     return cudaGetLastError();
 }
@@ -690,9 +689,8 @@ template <typename T>
 ob_status run_align(const ob_cloud_align_io* io, const Rows& sr, const Rows& tr, const void* snrm, const void* tnrm,
                     const double* guess, Staging& stg, cudaStream_t st, double* pose, int32_t* iters) {
     const bool plane = io->mode == OB_ALIGN_POINT_TO_PLANE;
-    uint64_t launches = 0;
     Grid g{};
-    cudaError_t e = build_grid<T>(tr, plane ? tnrm : nullptr, io->max_corr_dist, stg, st, &g, &launches);
+    cudaError_t e = build_grid<T>(tr, plane ? tnrm : nullptr, io->max_corr_dist, stg, st, &g);
     if (e != cudaSuccess) return fail_cuda(e, "cloud align grid");
     const unsigned kcap = std::max(sr.cap, 1u);
     const unsigned nb = (kcap + kThreads - 1) / kThreads;
@@ -718,34 +716,31 @@ ob_status run_align(const ob_cloud_align_io* io, const Rows& sr, const Rows& tr,
     const double max_d2 = io->max_corr_dist * io->max_corr_dist;
     const double cos_gate = plane ? std::cos(io->max_normal_angle_deg * M_PI / 180.0) : 0.0;
     const unsigned lb = (slots + 255) / 256;
-    al_init_kernel<<<1, 1, 0, st>>>(sr, tr, guess, state);
-    launches += 1;
+    launch(OB_FAM_ALIGN, al_init_kernel, 1, 1, 0, st, sr, tr, guess, state);
     for (int it = 0; it < kMaxIterations; ++it) {
         if (plane)
-            al_assoc_kernel<T, true><<<nb, kThreads, 0, st>>>(sr, snrm, tr.p, tnrm, g, max_d2, cos_gate, kcap, state,
-                                                               rows, valid, bc, keys);
+            launch(OB_FAM_ALIGN, al_assoc_kernel<T, true>, nb, kThreads, 0, st, sr, snrm, tr.p, tnrm, g, max_d2,
+                   cos_gate, kcap, state, rows, valid, bc, keys);
         else
-            al_assoc_kernel<T, false><<<nb, kThreads, 0, st>>>(sr, nullptr, tr.p, nullptr, g, max_d2, 0.0, kcap, state,
-                                                                rows, valid, bc, keys);
-        al_compact_kernel<<<nb, kThreads, 0, st>>>(kcap, rows, valid, bc, pairs, state);
+            launch(OB_FAM_ALIGN, al_assoc_kernel<T, false>, nb, kThreads, 0, st, sr, nullptr, tr.p, nullptr, g, max_d2,
+                   0.0, kcap, state, rows, valid, bc, keys);
+        launch(OB_FAM_ALIGN, al_compact_kernel, nb, kThreads, 0, st, kcap, rows, valid, bc, pairs, state);
         e = cub::DeviceRadixSort::SortKeys(tmp, tmp_bytes, keys, skeys, static_cast<int>(kcap), 0, 64, st);
         if (e != cudaSuccess) return fail_cuda(e, "cloud align median");
         if (plane) {
-            al_leaf_kernel<kPlaneSystem><<<lb, 256, 0, st>>>(pairs, skeys, io->max_corr_dist, state, slots, val);
-            al_plane_solve_kernel<<<1, kTreeThreads, 0, st>>>(val, state);
-            launches += 4;
+            launch(OB_FAM_ALIGN, al_leaf_kernel<kPlaneSystem>, lb, 256, 0, st, pairs, skeys, io->max_corr_dist, state,
+                   slots, val);
+            launch(OB_FAM_ALIGN, al_plane_solve_kernel, 1, kTreeThreads, 0, st, val, state);
         } else {
-            al_leaf_kernel<kCentroid><<<lb, 256, 0, st>>>(pairs, skeys, io->max_corr_dist, state, slots, val);
-            al_centroid_kernel<<<1, kTreeThreads, 0, st>>>(val, state);
-            al_leaf_kernel<kCovariance><<<lb, 256, 0, st>>>(pairs, skeys, io->max_corr_dist, state, slots, val);
-            al_p2p_solve_kernel<<<1, kTreeThreads, 0, st>>>(val, state);
-            launches += 6;
+            launch(OB_FAM_ALIGN, al_leaf_kernel<kCentroid>, lb, 256, 0, st, pairs, skeys, io->max_corr_dist, state,
+                   slots, val);
+            launch(OB_FAM_ALIGN, al_centroid_kernel, 1, kTreeThreads, 0, st, val, state);
+            launch(OB_FAM_ALIGN, al_leaf_kernel<kCovariance>, lb, 256, 0, st, pairs, skeys, io->max_corr_dist, state,
+                   slots, val);
+            launch(OB_FAM_ALIGN, al_p2p_solve_kernel, 1, kTreeThreads, 0, st, val, state);
         }
     }
-    al_finish_kernel<<<1, 1, 0, st>>>(state, pose, iters);
-    launches += 1;
-    count_launch(launches);
-    count_launch_of(OB_FAM_ALIGN, launches);
+    launch(OB_FAM_ALIGN, al_finish_kernel, 1, 1, 0, st, state, pose, iters);
     e = cudaGetLastError();
     if (e != cudaSuccess) return fail_cuda(e, "cloud align launch");
     return OB_OK;
@@ -828,19 +823,18 @@ ob_status ob_cloud_nearest(const ob_cloud_nearest_io* io, ob_stream* s) {
     if (io->target_normals) e = stg.in(io->target_normals, tr.cap * 3 * elem_size(io->target.dtype), &nrm);
     if (e == cudaSuccess) e = stg.out(io->indices, qr.cap * 4ull, &out);
     if (e != cudaSuccess) return fail_cuda(e, "stage nearest");
-    uint64_t launches = 1;
     Grid g{};
     if (io->target.dtype == OB_F64) {
-        e = build_grid<double>(tr, nrm, io->cell_size, stg, st, &g, &launches);
+        e = build_grid<double>(tr, nrm, io->cell_size, stg, st, &g);
         if (e == cudaSuccess)
-            al_nearest_kernel<double><<<blocks_for(qr.cap), 256, 0, st>>>(qr, g, io->max_dist_sq, static_cast<int32_t*>(out));
+            launch(OB_FAM_ALIGN, al_nearest_kernel<double>, blocks_for(qr.cap), 256, 0, st, qr, g, io->max_dist_sq,
+                   static_cast<int32_t*>(out));
     } else {
-        e = build_grid<float>(tr, nrm, io->cell_size, stg, st, &g, &launches);
+        e = build_grid<float>(tr, nrm, io->cell_size, stg, st, &g);
         if (e == cudaSuccess)
-            al_nearest_kernel<float><<<blocks_for(qr.cap), 256, 0, st>>>(qr, g, io->max_dist_sq, static_cast<int32_t*>(out));
+            launch(OB_FAM_ALIGN, al_nearest_kernel<float>, blocks_for(qr.cap), 256, 0, st, qr, g, io->max_dist_sq,
+                   static_cast<int32_t*>(out));
     }
-    count_launch(launches);
-    count_launch_of(OB_FAM_ALIGN, launches);
     if (e == cudaSuccess) e = cudaGetLastError();
     if (e == cudaSuccess) e = stg.finish();
     if (e != cudaSuccess) return fail_cuda(e, "cloud nearest");

@@ -14,16 +14,16 @@
 namespace ob {
 
 static thread_local std::string g_last_error;
-static std::atomic<uint64_t> g_launches{0};
 
 static std::atomic<uint64_t> g_family[OB_FAM_COUNT];
 static const char* const kFamilies[OB_FAM_COUNT] = {"decode_pipe", "decode", "cloud", "normals", "voxel",
                                                     "voxel_map", "icp", "align", "zone", "image",
-                                                    "frame_ops", "pose"};
+                                                    "frame_ops", "pose", "dewarp", "destagger", "lut",
+                                                    "encode"};
 
-void count_launch(uint64_t n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
-void count_launch_of(int family, uint64_t n) {
-    if (family >= 0 && family < OB_FAM_COUNT) g_family[family].fetch_add(n, std::memory_order_relaxed);
+void record_launch(int family) {
+    g_family[family].fetch_add(1, std::memory_order_relaxed);
+    if (family == OB_FAM_DECODE_PIPE) g_family[OB_FAM_DECODE].fetch_add(1, std::memory_order_relaxed);
 }
 
 ob_status fail(ob_status st, const std::string& msg) {
@@ -440,7 +440,12 @@ int ob_device_count(void) {
     return n;
 }
 
-uint64_t ob_kernel_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
+uint64_t ob_kernel_launch_count(void) {
+    uint64_t n = 0;
+    for (int i = 0; i < OB_FAM_COUNT; ++i)
+        if (i != OB_FAM_DECODE_PIPE) n += g_family[i].load(std::memory_order_relaxed);
+    return n;
+}
 
 uint64_t ob_kernel_launch_count_of(const char* name) {
     if (!name) return 0;

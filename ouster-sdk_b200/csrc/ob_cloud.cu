@@ -625,8 +625,7 @@ cudaError_t launch_cloud(const CloudArgs<T>& a, int device, cudaStream_t st) {
         const int threads = 256;
         const size_t want = (total + threads - 1) / threads;
         const int blocks = static_cast<int>(std::min<size_t>(want, static_cast<size_t>(tn.sm_count) * 16));
-        cloud_generic_kernel<T><<<std::max(blocks, 1), threads, 0, st>>>(p, a.n_returns);
-        count_launch();
+        launch(OB_FAM_CLOUD, cloud_generic_kernel<T>, std::max(blocks, 1), threads, 0, st, p, a.n_returns);
         return cudaGetLastError();
     }
 
@@ -675,12 +674,12 @@ cudaError_t launch_cloud(const CloudArgs<T>& a, int device, cudaStream_t st) {
         if (a.n_frames > 65535) return cudaErrorInvalidValue;
         e = cudaMallocAsync(reinterpret_cast<void**>(&planes), static_cast<size_t>(a.n_frames) * 12u * a.W * sizeof(T), st);
         if (e != cudaSuccess) return e;
-        pose_planes_kernel<T><<<dim3((a.W + 255) / 256, a.n_frames), 256, 0, st>>>(a.poses, a.poses_fs, planes, a.W, a.n_frames);
-        count_launch();
+        launch(OB_FAM_CLOUD, pose_planes_kernel<T>, dim3((a.W + 255) / 256, a.n_frames), 256, 0, st, a.poses,
+               a.poses_fs, planes, a.W, a.n_frames);
         p.planes = planes;
     }
-    kern<<<std::max(grid, 1), (pose ? tn.cloud_pose_threads : tn.cloud_threads) + 32, smem, st>>>(p);  // + the copy warp
-    count_launch();
+    const int threads = (pose ? tn.cloud_pose_threads : tn.cloud_threads) + 32;  // + the copy warp
+    launch(OB_FAM_CLOUD, kern, std::max(grid, 1), threads, smem, st, p);
     e = cudaGetLastError();
     if (planes != nullptr) {
         const cudaError_t e2 = cudaFreeAsync(planes, st);
@@ -737,8 +736,7 @@ cudaError_t launch_dewarp(const T* pts, const T* poses, T* out, size_t H, size_t
     bands = static_cast<unsigned>((H + rows_per_block - 1) / rows_per_block);
     if (bands > 65535) return cudaErrorInvalidValue;
     dim3 grid(col_blocks, bands);
-    dewarp_kernel<T><<<grid, 256, 0, st>>>(pts, poses, out, H, W, rows_per_block);
-    count_launch();
+    launch(OB_FAM_DEWARP, dewarp_kernel<T>, grid, 256, 0, st, pts, poses, out, H, W, rows_per_block);
     return cudaGetLastError();
 }
 template cudaError_t launch_dewarp<float>(const float*, const float*, float*, size_t, size_t, cudaStream_t);
@@ -828,10 +826,8 @@ cudaError_t launch_destagger(size_t elem_size, size_t k, const void* img, const 
         if (e != cudaSuccess) return e;
         dim3 grid(static_cast<unsigned>(std::min<size_t>((row_bytes + 255) / 256, 64)),
                   static_cast<unsigned>(h));
-        destagger_bytes_dev_kernel<<<grid, 256, 0, st>>>(static_cast<const uint8_t*>(img),
-                                                         static_cast<uint8_t*>(out), row_bytes,
-                                                         static_cast<unsigned>(px_bytes), dsh);
-        count_launch();
+        launch(OB_FAM_DESTAGGER, destagger_bytes_dev_kernel, grid, 256, 0, st, static_cast<const uint8_t*>(img),
+               static_cast<uint8_t*>(out), row_bytes, static_cast<unsigned>(px_bytes), dsh);
         e = cudaGetLastError();
         cudaFreeAsync(dsh, st);
         return e;
@@ -849,13 +845,12 @@ cudaError_t launch_destagger(size_t elem_size, size_t k, const void* img, const 
         const size_t row_words = row_bytes / 4;
         dim3 grid(static_cast<unsigned>(std::min<size_t>((row_words + 255) / 256, 64)),
                   static_cast<unsigned>(h));
-        destagger_words_kernel<<<grid, 256, 0, st>>>(p);
+        launch(OB_FAM_DESTAGGER, destagger_words_kernel, grid, 256, 0, st, p);
     } else {
         dim3 grid(static_cast<unsigned>(std::min<size_t>((row_bytes + 255) / 256, 64)),
                   static_cast<unsigned>(h));
-        destagger_bytes_kernel<<<grid, 256, 0, st>>>(p);
+        launch(OB_FAM_DESTAGGER, destagger_bytes_kernel, grid, 256, 0, st, p);
     }
-    count_launch();
     return cudaGetLastError();
 }
 
@@ -931,8 +926,7 @@ cudaError_t launch_make_lut(size_t w, size_t h, double range_unit, const double*
     p.per_beam = (n_az == h && n_alt == h) ? 1 : 0;
     const size_t n = w * h;
     const int blocks = static_cast<int>(std::min<size_t>((n + 255) / 256, 1184));
-    make_lut_kernel<<<std::max(blocks, 1), 256, 0, st>>>(p, az_dev, alt_dev, dir_dev, off_dev);
-    count_launch();
+    launch(OB_FAM_LUT, make_lut_kernel, std::max(blocks, 1), 256, 0, st, p, az_dev, alt_dev, dir_dev, off_dev);
     return cudaGetLastError();
 }
 
@@ -945,8 +939,7 @@ __global__ void cast_f64_f32_kernel(const double* __restrict__ src, float* __res
 
 cudaError_t launch_cast_f64_f32(const double* src, float* dst, size_t n, cudaStream_t st) {
     const int blocks = static_cast<int>(std::min<size_t>((n + 255) / 256, 1184));
-    cast_f64_f32_kernel<<<std::max(blocks, 1), 256, 0, st>>>(src, dst, n);
-    count_launch();
+    launch(OB_FAM_LUT, cast_f64_f32_kernel, std::max(blocks, 1), 256, 0, st, src, dst, n);
     return cudaGetLastError();
 }
 

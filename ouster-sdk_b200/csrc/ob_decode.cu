@@ -510,9 +510,7 @@ cudaError_t launch_decode(const DecodeLaunch& a, int device, cudaStream_t st) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          static_cast<int>(smem));
     if (e != cudaSuccess) return e;
-    kern<<<std::max(grid, 1), threads, smem, st>>>(p);
-    count_launch();
-    count_launch_of(OB_FAM_DECODE);
+    launch(OB_FAM_DECODE, kern, std::max(grid, 1), threads, smem, st, p);
     return cudaGetLastError();
 }
 

@@ -1126,10 +1126,7 @@ cudaError_t launch_decode_pipe(DecodeParams& p, const DecodeLaunch& a, int devic
                                      : decode_pipe_kernel<float, (kPipeMaxComputeWarps + 3) * 32>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
     if (e != cudaSuccess) return e;
-    kern<<<std::max(grid, 1), threads, smem, st>>>(pp);
-    count_launch();
-    count_launch_of(OB_FAM_DECODE_PIPE);
-    count_launch_of(OB_FAM_DECODE);
+    launch(OB_FAM_DECODE_PIPE, kern, std::max(grid, 1), threads, smem, st, pp);
     return cudaGetLastError();
 }
 

@@ -188,17 +188,16 @@ cudaError_t launch_dewarp_fused(const K3Frame* frames_dev, unsigned n_frames, un
             e = cudaFuncSetAttribute(k3_fused_kernel<double>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
             if (e != cudaSuccess) return e;
         }
-        k3_fused_kernel<double><<<n_blocks, 256, smem, st>>>(frames_dev, n_frames, min_r, max_r, sc,
-                                                               static_cast<double*>(points), frame_idx, col_idx, ts_out, capacity);
+        launch(OB_FAM_DEWARP, k3_fused_kernel<double>, n_blocks, 256, smem, st, frames_dev, n_frames, min_r, max_r, sc,
+               static_cast<double*>(points), frame_idx, col_idx, ts_out, capacity);
     } else {
         if (smem > 48u * 1024u) {
             e = cudaFuncSetAttribute(k3_fused_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
             if (e != cudaSuccess) return e;
         }
-        k3_fused_kernel<float><<<n_blocks, 256, smem, st>>>(frames_dev, n_frames, min_r, max_r, sc,
-                                                              static_cast<float*>(points), frame_idx, col_idx, ts_out, capacity);
+        launch(OB_FAM_DEWARP, k3_fused_kernel<float>, n_blocks, 256, smem, st, frames_dev, n_frames, min_r, max_r, sc,
+               static_cast<float*>(points), frame_idx, col_idx, ts_out, capacity);
     }
-    count_launch();
     return cudaGetLastError();
 }
 

@@ -285,8 +285,7 @@ cudaError_t launch_encode(const DecodeLayout& L, const EncodeFrame* frames_dev, 
     if (smem > 227 * 1024) return cudaErrorInvalidValue;
     cudaError_t e = cudaFuncSetAttribute(encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
     if (e != cudaSuccess) return e;
-    encode_kernel<<<n_frames * p.n_packets_per_frame, kEncThreads, smem, st>>>(p);
-    count_launch();
+    launch(OB_FAM_ENCODE, encode_kernel, n_frames * p.n_packets_per_frame, kEncThreads, smem, st, p);
     return cudaGetLastError();
 }
 

@@ -352,7 +352,7 @@ cudaError_t launch_mask(MaskParams<CAP>& p, const std::vector<MaskEntry>& ents, 
     std::copy(ents.begin() + e0, ents.begin() + fbeg[f1], p.e);
     const size_t runs = (size_t(p.npx) + kRun - 1) / kRun;
     dim3 grid(unsigned((runs + kThreads - 1) / kThreads), f1 - f0);
-    frame_mask_kernel<CAP><<<grid, kThreads, 0, st>>>(p);
+    launch(OB_FAM_FRAME_OPS, frame_mask_kernel<CAP>, grid, kThreads, 0, st, p);
     return cudaGetLastError();
 }
 
@@ -361,7 +361,7 @@ cudaError_t launch_rows(RowParams<CAP>& p, const RowEntry* ents, uint32_t n, cud
     p.n_entries = n;
     std::copy(ents, ents + n, p.e);
     const unsigned gx = unsigned(std::min<size_t>((size_t(max_units) + kThreads - 1) / kThreads, 4096));
-    frame_rows_kernel<CAP><<<dim3(std::max(gx, 1u), n), kThreads, 0, st>>>(p);
+    launch(OB_FAM_FRAME_OPS, frame_rows_kernel<CAP>, dim3(std::max(gx, 1u), n), kThreads, 0, st, p);
     return cudaGetLastError();
 }
 
@@ -491,13 +491,11 @@ ob_status ob_frame_mask_fields(const ob_frame_ops_io* io, ob_stream* s) {
         p.poses = dposes;
         for (size_t r = 0; r < sh.size(); ++r) p.shift[r] = sh[r];
     };
-    uint64_t launches = 0;
     constexpr int kSmall = 32, kLarge = 512;
     if (ents.size() <= size_t(kSmall) && a.n_frames <= uint32_t(kSmall)) {
         auto p = std::make_unique<MaskParams<kSmall>>();
         fill(*p);
         e = launch_mask(*p, ents, fbeg, 0, a.n_frames, st);
-        ++launches;
     } else {
         auto p = std::make_unique<MaskParams<kLarge>>();
         fill(*p);
@@ -506,12 +504,9 @@ ob_status ob_frame_mask_fields(const ob_frame_ops_io* io, ob_stream* s) {
             uint32_t f1 = f0 + 1;
             while (f1 < a.n_frames && f1 - f0 < uint32_t(kLarge) && fbeg[f1 + 1] - fbeg[f0] <= uint32_t(kLarge)) ++f1;
             e = launch_mask(*p, ents, fbeg, f0, f1, st);
-            ++launches;
             f0 = f1;
         }
     }
-    count_launch(launches);
-    count_launch_of(OB_FAM_FRAME_OPS, launches);
     if (e == cudaSuccess) e = stg.flush();
     if (e == cudaSuccess && host_io) e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail_cuda(e, "frame mask");
@@ -558,7 +553,6 @@ ob_status ob_frame_select_rows(const ob_frame_rows_io* io, ob_stream* s) {
         ents.push_back(x);
     }
     if (e != cudaSuccess) return fail_cuda(e, "stage frame rows");
-    uint64_t launches = 0;
     constexpr int kCap = 768;   // 18 KB of entries + 8 KB of rows: within the 32 KB parameter limit
     auto p = std::make_unique<RowParams<kCap>>();
     p->n_rows = a.n_rows;
@@ -566,10 +560,7 @@ ob_status ob_frame_select_rows(const ob_frame_rows_io* io, ob_stream* s) {
     for (size_t b = 0; b < ents.size() && e == cudaSuccess; b += kCap) {
         const uint32_t n = uint32_t(std::min<size_t>(kCap, ents.size() - b));
         e = launch_rows(*p, ents.data() + b, n, st, max_units);
-        ++launches;
     }
-    count_launch(launches);
-    count_launch_of(OB_FAM_FRAME_OPS, launches);
     if (e == cudaSuccess) e = stg.flush();
     if (e == cudaSuccess && host_io) e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail_cuda(e, "frame select rows");

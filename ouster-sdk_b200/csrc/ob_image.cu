@@ -572,44 +572,38 @@ cudaError_t grow(void** buf, size_t* have, size_t need) {
 }
 
 template <typename T, int L>
-void launch_ae(ob_image_proc* p, const void* in, T* out, uint32_t npx, int update_state, cudaStream_t st,
-               uint64_t* launches) {
-    ae_select_kernel<T, L><<<1, kSelectThreads, 0, st>>>(in, npx, p->st, p->p, update_state, 0);
+void launch_ae(ob_image_proc* p, const void* in, T* out, uint32_t npx, int update_state, cudaStream_t st) {
+    launch(OB_FAM_IMAGE, ae_select_kernel<T, L>, 1, kSelectThreads, 0, st, in, npx, p->st, p->p, update_state, 0);
     const size_t n = size_t(npx) * (L == 0 ? 1 : 3);
-    ae_apply_kernel<T, L><<<ew_blocks(n), kEwThreads, 0, st>>>(in, out, n, p->st);
-    *launches += 2;
+    launch(OB_FAM_IMAGE, ae_apply_kernel<T, L>, ew_blocks(n), kEwThreads, 0, st, in, out, n, p->st);
 }
 
 template <typename T, int L>
 void launch_ltm(ob_image_proc* p, const void* in, T* out, uint32_t rows, uint32_t cols, int update_state,
-                cudaStream_t st, uint64_t* launches) {
+                cudaStream_t st) {
     const uint32_t npx = rows * cols;
     T* lum = static_cast<T*>(p->scratch);
     float* luts = reinterpret_cast<float*>(static_cast<char*>(p->scratch) + ((size_t(npx) * sizeof(T) + 255) & ~size_t(255)));
-    ae_select_kernel<T, L><<<1, kSelectThreads, 0, st>>>(in, npx, p->st, p->p, update_state, 1);
-    ltm_pixel_kernel<T, L><<<ew_blocks(npx), kEwThreads, 0, st>>>(in, out, lum, npx, p->st);
-    clahe_lut_kernel<T><<<kTiles * kTiles, 1024, 0, st>>>(lum, int(rows), int(cols), luts, p->st);
-    ltm_apply_kernel<T><<<ew_blocks(npx), kEwThreads, 0, st>>>(out, lum, int(rows), int(cols), luts, p->st,
-                                                              p->p.color_correct);
-    *launches += 4;
+    launch(OB_FAM_IMAGE, ae_select_kernel<T, L>, 1, kSelectThreads, 0, st, in, npx, p->st, p->p, update_state, 1);
+    launch(OB_FAM_IMAGE, ltm_pixel_kernel<T, L>, ew_blocks(npx), kEwThreads, 0, st, in, out, lum, npx, p->st);
+    launch(OB_FAM_IMAGE, clahe_lut_kernel<T>, kTiles * kTiles, 1024, 0, st, lum, int(rows), int(cols), luts, p->st);
+    launch(OB_FAM_IMAGE, ltm_apply_kernel<T>, ew_blocks(npx), kEwThreads, 0, st, out, lum, int(rows), int(cols), luts,
+           p->st, p->p.color_correct);
 }
 
 template <typename T>
-void launch_buc(ob_image_proc* p, T* img, uint32_t rows, uint32_t cols, int update_state, cudaStream_t st,
-                uint64_t* launches) {
+void launch_buc(ob_image_proc* p, T* img, uint32_t rows, uint32_t cols, int update_state, cudaStream_t st) {
     uint8_t* mask = static_cast<uint8_t*>(p->scratch);
     T* dc = reinterpret_cast<T*>(static_cast<char*>(p->scratch) + ((size_t(cols) + 255) & ~size_t(255)));
     T* lu = dc + rows;
-    buc_mask_kernel<T><<<ew_blocks(cols), kEwThreads, 0, st>>>(img, rows, cols, mask, p->st, update_state);
-    *launches += 1;
-    if (rows > 1) {
-        buc_median_kernel<T><<<rows - 1, kMedianThreads, 0, st>>>(img, rows, cols, mask, dc, p->st, update_state);
-        *launches += 1;
-    }
-    buc_tail_kernel<T><<<1, 1, 0, st>>>(rows, cols, mask, dc, lu, p->dark, p->st, update_state);
+    launch(OB_FAM_IMAGE, buc_mask_kernel<T>, ew_blocks(cols), kEwThreads, 0, st, img, rows, cols, mask, p->st,
+           update_state);
+    if (rows > 1)
+        launch(OB_FAM_IMAGE, buc_median_kernel<T>, rows - 1, kMedianThreads, 0, st, img, rows, cols, mask, dc, p->st,
+               update_state);
+    launch(OB_FAM_IMAGE, buc_tail_kernel<T>, 1, 1, 0, st, rows, cols, mask, dc, lu, p->dark, p->st, update_state);
     const size_t n = size_t(rows) * cols;
-    buc_apply_kernel<T><<<ew_blocks(n), kEwThreads, 0, st>>>(img, cols, n, p->dark);
-    *launches += 2;
+    launch(OB_FAM_IMAGE, buc_apply_kernel<T>, ew_blocks(n), kEwThreads, 0, st, img, cols, n, p->dark);
 }
 
 }  // namespace
@@ -695,24 +689,21 @@ ob_status ob_image_proc_update(ob_image_proc* p, int layout, int dtype, const vo
     }
     if (e != cudaSuccess) return fail_cuda(e, "stage image");
     const uint32_t np = uint32_t(npx);
-    uint64_t launches = 0;
     const int us = update_state ? 1 : 0;
     if (p->kind == OB_IMAGE_AUTO_EXPOSURE) {
-        if (f16) launch_ae<float, 2>(p, din, static_cast<float*>(dout), np, us, st, &launches);
-        else if (layout == OB_IMAGE_MONO && dtype == OB_F32) launch_ae<float, 0>(p, din, static_cast<float*>(dout), np, us, st, &launches);
-        else if (layout == OB_IMAGE_MONO) launch_ae<double, 0>(p, din, static_cast<double*>(dout), np, us, st, &launches);
-        else if (dtype == OB_F32) launch_ae<float, 1>(p, din, static_cast<float*>(dout), np, us, st, &launches);
-        else launch_ae<double, 1>(p, din, static_cast<double*>(dout), np, us, st, &launches);
+        if (f16) launch_ae<float, 2>(p, din, static_cast<float*>(dout), np, us, st);
+        else if (layout == OB_IMAGE_MONO && dtype == OB_F32) launch_ae<float, 0>(p, din, static_cast<float*>(dout), np, us, st);
+        else if (layout == OB_IMAGE_MONO) launch_ae<double, 0>(p, din, static_cast<double*>(dout), np, us, st);
+        else if (dtype == OB_F32) launch_ae<float, 1>(p, din, static_cast<float*>(dout), np, us, st);
+        else launch_ae<double, 1>(p, din, static_cast<double*>(dout), np, us, st);
     } else if (p->kind == OB_IMAGE_LOCAL_TONE_MAP) {
-        if (f16) launch_ltm<float, 2>(p, din, static_cast<float*>(dout), rows, cols, us, st, &launches);
-        else if (dtype == OB_F32) launch_ltm<float, 1>(p, din, static_cast<float*>(dout), rows, cols, us, st, &launches);
-        else launch_ltm<double, 1>(p, din, static_cast<double*>(dout), rows, cols, us, st, &launches);
+        if (f16) launch_ltm<float, 2>(p, din, static_cast<float*>(dout), rows, cols, us, st);
+        else if (dtype == OB_F32) launch_ltm<float, 1>(p, din, static_cast<float*>(dout), rows, cols, us, st);
+        else launch_ltm<double, 1>(p, din, static_cast<double*>(dout), rows, cols, us, st);
     } else {
-        if (dtype == OB_F32) launch_buc<float>(p, static_cast<float*>(dout), rows, cols, us, st, &launches);
-        else launch_buc<double>(p, static_cast<double*>(dout), rows, cols, us, st, &launches);
+        if (dtype == OB_F32) launch_buc<float>(p, static_cast<float*>(dout), rows, cols, us, st);
+        else launch_buc<double>(p, static_cast<double*>(dout), rows, cols, us, st);
     }
-    count_launch(launches);
-    count_launch_of(OB_FAM_IMAGE, launches);
     e = cudaGetLastError();
     if (e == cudaSuccess) e = stg.flush();
     if (e == cudaSuccess && (!is_device_ptr(out) || (f16 && !is_device_ptr(in)))) e = cudaStreamSynchronize(st);

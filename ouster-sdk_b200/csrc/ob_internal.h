@@ -5,6 +5,7 @@
 #include <cstddef>
 #include <cstdint>
 #include <string>
+#include <utility>
 
 #include "../../include/ouster_b200.h"
 
@@ -187,10 +188,21 @@ bool decode_pipe_eligible(const DecodeParams& p, const DecodeLaunch& a, int devi
 cudaError_t launch_decode_pipe(DecodeParams& p, const DecodeLaunch& a, int device, cudaStream_t st);
 cudaError_t make_decode_params(const DecodeLaunch& a, int device, bool pipe, DecodeParams& p);
 
-void count_launch(uint64_t n = 1);
+// Kernel families of ob_kernel_launch_count_of; the names are in ob_api.cu.  DECODE_PIPE is a sub-family of
+// DECODE: a launch counted as DECODE_PIPE also counts as DECODE, and ob_kernel_launch_count leaves it out.
 enum { OB_FAM_DECODE_PIPE = 0, OB_FAM_DECODE = 1, OB_FAM_CLOUD = 2, OB_FAM_NORMALS = 3, OB_FAM_VOXEL = 4,
        OB_FAM_VOXEL_MAP = 5, OB_FAM_ICP = 6, OB_FAM_ALIGN = 7, OB_FAM_ZONE = 8, OB_FAM_IMAGE = 9,
-       OB_FAM_FRAME_OPS = 10, OB_FAM_POSE = 11, OB_FAM_COUNT = 12 };
-void count_launch_of(int family, uint64_t n = 1);
+       OB_FAM_FRAME_OPS = 10, OB_FAM_POSE = 11, OB_FAM_DEWARP = 12, OB_FAM_DESTAGGER = 13, OB_FAM_LUT = 14,
+       OB_FAM_ENCODE = 15, OB_FAM_COUNT = 16 };
+void record_launch(int family);
+
+// Every kernel of the library is launched through here, so the launch counters cannot drift from the launches.
+// Errors are left to the caller's cudaGetLastError().  The kernels CUB launches inside DeviceRadixSort and
+// DeviceScan do not come through here and are not counted.
+template <typename... P, typename... A>
+void launch(int family, void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, A&&... args) {
+    kernel<<<grid, block, smem, st>>>(std::forward<A>(args)...);
+    record_launch(family);
+}
 
 }  // namespace ob

@@ -212,10 +212,8 @@ extern "C" ob_status ob_frames_to_map_rows(const ob_map_rows_item* items, size_t
     lb.agg = reinterpret_cast<unsigned long long*>(b + state_bytes(nb));
     lb.incl = lb.agg + nb;
     unsigned long long* item_end = lb.incl + nb;
-    map_rows_kernel<<<nb, kMrThreads, 0, st>>>(static_cast<const MrItem*>(tab), ni, static_cast<unsigned>(cols),
-                                               reinterpret_cast<unsigned*>(b), lb, item_end, dout, capacity);
-    count_launch();
-    count_launch_of(OB_FAM_VOXEL_MAP);
+    launch(OB_FAM_VOXEL_MAP, map_rows_kernel, nb, kMrThreads, 0, st, static_cast<const MrItem*>(tab), ni,
+           static_cast<unsigned>(cols), reinterpret_cast<unsigned*>(b), lb, item_end, dout, capacity);
     e = cudaGetLastError();
     if (e != cudaSuccess) return fail_cuda(e, "map rows launch");
     return res.finish(item_end + (ni - 1));

@@ -390,16 +390,14 @@ extern "C" ob_status ob_normals(ob_dtype dtype, const ob_normals_io* io, ob_stre
     if (grid.y > 65535) return fail(OB_INVALID_ARGUMENT, "frame too tall");
     const unsigned sub_threads = dual ? 64 : 32;  // one warp per return
     if (dtype == OB_F64) {
-        normals_subtent_kernel<double><<<static_cast<unsigned>(F), sub_threads, 0, st>>>(p);
-        normals_kernel<double><<<grid, 256, 0, st>>>(p, 0);
-        if (dual) normals_kernel<double><<<grid, 256, 0, st>>>(p, 1);
+        launch(OB_FAM_NORMALS, normals_subtent_kernel<double>, static_cast<unsigned>(F), sub_threads, 0, st, p);
+        launch(OB_FAM_NORMALS, normals_kernel<double>, grid, 256, 0, st, p, 0);
+        if (dual) launch(OB_FAM_NORMALS, normals_kernel<double>, grid, 256, 0, st, p, 1);
     } else {
-        normals_subtent_kernel<float><<<static_cast<unsigned>(F), sub_threads, 0, st>>>(p);
-        normals_kernel<float><<<grid, 256, 0, st>>>(p, 0);
-        if (dual) normals_kernel<float><<<grid, 256, 0, st>>>(p, 1);
+        launch(OB_FAM_NORMALS, normals_subtent_kernel<float>, static_cast<unsigned>(F), sub_threads, 0, st, p);
+        launch(OB_FAM_NORMALS, normals_kernel<float>, grid, 256, 0, st, p, 0);
+        if (dual) launch(OB_FAM_NORMALS, normals_kernel<float>, grid, 256, 0, st, p, 1);
     }
-    count_launch(dual ? 3 : 2);
-    count_launch_of(OB_FAM_NORMALS, dual ? 3 : 2);
     e = cudaGetLastError();
     if (e != cudaSuccess) return fail_cuda(e, "normals launch");
     e = stg.flush();

@@ -429,30 +429,23 @@ cudaError_t launch_interp(const ob_interp_pose_io* io, const void* x, const void
                           void* out, ScanFlags* fl, size_t* ends, Seg* segs, long long* err, long long* vals,
                           int device, cudaStream_t st) {
     const size_t n = io->n, m = io->m, S = io->two_pose ? 1 : m - 1;
-    uint64_t launches = 0;
     cudaError_t e = cudaMemsetAsync(fl, 0xff, 8, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(&fl->nan, 0, 8, st);
     if (e != cudaSuccess) return e;
     if (n > 0) {
         const unsigned blocks = static_cast<unsigned>(std::min<size_t>((n + 255) / 256, tunables(device).sm_count * 8ull));
         if constexpr (sizeof(T) == 8 && std::is_same<T, double>::value)
-            scan_kernel_f64<<<blocks, 256, 0, st>>>(static_cast<const double*>(x), n, fl);
+            launch(OB_FAM_POSE, scan_kernel_f64, blocks, 256, 0, st, static_cast<const double*>(x), n, fl);
         else
-            scan_kernel_i64<<<blocks, 256, 0, st>>>(static_cast<const long long*>(x), n, fl);
-        ++launches;
+            launch(OB_FAM_POSE, scan_kernel_i64, blocks, 256, 0, st, static_cast<const long long*>(x), n, fl);
     }
-    plan_kernel<T, P><<<1, kPlanThreads, 0, st>>>(static_cast<const T*>(x), n, static_cast<const T*>(knots), m,
-                                                  static_cast<const P*>(poses_known), io->two_pose, fl, ends, segs, err,
-                                                  vals);
-    ++launches;
-    if (n > 0) {
-        interp_kernel<T, P><<<static_cast<unsigned>((n + kQThreads - 1) / kQThreads), kQThreads, 0, st>>>(
-            static_cast<const T*>(x), n, ends, S, segs, err, static_cast<P*>(out),
-            (reinterpret_cast<uintptr_t>(out) & 15u) == 0);
-        ++launches;
-    }
-    count_launch(launches);
-    count_launch_of(OB_FAM_POSE, launches);
+    launch(OB_FAM_POSE, plan_kernel<T, P>, 1, kPlanThreads, 0, st, static_cast<const T*>(x), n,
+           static_cast<const T*>(knots), m, static_cast<const P*>(poses_known), io->two_pose, fl, ends, segs, err,
+           vals);
+    if (n > 0)
+        launch(OB_FAM_POSE, interp_kernel<T, P>, static_cast<unsigned>((n + kQThreads - 1) / kQThreads), kQThreads, 0,
+               st, static_cast<const T*>(x), n, ends, S, segs, err, static_cast<P*>(out),
+               (reinterpret_cast<uintptr_t>(out) & 15u) == 0);
     return cudaGetLastError();
 }
 
@@ -589,16 +582,11 @@ extern "C" ob_status ob_frames_interp_pose(const ob_frame_poses_item* frames, si
     if (e == cudaSuccess && !items.empty()) {
         if (x1) e = cudaMemsetAsync(&fs->fail_item, 0xff, 8, st);
         if (e != cudaSuccess) return fail_cuda(e, "stage frames_interp_pose");
-        uint64_t launches = 1;
-        if (x1) {
-            frame_check_kernel<<<static_cast<unsigned>(items.size()), kCheckThreads, 0, st>>>(
-                ditems, fs, desc, t0, static_cast<const double*>(dx0), t1, static_cast<const double*>(dx1));
-            ++launches;
-        }
-        frame_write_kernel<<<nb, kWriteThreads, 0, st>>>(ditems, static_cast<unsigned>(items.size()), x1 ? fs : nullptr,
-                                                         desc, static_cast<const double*>(dx0), err, vals);
-        count_launch(launches);
-        count_launch_of(OB_FAM_POSE, launches);
+        if (x1)
+            launch(OB_FAM_POSE, frame_check_kernel, static_cast<unsigned>(items.size()), kCheckThreads, 0, st, ditems,
+                   fs, desc, t0, static_cast<const double*>(dx0), t1, static_cast<const double*>(dx1));
+        launch(OB_FAM_POSE, frame_write_kernel, nb, kWriteThreads, 0, st, ditems, static_cast<unsigned>(items.size()),
+               x1 ? fs : nullptr, desc, static_cast<const double*>(dx0), err, vals);
         e = cudaGetLastError();
     }
     if (e != cudaSuccess) return fail_cuda(e, "frames_interp_pose launch");

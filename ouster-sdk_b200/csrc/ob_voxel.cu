@@ -442,7 +442,6 @@ cudaError_t run_voxel(VoxelParams p, Staging& stg, cudaStream_t st, double* out,
         return e;
     };
     cudaError_t e = cudaSuccess;
-    uint64_t launches = 0;
     size_t tmp_bytes = 0, need = 0;
     void* tmp = nullptr;
     // CUB temporary storage: one block sized for the largest of the calls below
@@ -476,14 +475,13 @@ cudaError_t run_voxel(VoxelParams p, Staging& stg, cudaStream_t st, double* out,
         if (e == cudaSuccess) e = alloc(cap * 4ull, &last_of);
         if (e == cudaSuccess) e = cudaMemsetAsync(last_of, 0xff, cap * 4ull, st);
         if (e != cudaSuccess) return e;
-        vx_shuffle_draw_kernel<<<nb, 256, 0, st>>>(p, jkey, step);
+        launch(OB_FAM_VOXEL, vx_shuffle_draw_kernel, nb, 256, 0, st, p, jkey, step);
         int bits = 1;
         while (bits < 32 && (1ull << bits) <= cap) ++bits;
         e = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, jkey, sj, step, ss, static_cast<int>(cap), 0, bits, st);
         if (e != cudaSuccess) return e;
-        vx_shuffle_index_kernel<<<nb, 256, 0, st>>>(cap, sj, ss, where, last_of);
-        vx_shuffle_perm_kernel<<<nb, 256, 0, st>>>(p, sj, ss, where, last_of, order);
-        launches += 3;
+        launch(OB_FAM_VOXEL, vx_shuffle_index_kernel, nb, 256, 0, st, cap, sj, ss, where, last_of);
+        launch(OB_FAM_VOXEL, vx_shuffle_perm_kernel, nb, 256, 0, st, p, sj, ss, where, last_of, order);
         p.order = order;
     }
     VKey *keys, *sk;
@@ -516,34 +514,27 @@ cudaError_t run_voxel(VoxelParams p, Staging& stg, cudaStream_t st, double* out,
     w.seg_start = seg_start;
     w.cnt = cnt;
     w.draw = draw;
-    vx_key_kernel<T><<<nb, 256, 0, st>>>(p, keys, seq);
+    launch(OB_FAM_VOXEL, vx_key_kernel<T>, nb, 256, 0, st, p, keys, seq);
     e = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, sk, seq, sseq, static_cast<int>(cap), VKeyDecomposer{}, 0,
                                         kKeyBits, st);
     if (e != cudaSuccess) return e;
-    vx_head_kernel<<<nb, 256, 0, st>>>(cap, sk, sseq, opens);
+    launch(OB_FAM_VOXEL, vx_head_kernel, nb, 256, 0, st, cap, sk, sseq, opens);
     e = cub::DeviceScan::InclusiveSum(tmp, tmp_bytes, opens, vrank, static_cast<int>(cap), st);
     if (e != cudaSuccess) return e;
-    vx_seg_kernel<<<nb, 256, 0, st>>>(cap, sk, sseq, vrank, seg_start);
-    launches += 3;
+    launch(OB_FAM_VOXEL, vx_seg_kernel, nb, 256, 0, st, cap, sk, sseq, vrank, seg_start);
     if (sums) {
-        vx_reduce_sum_kernel<T><<<nb, 256, 0, st>>>(p, w);
-        launches += 1;
+        launch(OB_FAM_VOXEL, vx_reduce_sum_kernel<T>, nb, 256, 0, st, p, w);
     } else if (p.mode == OB_VOXEL_RANDOM) {
-        vx_random_flags_kernel<<<nb, 256, 0, st>>>(p, w);
+        launch(OB_FAM_VOXEL, vx_random_flags_kernel, nb, 256, 0, st, p, w);
         e = cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, w.full, draw, static_cast<int>(cap), st);
         if (e != cudaSuccess) return e;
-        vx_random_pick_kernel<<<nb, 256, 0, st>>>(p, w);
-        launches += 2;
+        launch(OB_FAM_VOXEL, vx_random_pick_kernel, nb, 256, 0, st, p, w);
     } else {
-        vx_reduce_first_kernel<T><<<nb, 256, 0, st>>>(p, w);
-        launches += 1;
+        launch(OB_FAM_VOXEL, vx_reduce_first_kernel<T>, nb, 256, 0, st, p, w);
     }
     e = cub::DeviceScan::InclusiveSum(tmp, tmp_bytes, cnt, coff, static_cast<int>(cap), st);
     if (e != cudaSuccess) return e;
-    vx_emit_kernel<T><<<nb, 256, 0, st>>>(p, w, coff, out, out_n, out_idx, n_out_dev);
-    launches += 1;
-    count_launch(launches);
-    count_launch_of(OB_FAM_VOXEL, launches);
+    launch(OB_FAM_VOXEL, vx_emit_kernel<T>, nb, 256, 0, st, p, w, coff, out, out_n, out_idx, n_out_dev);
     return cudaGetLastError();
 }
 

@@ -776,9 +776,7 @@ ob_status reserve(ob_voxel_map* m, size_t rows, const uint32_t* nv_dev, cudaStre
     e = alloc_table(&nt, static_cast<unsigned>(cap), st);
     if (e != cudaSuccess) return fail_cuda(e, "voxel map allocation");
     if (m->cap) {
-        vm_rehash_kernel<<<blocks_for(m->cap), 256, 0, st>>>(table_of(m), table_of(&nt));
-        count_launch();
-        count_launch_of(OB_FAM_VOXEL_MAP);
+        launch(OB_FAM_VOXEL_MAP, vm_rehash_kernel, blocks_for(m->cap), 256, 0, st, table_of(m), table_of(&nt));
         e = cudaGetLastError();
     }
     const unsigned long long occ = live;
@@ -829,27 +827,23 @@ cudaError_t sort_batch(const ob_voxel_map* m, Rows r, unsigned cols, Staging& st
     void* tmp = nullptr;
     if (e == cudaSuccess) e = stg.scratch(tmp_bytes, &tmp);
     if (e != cudaSuccess) return e;
-    vm_key_kernel<T><<<nb, 256, 0, st>>>(r, cols, m->inv, keys, seq);
+    launch(OB_FAM_VOXEL_MAP, vm_key_kernel<T>, nb, 256, 0, st, r, cols, m->inv, keys, seq);
     e = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, b->sk, seq, b->sseq, static_cast<int>(cap),
                                         VKeyDecomposer{}, 0, kKeyBits, st);
     if (e != cudaSuccess) return e;
-    vx_head_kernel<<<nb, 256, 0, st>>>(cap, b->sk, b->sseq, opens);
+    launch(OB_FAM_VOXEL_MAP, vx_head_kernel, nb, 256, 0, st, cap, b->sk, b->sseq, opens);
     e = cub::DeviceScan::InclusiveSum(tmp, tmp_bytes, opens, b->vrank, static_cast<int>(cap), st);
     if (e != cudaSuccess) return e;
-    vx_seg_kernel<<<nb, 256, 0, st>>>(cap, b->sk, b->sseq, b->vrank, b->seg_start);
-    count_launch(3);
-    count_launch_of(OB_FAM_VOXEL_MAP, 3);
+    launch(OB_FAM_VOXEL_MAP, vx_seg_kernel, nb, 256, 0, st, cap, b->sk, b->sseq, b->vrank, b->seg_start);
     return cudaGetLastError();
 }
 
 // the second half: every distinct voxel of the batch into the table
 template <typename T>
 cudaError_t insert_batch(ob_voxel_map* m, Rows r, unsigned cols, const AddBatch& b, cudaStream_t st) {
-    vm_insert_kernel<T><<<blocks_for(r.cap), 256, 0, st>>>(r, cols, table_of(m), m->ctr, b.sk, b.sseq, b.vrank,
-                                                            b.seg_start, m->res_sq);
-    vm_advance_stamp_kernel<<<1, 1, 0, st>>>(r.cap, b.vrank, m->ctr);
-    count_launch(2);
-    count_launch_of(OB_FAM_VOXEL_MAP, 2);
+    launch(OB_FAM_VOXEL_MAP, vm_insert_kernel<T>, blocks_for(r.cap), 256, 0, st, r, cols, table_of(m), m->ctr, b.sk,
+           b.sseq, b.vrank, b.seg_start, m->res_sq);
+    launch(OB_FAM_VOXEL_MAP, vm_advance_stamp_kernel, 1, 1, 0, st, r.cap, b.vrank, m->ctr);
     return cudaGetLastError();
 }
 
@@ -878,15 +872,13 @@ cudaError_t run_emit(const ob_voxel_map* m, const uint32_t* sel, Staging& stg, c
     if (e != cudaSuccess) return e;
     const Table t = table_of(m);
     const unsigned nb = blocks_for(cap);
-    vm_emit_keys_kernel<<<nb, 256, 0, st>>>(t, sel, keys, slots);
+    launch(OB_FAM_VOXEL_MAP, vm_emit_keys_kernel, nb, 256, 0, st, t, sel, keys, slots);
     e = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, skeys, slots, sslots, static_cast<int>(cap), 0, 64, st);
     if (e != cudaSuccess) return e;
-    vm_emit_counts_kernel<<<nb, 256, 0, st>>>(t, skeys, sslots, c);
+    launch(OB_FAM_VOXEL_MAP, vm_emit_counts_kernel, nb, 256, 0, st, t, skeys, sslots, c);
     e = cub::DeviceScan::InclusiveSum(tmp, tmp_bytes, c, off, static_cast<int>(cap), st);
     if (e != cudaSuccess) return e;
-    vm_emit_kernel<<<nb, 256, 0, st>>>(t, skeys, sslots, off, out, capacity, n_dev);
-    count_launch(3);
-    count_launch_of(OB_FAM_VOXEL_MAP, 3);
+    launch(OB_FAM_VOXEL_MAP, vm_emit_kernel, nb, 256, 0, st, t, skeys, sslots, off, out, capacity, n_dev);
     return cudaGetLastError();
 }
 
@@ -1052,10 +1044,8 @@ ob_status ob_voxel_map_remove_far(ob_voxel_map* m, const ob_voxel_map_cull_io* i
         e = scratch(stg, m->cap * 4ull, &removed);
         if (e != cudaSuccess) return fail_cuda(e, "voxel map cull");
     }
-    vm_cull_kernel<<<blocks_for(m->cap), 256, 0, st>>>(table_of(m), m->ctr, static_cast<const double*>(org), m->inv,
-                                                        cull_threshold(m->max_distance, m->inv), removed);
-    count_launch();
-    count_launch_of(OB_FAM_VOXEL_MAP);
+    launch(OB_FAM_VOXEL_MAP, vm_cull_kernel, blocks_for(m->cap), 256, 0, st, table_of(m), m->ctr,
+           static_cast<const double*>(org), m->inv, cull_threshold(m->max_distance, m->inv), removed);
     e = cudaGetLastError();
     if (e != cudaSuccess) return fail_cuda(e, "voxel map cull");
     if (!extract) return OB_OK;
@@ -1109,10 +1099,8 @@ ob_status ob_voxel_map_closest_neighbors(const ob_voxel_map* m, const ob_voxel_q
     const bool f64 = io->queries.dtype == OB_F64, attr = m->na != 0;
     auto kern = f64 ? (attr ? vm_closest_kernel<double, true> : vm_closest_kernel<double, false>)
                     : (attr ? vm_closest_kernel<float, true> : vm_closest_kernel<float, false>);
-    kern<<<blocks_for(r.cap), 256, 0, st>>>(r, t, m->inv, m->voxel_size, io->max_distance_sq, static_cast<double*>(nb),
-                                            static_cast<double*>(d2));
-    count_launch();
-    count_launch_of(OB_FAM_VOXEL_MAP);
+    launch(OB_FAM_VOXEL_MAP, kern, blocks_for(r.cap), 256, 0, st, r, t, m->inv, m->voxel_size, io->max_distance_sq,
+           static_cast<double*>(nb), static_cast<double*>(d2));
     e = cudaGetLastError();
     if (e == cudaSuccess) e = stg.flush();
     if (e != cudaSuccess) return fail_cuda(e, "voxel map closest neighbors");
@@ -1143,11 +1131,10 @@ ob_status ob_icp_linear_system(const ob_icp_system_io* io, ob_stream* s) {
     double* val = nullptr;
     if (e == cudaSuccess) e = scratch(stg, slots * kSys * 8ull, &val);
     if (e != cudaSuccess) return fail_cuda(e, "stage linear system");
-    icp_leaf_kernel<<<blocks_for(slots), 256, 0, st>>>(static_cast<const double*>(src), static_cast<const double*>(tgt), n,
-                                                        cap, io->kernel_scale, nullptr, slots, val);
-    icp_system_kernel<<<1, kTreeThreads, 0, st>>>(n, cap, val, static_cast<double*>(jtj), static_cast<double*>(jtr));
-    count_launch(2);
-    count_launch_of(OB_FAM_ICP, 2);
+    launch(OB_FAM_ICP, icp_leaf_kernel, blocks_for(slots), 256, 0, st, static_cast<const double*>(src),
+           static_cast<const double*>(tgt), n, cap, io->kernel_scale, nullptr, slots, val);
+    launch(OB_FAM_ICP, icp_system_kernel, 1, kTreeThreads, 0, st, n, cap, val, static_cast<double*>(jtj),
+           static_cast<double*>(jtr));
     e = cudaGetLastError();
     if (e == cudaSuccess) e = stg.finish();
     if (e != cudaSuccess) return fail_cuda(e, "icp linear system");
@@ -1184,20 +1171,19 @@ ob_status ob_icp_align(const ob_voxel_map* m, const ob_icp_io* io, ob_stream* s)
     const Table t = table_of(m);
     const double md2 = io->max_distance * io->max_distance;  // square(max_correspondance_distance)
     const double crit_sq = io->convergence_criterion * io->convergence_criterion;
-    if (io->source.dtype == OB_F64) icp_init_kernel<double><<<nb, kAssocThreads, 0, st>>>(r, m->ctr, src, state);
-    else icp_init_kernel<float><<<nb, kAssocThreads, 0, st>>>(r, m->ctr, src, state);
-    uint64_t launches = 2;
+    if (io->source.dtype == OB_F64)
+        launch(OB_FAM_ICP, icp_init_kernel<double>, nb, kAssocThreads, 0, st, r, m->ctr, src, state);
+    else
+        launch(OB_FAM_ICP, icp_init_kernel<float>, nb, kAssocThreads, 0, st, r, m->ctr, src, state);
     for (int it = 0; it < io->max_num_iterations; ++it) {
-        icp_assoc_kernel<<<nb, kAssocThreads, 0, st>>>(r, t, m->inv, m->voxel_size, md2, src, tgt, valid, bc, state);
-        icp_compact_kernel<<<nb, kAssocThreads, 0, st>>>(r.cap, src, tgt, valid, bc, ps, pt, state);
-        icp_leaf_kernel<<<blocks_for(slots), 256, 0, st>>>(ps, pt, &state->n_pairs, cap, io->kernel_scale, &state->done,
-                                                            slots, val);
-        icp_solve_kernel<<<1, kTreeThreads, 0, st>>>(val, crit_sq, state);
-        launches += 4;
+        launch(OB_FAM_ICP, icp_assoc_kernel, nb, kAssocThreads, 0, st, r, t, m->inv, m->voxel_size, md2, src, tgt,
+               valid, bc, state);
+        launch(OB_FAM_ICP, icp_compact_kernel, nb, kAssocThreads, 0, st, r.cap, src, tgt, valid, bc, ps, pt, state);
+        launch(OB_FAM_ICP, icp_leaf_kernel, blocks_for(slots), 256, 0, st, ps, pt, &state->n_pairs, cap,
+               io->kernel_scale, &state->done, slots, val);
+        launch(OB_FAM_ICP, icp_solve_kernel, 1, kTreeThreads, 0, st, val, crit_sq, state);
     }
-    icp_finish_kernel<<<1, 1, 0, st>>>(state, static_cast<double*>(pose), static_cast<int32_t*>(iters));
-    count_launch(launches);
-    count_launch_of(OB_FAM_ICP, launches);
+    launch(OB_FAM_ICP, icp_finish_kernel, 1, 1, 0, st, state, static_cast<double*>(pose), static_cast<int32_t*>(iters));
     e = cudaGetLastError();
     if (e != cudaSuccess) return fail_cuda(e, "icp launch");
     e = stg.finish();  // host pose / iterations: one wait; device ones: nothing waits for the GPU

@@ -423,12 +423,10 @@ ob_status ob_zone_render(const ob_zone_render_io* io, ob_stream* s) {
     uint32_t* hits = static_cast<uint32_t*>(flags);
     uint32_t* ovf = hits + io->n_zones;
     const dim3 grid(unsigned((npx + kRenderTile - 1) / kRenderTile), io->n_zones);
-    zone_render_kernel<<<grid, kRenderThreads, size_t(max_tri) * 9 * sizeof(float), st>>>(
-        static_cast<const ZoneGpu*>(zdev), static_cast<const float*>(tris), static_cast<const double*>(bd),
-        static_cast<const double*>(bo), static_cast<const double*>(sd), static_cast<const double*>(so),
-        uint32_t(npx), static_cast<uint32_t*>(near), static_cast<uint32_t*>(far), hits, ovf);
-    count_launch(1);
-    count_launch_of(OB_FAM_ZONE, 1);
+    launch(OB_FAM_ZONE, zone_render_kernel, grid, kRenderThreads, size_t(max_tri) * 9 * sizeof(float), st,
+           static_cast<const ZoneGpu*>(zdev), static_cast<const float*>(tris), static_cast<const double*>(bd),
+           static_cast<const double*>(bo), static_cast<const double*>(sd), static_cast<const double*>(so),
+           uint32_t(npx), static_cast<uint32_t*>(near), static_cast<uint32_t*>(far), hits, ovf);
     e = cudaGetLastError();
     std::vector<uint32_t> hf(size_t(io->n_zones) * 2);
     if (e == cudaSuccess) e = cudaMemcpyAsync(hf.data(), flags, hf.size() * 4, cudaMemcpyDeviceToHost, st);
@@ -478,15 +476,12 @@ ob_status ob_zone_monitor_create(int device, uint32_t n_rows, uint32_t n_cols, c
     for (uint32_t i = n_live; i < OB_ZONE_MAX_LIVE; ++i) st0[i].id = 255;
     if (e == cudaSuccess) e = cudaMemcpy(m->states, st0, sizeof(st0), cudaMemcpyHostToDevice);
     if (e == cudaSuccess) {
-        zone_acc_reset_kernel<<<1, 32>>>(static_cast<ZoneAcc*>(m->acc));
-        uint64_t launches = 1;
+        launch(OB_FAM_ZONE, zone_acc_reset_kernel, 1, 32, 0, 0, static_cast<ZoneAcc*>(m->acc));
         if (n_live && npx) {
             const dim3 grid(unsigned(std::min<size_t>((npx + 255) / 256, 1024)), n_live);
-            zone_max_count_kernel<<<grid, 256>>>(m->near_mm, m->far_mm, uint32_t(npx), static_cast<ZoneCtl*>(m->ctl));
-            ++launches;
+            launch(OB_FAM_ZONE, zone_max_count_kernel, grid, 256, 0, 0, m->near_mm, m->far_mm, uint32_t(npx),
+                   static_cast<ZoneCtl*>(m->ctl));
         }
-        count_launch(launches);
-        count_launch_of(OB_FAM_ZONE, launches);
         e = cudaGetLastError();
     }
     if (e == cudaSuccess) e = cudaDeviceSynchronize();
@@ -517,17 +512,12 @@ ob_status ob_zone_monitor_update(ob_zone_monitor* m, const uint32_t* range, uint
         if (e == cudaSuccess && host_bm) e = cudaMemcpyAsync(bm, bitmask, npx * 4, cudaMemcpyHostToDevice, st);
     }
     if (e != cudaSuccess) return fail_cuda(e, "stage zone update");
-    uint64_t launches = 1;
-    if (npx) {
-        zone_occupancy_kernel<<<unsigned((npx + kOccTile - 1) / kOccTile), kOccThreads, 0, st>>>(
-            static_cast<const uint32_t*>(r), m->near_mm, m->far_mm, m->n_live, uint32_t(npx),
-            static_cast<ZoneAcc*>(m->acc), static_cast<uint32_t*>(bm));
-        ++launches;
-    }
-    zone_tail_kernel<<<1, 32, 0, st>>>(static_cast<ZoneAcc*>(m->acc), static_cast<ZoneCtl*>(m->ctl), m->n_live,
-                                       m->states);
-    count_launch(launches);
-    count_launch_of(OB_FAM_ZONE, launches);
+    if (npx)
+        launch(OB_FAM_ZONE, zone_occupancy_kernel, unsigned((npx + kOccTile - 1) / kOccTile), kOccThreads, 0, st,
+               static_cast<const uint32_t*>(r), m->near_mm, m->far_mm, m->n_live, uint32_t(npx),
+               static_cast<ZoneAcc*>(m->acc), static_cast<uint32_t*>(bm));
+    launch(OB_FAM_ZONE, zone_tail_kernel, 1, 32, 0, st, static_cast<ZoneAcc*>(m->acc), static_cast<ZoneCtl*>(m->ctl),
+           m->n_live, m->states);
     e = cudaGetLastError();
     if (e == cudaSuccess) e = stg.flush();
     if (e == cudaSuccess && (host_bm || (npx && !is_device_ptr(range)))) e = cudaStreamSynchronize(st);
