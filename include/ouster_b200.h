@@ -74,8 +74,11 @@ uint64_t ob_kernel_launch_count_of(const char* name);
  * cloud_threads (compute threads; a copy warp is added), cloud_ctas_per_sm, cloud_store_lag,
  * cloud_pose_tw, cloud_pose_stages, cloud_pose_ctas_per_sm, decode_stages, decode_threads,
  * decode_ctas_per_sm, decode_tile_packets, decode_prefetch, decode_runtime_plans, force_generic (K1: generic GPU kernel
- * instead of the TMA one).
- * Defaults come from OB_* environment variables of the same (upper-case) names. */
+ * instead of the TMA one), cloud_auto (1: K1 picks its geometry per launch, e.g. wider tiles for single-return float
+ * frames; setting cloud_tw, cloud_stages, cloud_threads or cloud_ctas_per_sm clears it, setting it to 1 restores
+ * the automatic choice).
+ * Defaults come from OB_* environment variables of the same (upper-case) names; cloud_auto starts at 0 when one of
+ * OB_CLOUD_TW, OB_CLOUD_STAGES, OB_CLOUD_THREADS or OB_CLOUD_CTAS_PER_SM is set, else at 1. */
 ob_status ob_set_tunable(int device, const char* name, int value);
 
 /* ---- streams ---- */
@@ -788,7 +791,8 @@ ob_status ob_frame_select_rows(const ob_frame_rows_io* io, ob_stream* s);
  * (impl/lidar_frame_impl.h:825-834), optionally destagger<T,3>(xyz) (:849-860) and
  * dewarp<T>(xyz, poses) (pose_util.h:37-59).
  * Layout: element (f, r, ...) of an array lives at base + f*frame_stride + r*return_stride
- * (strides in ELEMENTS of that array's scalar type).  NULL outputs are skipped.
+ * (strides in ELEMENTS of that array's scalar type).  NULL outputs are skipped.  Only the pixels are
+ * written: bytes between frames and returns (padded strides) are left untouched, in host and in device memory.
  */
 typedef struct ob_cloud_io {
     uint32_t n_frames;

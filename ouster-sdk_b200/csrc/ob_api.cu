@@ -99,8 +99,10 @@ bool set_tunable(int device, const char* name, int value) {
     std::lock_guard<std::mutex> lk(g_tun_mx);
     Tunables& t = tunables_mut(device);
     const std::string n(name);
-    if (n.rfind("cloud_", 0) == 0 && n != "cloud_store_lag" && n.find("pose") == std::string::npos) t.cloud_auto = 0;
-    if (n == "cloud_tw") t.cloud_tw = std::max(4, value / 4 * 4);
+    // setting one of the plain K1 geometry tunables pins that geometry; cloud_auto = 1 gives the choice back
+    if (n == "cloud_tw" || n == "cloud_stages" || n == "cloud_threads" || n == "cloud_ctas_per_sm") t.cloud_auto = 0;
+    if (n == "cloud_auto") t.cloud_auto = value ? 1 : 0;
+    else if (n == "cloud_tw") t.cloud_tw = std::max(4, value / 4 * 4);
     else if (n == "cloud_stages") t.cloud_stages = std::max(2, value);
     else if (n == "cloud_threads") t.cloud_threads = std::min(256, std::max(32, value / 32 * 32));
     else if (n == "cloud_ctas_per_sm") t.cloud_ctas_per_sm = std::max(1, value);
@@ -743,6 +745,18 @@ static ob_status scan_to_cloud_t(const ob_lut* lut, const uint16_t* shift, const
     auto extent = [&](size_t fs, size_t rs, size_t n) {
         return (F - 1) * fs + (R - 1) * rs + n;
     };
+    // true when the [F][R][n] blocks tile their extent with no gap (frame- or return-major); a host output with
+    // gaps is uploaded first, so that the copy back leaves the caller's bytes between the blocks as they were
+    auto dense = [&](size_t fs, size_t rs, size_t n) {
+        if (F > 1 && R > 1) return (rs == n && fs == R * n) || (fs == n && rs == F * n);
+        if (R > 1) return rs == n;
+        if (F > 1) return fs == n;
+        return true;
+    };
+    auto stage_out = [&](void* p, size_t fs, size_t rs, size_t n, size_t esz, void** d) {
+        const size_t bytes = extent(fs, rs, n) * esz;
+        return dense(fs, rs, n) ? stg.out(p, bytes, d) : stg.inout(p, bytes, d);
+    };
     CloudArgs<T> a;
     a.dir = static_cast<const T*>(lut->dir);
     a.off = static_cast<const T*>(lut->off);
@@ -769,17 +783,17 @@ static ob_status scan_to_cloud_t(const ob_lut* lut, const uint16_t* shift, const
     a.rd = nullptr;
     a.xd = nullptr;
     if (io->xyz) {
-        e = stg.out(io->xyz, extent(a.xyz_fs, a.xyz_rs, n_px * 3) * sizeof(T), &dout);
+        e = stage_out(io->xyz, a.xyz_fs, a.xyz_rs, n_px * 3, sizeof(T), &dout);
         if (e != cudaSuccess) return fail_cuda(e, "stage xyz");
         a.xyz = static_cast<T*>(dout);
     }
     if (io->range_destaggered) {
-        e = stg.out(io->range_destaggered, extent(a.rd_fs, a.rd_rs, n_px) * 4, &dout);
+        e = stage_out(io->range_destaggered, a.rd_fs, a.rd_rs, n_px, 4, &dout);
         if (e != cudaSuccess) return fail_cuda(e, "stage range_destaggered");
         a.rd = static_cast<uint32_t*>(dout);
     }
     if (io->xyz_destaggered) {
-        e = stg.out(io->xyz_destaggered, extent(a.xd_fs, a.xd_rs, n_px * 3) * sizeof(T), &dout);
+        e = stage_out(io->xyz_destaggered, a.xd_fs, a.xd_rs, n_px * 3, sizeof(T), &dout);
         if (e != cudaSuccess) return fail_cuda(e, "stage xyz_destaggered");
         a.xd = static_cast<T*>(dout);
     }
