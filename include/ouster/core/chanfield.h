@@ -33,6 +33,14 @@ static constexpr const char* RAW32_WORD2 = "RAW32_WORD2";
 static constexpr const char* RAW32_WORD3 = "RAW32_WORD3";
 static constexpr const char* RAW32_WORD4 = "RAW32_WORD4";
 static constexpr const char* RAW32_WORD5 = "RAW32_WORD5";
+static constexpr const char* NORMALS = "NORMALS";
+static constexpr const char* NORMALS2 = "NORMALS2";
+static constexpr const char* GROUND = "GROUND";
+static constexpr const char* GROUND2 = "GROUND2";
+/// The field of return `ret` (0-based): `base` for the first return, then base + "2", base + "3", ...
+inline std::string return_field_name(const std::string& base, int ret) {
+    return ret <= 0 ? base : base + std::to_string(ret + 1);
+}
 }  // namespace ChanField
 
 enum class ChanFieldType {

@@ -55,7 +55,7 @@ int ob_abi_version(void);
  * "ob_cloud_align_io", "ob_cloud_nearest_io", "ob_zone_desc", "ob_zone_render_io", "ob_zone_live", "ob_zone_state",
  * "ob_image_params", "ob_image_state", "ob_frame_field", "ob_frame_ops_io", "ob_frame_rows_entry",
  * "ob_frame_rows_io", "ob_map_rows", "ob_map_field", "ob_map_rows_item", "ob_interp_pose_io",
- * "ob_frame_poses_item");
+ * "ob_frame_poses_item", "ob_ground_model", "ob_ground_item");
  * 0 for unknown names.  Lets FFI bindings verify their layout. */
 size_t ob_abi_sizeof(const char* struct_name);
 const char* ob_last_error(void);
@@ -67,7 +67,7 @@ uint64_t ob_kernel_launch_count(void);
 /* launches of one named kernel family since load: "decode_pipe" (pipelined K2, also counted in "decode"),
  * "decode" (K2, any kernel), "cloud" (K1), "normals", "voxel", "voxel_map", "icp", "align", "zone", "image",
  * "frame_ops", "pose", "dewarp" (K3 and the per-column dewarp), "destagger", "lut" (LUT from intrinsics and
- * its f32 cast), "encode" (K4); 0 for unknown names.  Every launch belongs to exactly one family, so tests
+ * its f32 cast), "encode" (K4), "ground"; 0 for unknown names.  Every launch belongs to exactly one family, so tests
  * can assert which code path ran. */
 uint64_t ob_kernel_launch_count_of(const char* name);
 /* tuning hook (launch geometry and code-path selection only, never results): cloud_tw, cloud_stages,
@@ -312,6 +312,82 @@ typedef struct ob_normals_io {
     double* vertical_subtent_out;      /* optional, n_frames doubles: the first return's vertical pixel subtent */
 } ob_normals_io;
 ob_status ob_normals(ob_dtype dtype, const ob_normals_io* io, ob_stream* s);
+
+/* ---- ground segmentation (DESIGN f-13) ----
+ * replaces impl::get_ground_mask / get_ground_mask_into     ouster_algorithm/src/ground_seg.cpp:1137-1314
+ *          build_lower_envelope_ground_model and its passes ground_seg.cpp:179-945
+ *          GroundSegEngine::update (one call per FrameSet)   ground_seg.cpp:1319-1343
+ * One call segments every frame of a set (lut == NULL marks an empty slot, as in ob_dewarp_frames_io); each frame
+ * has its own shape, LUT and grid, and grid_size is one value for the call.  The model is built from the first two
+ * returns; every return gets a mask (1 = ground), and returns 3 and later are classified without normals.
+ * Arithmetic and orders are those of the oracle (oracle/orc_ground.c, DESIGN §9): given the same normals, the
+ * model after every pass and every mask pixel are bit-identical to it.
+ * normals / normals2: the frame's NORMALS / NORMALS2 fields (float32, h*w x 3, widened exactly); normals2 is read
+ * only alongside normals, and a second return without it is classified without normals.  A frame without normals
+ * and with compute_normals set gets the normals get_ground_mask computes (ground_seg.cpp:1195-1250): ob_normals with
+ * the reference's defaults on the dewarped float64 points of the first two returns, with per-column sensor origins
+ * (pose_c * sensor_to_body).translation; those launches count as "normals" (one ob_normals batch per distinct
+ * frame shape and return count in the call).  vertical_subtent_out receives the vertical pixel subtent they used
+ * (one device acos: the only way such a run can differ from a CPU one, DESIGN §9).  A frame without normals and
+ * without compute_normals is segmented without normals.
+ * stop: the pass to stop after (OB_GROUND_CELLS .. OB_GROUND_FINAL); the masks are classified only at
+ * OB_GROUND_FINAL and are zeroed otherwise.  Masks are written whole.
+ * Optional model outputs: the header, and the five grids (rows x cols, row-major) after pass `stop`; grid_capacity
+ * is their length in cells.
+ * Errors, checked before anything is launched (OB_INVALID_ARGUMENT, the reference's texts): "GroundSegConfig.grid_size
+ * must be > 0", then per frame "frame must contain RANGE field for get_ground_mask", "not enough output masks
+ * provided for get_ground_mask_into", "output mask shape does not match frame shape"; then OB_NO_DEVICE without a
+ * GPU, "ground segmentation needs a float64 lut" and "lut shape does not match frame shape".  The grid shapes are known only on the device: the call waits
+ * once for them, then fails "output capacity too small" when a frame's grid outputs are shorter than its grid.  A
+ * failing call writes no output.
+ * The wait makes the call impossible to capture in a CUDA graph.  Launches (family "ground", not counting CUB's
+ * sort and scan kernels): a fixed number for each `stop`, whatever the number of frames (22 at OB_GROUND_FINAL, one
+ * more when some frame computes its normals).
+ * An item with h * w == 0 has no pixel and is skipped.  Buffers may be host or device memory. */
+typedef enum ob_ground_stage {
+    OB_GROUND_CELLS = 0,
+    OB_GROUND_FILL1 = 1,
+    OB_GROUND_SMOOTH1 = 2,
+    OB_GROUND_PRUNE = 3,
+    OB_GROUND_FILL2 = 4,
+    OB_GROUND_SMOOTH2 = 5,
+    OB_GROUND_COMPONENTS = 6,
+    OB_GROUND_FILL3 = 7,
+    OB_GROUND_FINAL = 7
+} ob_ground_stage;
+typedef struct ob_ground_model {
+    double origin_x, origin_y; /* world xy of cell (0, 0)'s corner */
+    double fallback_z;         /* NaN without model points */
+    double footprint_bound;    /* 95th percentile of max(|x|, |y|); <= 25 m: indoor */
+    int32_t rows, cols;        /* 0 x 0 without model points */
+    int32_t valid;             /* some cell holds a height */
+    int32_t has_columns;       /* some column has status bit 0 */
+} ob_ground_model;
+typedef struct ob_ground_item {
+    const ob_lut* lut;             /* OB_F64, h x w, built with extrinsics; NULL: empty slot */
+    size_t h, w;
+    const uint32_t* const* range;  /* n_returns range images h x w (RANGE, RANGE2, ...); the array is host memory */
+    size_t n_returns;
+    const uint32_t* status;        /* w */
+    const double* poses;           /* w x 16: body_to_world per column */
+    const float* normals;          /* optional h*w x 3 */
+    const float* normals2;         /* optional h*w x 3, used only with normals */
+    const double* sensor_to_body;  /* 16, row-major: SensorInfo::extrinsic; read only when normals are computed */
+    int32_t compute_normals;       /* 1: compute normals when `normals` is NULL (what get_ground_mask does) */
+    int32_t pad;
+    double* vertical_subtent_out;  /* optional, 1 double: the subtent of the computed normals */
+    uint8_t* const* masks;         /* n_masks masks of mask_h x mask_w (the array is host memory) */
+    size_t n_masks, mask_h, mask_w;
+    ob_ground_model* model;        /* optional */
+    uint8_t* valid;                /* optional grids after pass `stop`, rows x cols */
+    uint8_t* obstacle;
+    double* floor_z;
+    double* height;
+    double* roughness;
+    size_t grid_capacity;          /* cells of each grid output */
+    int32_t* prune_levels;         /* optional: BFS levels the prune pass ran (0 when it did not run) */
+} ob_ground_item;
+ob_status ob_ground_mask(const ob_ground_item* items, size_t n_items, double grid_size, int stop, ob_stream* s);
 
 /* ---- voxel-grid downsampling (SURVEY 8f-2, the prefilter beside normals) ----
  * replaces core::voxel_downsample(frame, voxel_size)      ouster_core/src/voxel_hash_map.cpp:262-310   (SHUFFLE_FIRST)

@@ -61,6 +61,8 @@ ob_status obh_frame_add_field(obh_frame* f, const char* name, int32_t ty_tag, si
  * (1 PIXEL_FIELD, 2 COLUMN_FIELD, 3 PACKET_FIELD, 4 FRAME_FIELD); extra_dim > 1 adds one trailing dimension */
 ob_status obh_frame_add_field_class(obh_frame* f, const char* name, int32_t ty_tag, size_t extra_dim,
                                     int32_t field_class);
+/* LidarFrame::del_field(name): the field is dropped (std::invalid_argument when the frame has no such field) */
+ob_status obh_frame_del_field(obh_frame* f, const char* name);
 /* class and shape of a field: *ndim dimensions into shape[0..min(*ndim, 8)) */
 ob_status obh_frame_field_shape(obh_frame* f, const char* name, int32_t* field_class, size_t* ndim, size_t* shape);
 size_t obh_frame_n_fields(const obh_frame* f);

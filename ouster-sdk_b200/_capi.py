@@ -89,6 +89,26 @@ class FramePosesItem(C.Structure):
 OB_POSE_OK, OB_POSE_KNOT_ORDER, OB_POSE_ZERO_DURATION, OB_POSE_DESCENT = range(4)
 
 
+class GroundModel(C.Structure):
+    """ob_ground_model"""
+    _fields_ = [("origin_x", C.c_double), ("origin_y", C.c_double), ("fallback_z", C.c_double),
+                ("footprint_bound", C.c_double), ("rows", i32), ("cols", i32), ("valid", i32), ("has_columns", i32)]
+
+
+class GroundItem(C.Structure):
+    """ob_ground_item"""
+    _fields_ = [("lut", vp), ("h", sz), ("w", sz), ("range", C.POINTER(vp)), ("n_returns", sz), ("status", vp),
+                ("poses", vp), ("normals", vp), ("normals2", vp), ("sensor_to_body", vp), ("compute_normals", i32),
+                ("pad", i32), ("vertical_subtent_out", vp), ("masks", C.POINTER(vp)), ("n_masks", sz),
+                ("mask_h", sz), ("mask_w", sz), ("model", vp), ("valid", vp), ("obstacle", vp), ("floor_z", vp),
+                ("height", vp), ("roughness", vp), ("grid_capacity", sz), ("prune_levels", vp)]
+
+
+# passes of ob_ground_mask's model, in order (ob_ground_stage)
+GROUND_STAGES = ("cells", "fill1", "smooth1", "prune", "fill2", "smooth2", "components", "fill3")
+OB_GROUND_FINAL = len(GROUND_STAGES) - 1
+
+
 class VoxelMapCullIO(C.Structure):
     _fields_ = [("origin", vp), ("extracted", vp), ("capacity", sz), ("n_extracted", vp)]
 
@@ -282,6 +302,7 @@ _sig("ob_frames_to_map_rows", i32, C.POINTER(MapRowsItem), sz, vp, sz, sz, vp, v
 _sig("ob_voxel_map_destroy", i32, vp)
 _sig("ob_interp_pose", i32, C.POINTER(InterpPoseIO), vp)
 _sig("ob_frames_interp_pose", i32, C.POINTER(FramePosesItem), sz, C.c_double, vp, C.c_double, vp, vp, vp)
+_sig("ob_ground_mask", i32, C.POINTER(GroundItem), sz, C.c_double, i32, vp)
 _sig("ob_voxel_map_clear", i32, vp, vp)
 _sig("ob_voxel_map_add_points", i32, vp, C.POINTER(PointRows), vp)
 _sig("ob_voxel_map_remove_far", i32, vp, C.POINTER(VoxelMapCullIO), vp)

@@ -1031,6 +1031,104 @@ def frames_interp_pose(frames, t0, x0, t1=None, x1=None, error=None, stream=None
                                     _ptr(a1), _ptr(error), st.h))
 
 
+_GROUND_GRIDS = (("valid", np.uint8), ("obstacle", np.uint8), ("floor_z", np.float64), ("height", np.float64),
+                 ("roughness", np.float64))
+
+
+def ground_mask(frames, grid_size=0.5, stop=None, model=False, stream=None):
+    """ob_ground_mask: impl::get_ground_mask (ground_seg.cpp:1137-1314) over a frame set, one call for all frames.
+
+    `frames`: one entry per slot, None for an empty slot, else a dict {lut (a float64 XYZLutT built with
+    extrinsics), ranges (list of (H, W) uint32, one per return), status (W,), poses (W, 4, 4) float64[, normals,
+    normals2 (H, W, 3) float32: the NORMALS / NORMALS2 fields][, sensor_to_body (4, 4): given without normals, the
+    call computes the normals get_ground_mask would][, masks: contiguous (H, W) uint8 outputs, one per return]} --
+    numpy arrays or CUDA tensors; the masks of a frame
+    whose first range image is a CUDA tensor are CUDA tensors.  stop: the pass to stop after (an index into
+    _capi.GROUND_STAGES; default the last); masks are classified only after the last pass and are zero otherwise.
+    model=True also returns each frame's model after pass `stop`: its header and five (rows, cols) grids, on the
+    masks' side (a first call stopped after the cells pass learns the grid shapes).
+    -> list with, per slot, None or {"masks": [one (H, W) uint8 per return], and with model=True "model" (dict of
+    the ob_ground_model fields), "grids" (dict, None without a grid), "prune_levels"}; a frame whose normals were
+    computed also has "vertical_subtent" (the subtent they used).  Errors raise ValueError with
+    the reference's texts."""
+    stop = _capi.OB_GROUND_FINAL if stop is None else int(stop)
+    n = len(frames)
+    items = (_capi.GroundItem * max(n, 1))()
+    keep, out, ref, dev = [], [None] * n, None, 0
+    for i, fr in enumerate(frames):
+        if fr is None:
+            continue
+        lut = fr["lut"]
+        h, w = lut.h, lut.w
+        rngs = [_contig(r, np.uint32) for r in fr["ranges"]]
+        for r in rngs:
+            if _numel(r) != h * w:
+                raise ValueError("unexpected image dimensions")
+        status, poses = _contig(fr["status"], np.uint32), _contig(fr["poses"], np.float64)
+        if _numel(status) != w or _numel(poses) != w * 16:
+            raise ValueError("poses must be [W, 4, 4] and status [W]")
+        nrm = [None if fr.get(k) is None else _contig(fr[k], np.float32) for k in ("normals", "normals2")]
+        for x in nrm:
+            if x is not None and _numel(x) != h * w * 3:
+                raise ValueError("normals must be [H, W, 3]")
+        s2b = None
+        if nrm[0] is None and fr.get("sensor_to_body") is not None:
+            s2b = _contig(fr["sensor_to_body"], np.float64)
+        masks = fr.get("masks") or [_empty(rngs[0] if rngs else status, (h, w), np.uint8) for _ in rngs]
+        rp = (C.c_void_p * max(len(rngs), 1))(*[_ptr(r) for r in rngs])
+        mp = (C.c_void_p * max(len(masks), 1))(*[_ptr(m) for m in masks])
+        sub = np.zeros(1)
+        keep += [rngs, status, poses, nrm, masks, rp, mp, s2b, sub]
+        it = items[i]
+        it.lut, it.h, it.w, it.n_returns = lut._h, h, w, len(rngs)
+        it.range = C.cast(rp, C.POINTER(C.c_void_p)) if rngs else None
+        it.status, it.poses, it.normals, it.normals2 = _ptr(status), _ptr(poses), _ptr(nrm[0]), _ptr(nrm[1])
+        it.masks, it.n_masks, it.mask_h, it.mask_w = C.cast(mp, C.POINTER(C.c_void_p)), len(masks), h, w
+        out[i] = {"masks": masks}
+        if s2b is not None:
+            it.sensor_to_body, it.compute_normals, it.vertical_subtent_out = _ptr(s2b), 1, sub.ctypes.data
+            out[i]["_sub"] = sub
+        if ref is None:
+            ref, dev = (rngs[0] if rngs else status), lut.device
+    st = _stream_for(ref, stream, dev)
+    def done():
+        for o in out:
+            if o is not None and "_sub" in o:
+                o["vertical_subtent"] = float(o.pop("_sub")[0])
+        return out
+    if not model:
+        check(lib.ob_ground_mask(items, n, float(grid_size), stop, st.h))
+        return done()
+    headers = [_capi.GroundModel() for _ in range(n)]
+    levels = np.zeros(n, np.int32)
+    for i in range(n):
+        if out[i] is not None:
+            items[i].model = C.addressof(headers[i])
+    check(lib.ob_ground_mask(items, n, float(grid_size), _capi.GROUND_STAGES.index("cells"), st.h))
+    for i in range(n):
+        if out[i] is None:
+            continue
+        hd = headers[i]
+        cells = int(hd.rows) * int(hd.cols)
+        grids = None
+        if cells > 0:
+            like = out[i]["masks"][0] if out[i]["masks"] else None
+            grids = {k: _empty(like, (hd.rows, hd.cols), dt) for k, dt in _GROUND_GRIDS}
+            keep.append(grids)
+            for k, _ in _GROUND_GRIDS:
+                setattr(items[i], k, _ptr(grids[k]))
+            items[i].grid_capacity = cells
+        items[i].prune_levels = levels.ctypes.data + 4 * i
+        out[i]["grids"] = grids
+    check(lib.ob_ground_mask(items, n, float(grid_size), stop, st.h))
+    st.sync()
+    for i in range(n):
+        if out[i] is not None:
+            out[i]["model"] = {k: getattr(headers[i], k) for k, _ in _capi.GroundModel._fields_}
+            out[i]["prune_levels"] = int(levels[i])
+    return done()
+
+
 def transform(points, pose, out=None, stream=None, device=0):
     """transform(points (..., 3), pose (4, 4)): one pose for every point (pose_util.h:118-131)."""
     pose = pose if _is_torch(pose) else np.ascontiguousarray(pose, _np_dtype(points)).reshape(1, 16)

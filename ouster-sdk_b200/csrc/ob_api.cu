@@ -19,7 +19,7 @@ static std::atomic<uint64_t> g_family[OB_FAM_COUNT];
 static const char* const kFamilies[OB_FAM_COUNT] = {"decode_pipe", "decode", "cloud", "normals", "voxel",
                                                     "voxel_map", "icp", "align", "zone", "image",
                                                     "frame_ops", "pose", "dewarp", "destagger", "lut",
-                                                    "encode"};
+                                                    "encode", "ground"};
 
 void record_launch(int family) {
     g_family[family].fetch_add(1, std::memory_order_relaxed);
@@ -428,6 +428,8 @@ size_t ob_abi_sizeof(const char* name) {
     if (n == "ob_map_rows_item") return sizeof(ob_map_rows_item);
     if (n == "ob_interp_pose_io") return sizeof(ob_interp_pose_io);
     if (n == "ob_frame_poses_item") return sizeof(ob_frame_poses_item);
+    if (n == "ob_ground_model") return sizeof(ob_ground_model);
+    if (n == "ob_ground_item") return sizeof(ob_ground_item);
     return 0;
 }
 

@@ -193,7 +193,7 @@ cudaError_t make_decode_params(const DecodeLaunch& a, int device, bool pipe, Dec
 enum { OB_FAM_DECODE_PIPE = 0, OB_FAM_DECODE = 1, OB_FAM_CLOUD = 2, OB_FAM_NORMALS = 3, OB_FAM_VOXEL = 4,
        OB_FAM_VOXEL_MAP = 5, OB_FAM_ICP = 6, OB_FAM_ALIGN = 7, OB_FAM_ZONE = 8, OB_FAM_IMAGE = 9,
        OB_FAM_FRAME_OPS = 10, OB_FAM_POSE = 11, OB_FAM_DEWARP = 12, OB_FAM_DESTAGGER = 13, OB_FAM_LUT = 14,
-       OB_FAM_ENCODE = 15, OB_FAM_COUNT = 16 };
+       OB_FAM_ENCODE = 15, OB_FAM_GROUND = 16, OB_FAM_COUNT = 17 };
 void record_launch(int family);
 
 // Every kernel of the library is launched through here, so the launch counters cannot drift from the launches.

@@ -36,6 +36,7 @@ _sig("obh_sensor_destroy", i32, vp)
 _sig("obh_frame_create", i32, vp, PP(vp))
 _sig("obh_frame_add_field", i32, vp, C.c_char_p, C.c_int32, sz)
 _sig("obh_frame_add_field_class", i32, vp, C.c_char_p, C.c_int32, sz, C.c_int32)
+_sig("obh_frame_del_field", i32, vp, C.c_char_p)
 _sig("obh_frame_field_shape", i32, vp, C.c_char_p, PP(C.c_int32), PP(sz), PP(sz))
 _sig("obh_frame_n_fields", sz, vp)
 _sig("obh_frame_field_at", i32, vp, sz, C.c_char_p, sz, PP(C.c_int32), PP(sz), PP(vp))
@@ -266,6 +267,10 @@ class LidarFrame(_Handle):
         check(lib.obh_frame_add_field_class(self._h, name.encode(),
                                             NP_TAG[np.dtype(dtype)] if tag is None else int(tag), extra_dim,
                                             int(field_class)))
+
+    def del_field(self, name):
+        """LidarFrame::del_field: drops the field (ValueError when the frame has none of that name)."""
+        check(lib.obh_frame_del_field(self._h, name.encode()))
 
     def field_class(self, name):
         """FieldClass of a field (1 PIXEL_FIELD, 2 COLUMN_FIELD, 3 PACKET_FIELD, 4 FRAME_FIELD)."""

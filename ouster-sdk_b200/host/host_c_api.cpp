@@ -234,6 +234,13 @@ ob_status obh_frame_add_field_class(obh_frame* f, const char* name, int32_t tag,
     });
 }
 
+ob_status obh_frame_del_field(obh_frame* f, const char* name) {
+    return guard([&] {
+        if (!f || !name) throw std::invalid_argument("null pointer");
+        f->ref().del_field(name);
+    });
+}
+
 ob_status obh_frame_field_shape(obh_frame* f, const char* name, int32_t* cls, size_t* ndim, size_t* shape) {
     return guard([&] {
         if (!f || !name) throw std::invalid_argument("null pointer");

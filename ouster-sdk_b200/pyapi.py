@@ -40,6 +40,7 @@ class ChanField:
     RANGE, RANGE2, SIGNAL, SIGNAL2 = "RANGE", "RANGE2", "SIGNAL", "SIGNAL2"
     REFLECTIVITY, REFLECTIVITY2, NEAR_IR = "REFLECTIVITY", "REFLECTIVITY2", "NEAR_IR"
     FLAGS, FLAGS2, WINDOW = "FLAGS", "FLAGS2", "WINDOW"
+    NORMALS, NORMALS2, GROUND, GROUND2 = "NORMALS", "NORMALS2", "GROUND", "GROUND2"
 
 
 def _info_dict(info):
@@ -605,6 +606,100 @@ class ConstantVelocityDeskewMethod(DeskewMethod):
             _c.frames_interp_pose(items, 0.0, self._initial)
         else:
             _c.frames_interp_pose(items, self._ts[0], self._poses[0], self._ts[-1], self._poses[-1])
+        return frames
+
+
+def _return_field_name(base, ret):
+    """ChanField::return_field_name: `base` for return 0, then base + "2", base + "3", ..."""
+    return base if ret <= 0 else base + str(ret + 1)
+
+
+class GroundSegConfig:
+    """GroundSegConfig (ground_seg.h): grid_size, the cell size in metres of the 2.5-D height map."""
+
+    def __init__(self, grid_size=0.5):
+        self.grid_size = grid_size
+
+
+class GroundSegEngine:
+    """GroundSegEngine (ground_seg.cpp:1346-1416).  update(frames) segments the frames of a set in one
+    ob_ground_mask call: `frames` is a list with None for empty slots, of LidarScan or DeviceLidarScan.  Each frame
+    gets GROUND (and GROUND2, ... up to its sensor's returns) as uint8 pixel fields, deleted and re-added zeroed,
+    then filled where the frame keeps its pixels (host arrays, or device tensors); GROUND fields beyond the returns
+    the frame has (up to the first missing RANGEk) are removed.  A frame without float32 NORMALS gets the normals
+    the reference computes, with the sensor's sensor_to_body.  A DeviceLidarScan's poses and status are read from
+    its host side.  One LUT (with extrinsics) is kept per sensor serial number.  Returns `frames`."""
+
+    def __init__(self, config):
+        self.config = config
+        self._luts = {}
+
+    @staticmethod
+    def create(config=None):
+        config = GroundSegConfig() if config is None else config
+        g = float(config.grid_size)
+        if not np.isfinite(g) or g <= 0.0:
+            raise ValueError("GroundSegConfig.grid_size must be > 0")
+        return GroundSegEngine(config)
+
+    def _lut(self, info):
+        key = getattr(info, "sn", 0)
+        if key not in self._luts:
+            self._luts[key] = XYZLut(info, use_extrinsics=True)._lut
+        return self._luts[key]
+
+    def update(self, frames):
+        items, plans = [], []
+        for f in frames:
+            if f is None:
+                items.append(None)
+                continue
+            dev = isinstance(f, DeviceLidarScan)
+            info = f.info if dev else f.sensor_info
+            if info is None:
+                raise ValueError("frame.sensor_info is required for get_ground_mask")
+            names = f.fields
+            if ChanField.RANGE not in names:
+                raise ValueError("frame must contain RANGE field for get_ground_mask")
+            n_max = 2 if "DUAL" in str(getattr(info, "profile", "")).upper() else 1
+            ranges = [f.field(ChanField.RANGE)]
+            for ret in range(1, n_max):
+                name = _return_field_name(ChanField.RANGE, ret)
+                if name not in names:
+                    break
+                ranges.append(f.field(name))
+            masks = []
+            for ret in range(n_max):
+                name = _return_field_name(ChanField.GROUND, ret)
+                if dev:
+                    f._fields[name] = _torch().zeros((f.h, f.w), dtype=_torch().uint8, device=ranges[0].device)
+                    masks.append(f._fields[name])
+                else:
+                    if name in names:
+                        f.del_field(name)
+                    f.add_field(name, np.uint8)
+                    masks.append(f.field(name))
+            host = f.host if dev else f
+            item = {"lut": self._lut(info), "ranges": ranges, "status": host.status, "poses": host.body_to_world,
+                    "masks": masks[:len(ranges)]}
+            nrm = [f.field(k) if k in names else None for k in (ChanField.NORMALS, ChanField.NORMALS2)]
+            if nrm[0] is not None and str(nrm[0].dtype) in ("float32", "torch.float32"):
+                item["normals"] = nrm[0]
+                if nrm[1] is not None and len(ranges) > 1:
+                    item["normals2"] = nrm[1]
+            else:
+                s2b = getattr(info, "sensor_to_body", None)
+                item["sensor_to_body"] = np.eye(4) if s2b is None else np.asarray(s2b, np.float64)
+            items.append(item)
+            plans.append((f, dev, len(ranges), n_max))
+        _c.ground_mask(items, grid_size=self.config.grid_size)
+        for f, dev, n_found, n_max in plans:
+            for ret in range(n_found, n_max):
+                name = _return_field_name(ChanField.GROUND, ret)
+                if dev:
+                    f._fields.pop(name, None)
+                elif name in f.fields:
+                    f.del_field(name)
         return frames
 
 
