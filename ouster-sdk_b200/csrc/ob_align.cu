@@ -25,8 +25,6 @@
 //                 (point-to-plane), composes the pose and sets the stop flag.
 #include <cub/block/block_reduce.cuh>
 #include <cub/block/block_scan.cuh>
-#include <cub/device/device_radix_sort.cuh>
-#include <cub/device/device_scan.cuh>
 #include <cuda/std/tuple>
 
 #include <algorithm>
@@ -35,6 +33,7 @@
 #include <cmath>
 
 #include "ob_api_common.h"
+#include "ob_cub.cuh"
 #include "ob_ldlt.cuh"
 #include "ob_rows.cuh"
 #include "ob_se3.cuh"
@@ -640,32 +639,22 @@ cudaError_t build_grid(const Rows& t, const void* normals, double cell_size, Sta
     const unsigned cap = std::max(t.cap, 1u);
     unsigned slots = 64;
     while (slots < 2 * cap) slots <<= 1;
-    GKey *keys, *sk;
-    uint32_t *seq, *sseq, *head, *cid, *cbeg, *cend, *row;
-    int64_t* ckey;
-    int32_t* table;
-    double* pts;
-    cudaError_t e = scratch(stg, cap * sizeof(GKey), &keys);
-    if (e == cudaSuccess) e = scratch(stg, cap * sizeof(GKey), &sk);
-    if (e == cudaSuccess) e = scratch(stg, cap * 4ull, &seq);
-    if (e == cudaSuccess) e = scratch(stg, cap * 4ull, &sseq);
-    if (e == cudaSuccess) e = scratch(stg, cap * 4ull, &head);
-    if (e == cudaSuccess) e = scratch(stg, cap * 4ull, &cid);
-    if (e == cudaSuccess) e = scratch(stg, cap * 4ull, &cbeg);
-    if (e == cudaSuccess) e = scratch(stg, cap * 4ull, &cend);
-    if (e == cudaSuccess) e = scratch(stg, cap * 4ull, &row);
-    if (e == cudaSuccess) e = scratch(stg, cap * 24ull, &ckey);
-    if (e == cudaSuccess) e = scratch(stg, cap * 24ull, &pts);
-    if (e == cudaSuccess) e = scratch(stg, slots * 4ull, &table);
-    if (e != cudaSuccess) return e;
-    size_t need = 0, tmp_bytes = 0;
-    e = cub::DeviceRadixSort::SortPairs(nullptr, need, keys, sk, seq, sseq, static_cast<int>(cap), GKeyDecomposer{}, 0,
-                                        kGKeyBits, st);
-    tmp_bytes = need;
-    if (e == cudaSuccess) e = cub::DeviceScan::InclusiveSum(nullptr, need, head, cid, static_cast<int>(cap), st);
-    tmp_bytes = std::max(tmp_bytes, need);
-    void* tmp = nullptr;
-    if (e == cudaSuccess) e = stg.scratch(tmp_bytes, &tmp);
+    auto* keys = stg.scratch<GKey>(cap);
+    auto* sk = stg.scratch<GKey>(cap);
+    auto* seq = stg.scratch<uint32_t>(cap);
+    auto* sseq = stg.scratch<uint32_t>(cap);
+    auto* head = stg.scratch<uint32_t>(cap);
+    auto* cid = stg.scratch<uint32_t>(cap);
+    auto* cbeg = stg.scratch<uint32_t>(cap);
+    auto* cend = stg.scratch<uint32_t>(cap);
+    auto* row = stg.scratch<uint32_t>(cap);
+    auto* ckey = stg.scratch<int64_t>(cap * 3ull);
+    auto* pts = stg.scratch<double>(cap * 3ull);
+    auto* table = stg.scratch<int32_t>(slots);
+    const auto sort = sort_pairs(keys, sk, seq, sseq, static_cast<int>(cap), GKeyDecomposer{}, 0, kGKeyBits, st);
+    const auto scan = inclusive_sum(head, cid, static_cast<int>(cap), st);
+    CubTemp tmp(stg, sort, scan);
+    cudaError_t e = stg.error();
     if (e == cudaSuccess) e = cudaMemsetAsync(table, 0xff, slots * 4ull, st);
     if (e != cudaSuccess) return e;
     const unsigned nb = blocks_for(cap);
@@ -673,11 +662,10 @@ cudaError_t build_grid(const Rows& t, const void* normals, double cell_size, Sta
     tc.cap = cap;  // rows_n() still clamps to the real count; rows past it get the pad bit
     if (t.cap == 0) tc.n_dev = nullptr, tc.n_host = 0;
     launch(OB_FAM_ALIGN, gr_key_kernel<T>, nb, 256, 0, st, tc, normals, 1.0 / cell_size, keys, seq);
-    e = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, sk, seq, sseq, static_cast<int>(cap), GKeyDecomposer{}, 0,
-                                        kGKeyBits, st);
+    e = tmp.run(sort);
     if (e != cudaSuccess) return e;
     launch(OB_FAM_ALIGN, gr_head_kernel, nb, 256, 0, st, cap, sk, head);
-    e = cub::DeviceScan::InclusiveSum(tmp, tmp_bytes, head, cid, static_cast<int>(cap), st);
+    e = tmp.run(scan);
     if (e != cudaSuccess) return e;
     launch(OB_FAM_ALIGN, gr_fill_kernel<T>, nb, 256, 0, st, cap, t.p, sk, sseq, cid, ckey, cbeg, cend, table, slots - 1,
            pts, row);
@@ -695,23 +683,17 @@ ob_status run_align(const ob_cloud_align_io* io, const Rows& sr, const Rows& tr,
     const unsigned kcap = std::max(sr.cap, 1u);
     const unsigned nb = (kcap + kThreads - 1) / kThreads;
     const unsigned slots = (kcap + kLeaf - 1) / kLeaf;
-    AlignState* state = nullptr;
-    double *rows = nullptr, *pairs = nullptr, *val = nullptr;
-    uint32_t *valid = nullptr, *bc = nullptr;
-    unsigned long long *keys = nullptr, *skeys = nullptr;
-    e = scratch(stg, sizeof(AlignState), &state);
-    if (e == cudaSuccess) e = scratch(stg, kcap * 8ull * kPair, &rows);
-    if (e == cudaSuccess) e = scratch(stg, kcap * 8ull * kPair, &pairs);
-    if (e == cudaSuccess) e = scratch(stg, slots * 8ull * 27, &val);
-    if (e == cudaSuccess) e = scratch(stg, kcap * 4ull, &valid);
-    if (e == cudaSuccess) e = scratch(stg, nb * 4ull, &bc);
-    if (e == cudaSuccess) e = scratch(stg, kcap * 8ull, &keys);
-    if (e == cudaSuccess) e = scratch(stg, kcap * 8ull, &skeys);
-    size_t tmp_bytes = 0;
-    if (e == cudaSuccess)
-        e = cub::DeviceRadixSort::SortKeys(nullptr, tmp_bytes, keys, skeys, static_cast<int>(kcap), 0, 64, st);
-    void* tmp = nullptr;
-    if (e == cudaSuccess) e = stg.scratch(tmp_bytes, &tmp);
+    auto* state = stg.scratch<AlignState>(1);
+    auto* rows = stg.scratch<double>(static_cast<size_t>(kcap) * kPair);
+    auto* pairs = stg.scratch<double>(static_cast<size_t>(kcap) * kPair);
+    auto* val = stg.scratch<double>(slots * 27ull);
+    auto* valid = stg.scratch<uint32_t>(kcap);
+    auto* bc = stg.scratch<uint32_t>(nb);
+    auto* keys = stg.scratch<unsigned long long>(kcap);
+    auto* skeys = stg.scratch<unsigned long long>(kcap);
+    const auto median_sort = sort_keys(keys, skeys, static_cast<int>(kcap), 0, 64, st);
+    CubTemp tmp(stg, median_sort);
+    e = stg.error();
     if (e != cudaSuccess) return fail_cuda(e, "cloud align workspace");
     const double max_d2 = io->max_corr_dist * io->max_corr_dist;
     const double cos_gate = plane ? std::cos(io->max_normal_angle_deg * M_PI / 180.0) : 0.0;
@@ -725,7 +707,7 @@ ob_status run_align(const ob_cloud_align_io* io, const Rows& sr, const Rows& tr,
             launch(OB_FAM_ALIGN, al_assoc_kernel<T, false>, nb, kThreads, 0, st, sr, nullptr, tr.p, nullptr, g, max_d2,
                    0.0, kcap, state, rows, valid, bc, keys);
         launch(OB_FAM_ALIGN, al_compact_kernel, nb, kThreads, 0, st, kcap, rows, valid, bc, pairs, state);
-        e = cub::DeviceRadixSort::SortKeys(tmp, tmp_bytes, keys, skeys, static_cast<int>(kcap), 0, 64, st);
+        e = tmp.run(median_sort);
         if (e != cudaSuccess) return fail_cuda(e, "cloud align median");
         if (plane) {
             launch(OB_FAM_ALIGN, al_leaf_kernel<kPlaneSystem>, lb, 256, 0, st, pairs, skeys, io->max_corr_dist, state,
@@ -780,24 +762,16 @@ ob_status ob_cloud_align(const ob_cloud_align_io* io, ob_stream* s) {
     if (rs == OB_OK) rs = stage_rows(&io->target, stg, &tr, "stage align target");
     if (rs != OB_OK) return rs;
     const size_t esz = elem_size(io->source.dtype);
-    const void *snrm = nullptr, *tnrm = nullptr, *guess = nullptr;
-    cudaError_t e = cudaSuccess;
-    if (plane) {
-        e = stg.in(io->source_normals, sr.cap * 3 * esz, &snrm);
-        if (e == cudaSuccess) e = stg.in(io->target_normals, tr.cap * 3 * esz, &tnrm);
-    }
-    if (e == cudaSuccess && io->initial_guess) e = stg.in(io->initial_guess, 16 * 8, &guess);
-    void *pose = nullptr, *iters = nullptr;
-    if (e == cudaSuccess) e = stg.out(io->pose, 16 * 8, &pose);
-    if (e == cudaSuccess) e = stg.out(io->iterations, 4, &iters);
-    if (e != cudaSuccess) return fail_cuda(e, "stage cloud align");
-    const double* g = static_cast<const double*>(guess);
-    double* p = static_cast<double*>(pose);
-    int32_t* it = static_cast<int32_t*>(iters);
+    const void* snrm = plane ? stg.in(io->source_normals, sr.cap * 3 * esz) : nullptr;
+    const void* tnrm = plane ? stg.in(io->target_normals, tr.cap * 3 * esz) : nullptr;
+    const double* g = stg.in(io->initial_guess, 16);
+    double* p = stg.out(io->pose, 16);
+    int32_t* it = stg.out(io->iterations, 1);
+    if (cudaError_t e = stg.error()) return fail_cuda(e, "stage cloud align");
     rs = io->source.dtype == OB_F64 ? run_align<double>(io, sr, tr, snrm, tnrm, g, stg, st, p, it)
                                     : run_align<float>(io, sr, tr, snrm, tnrm, g, stg, st, p, it);
     if (rs != OB_OK) return rs;
-    e = stg.finish();  // host pose / iterations: one wait; device ones: nothing waits for the GPU
+    cudaError_t e = stg.finish();  // host pose / iterations: one wait; device ones: nothing waits for the GPU
     if (e != cudaSuccess) return fail_cuda(e, "cloud align result");
     return OB_OK;
 }
@@ -817,26 +791,25 @@ ob_status ob_cloud_nearest(const ob_cloud_nearest_io* io, ob_stream* s) {
     if (rs == OB_OK) rs = stage_rows(&io->queries, stg, &qr, "stage nearest queries");
     if (rs != OB_OK || qr.cap == 0) return rs;
     if (!io->indices) return fail(OB_INVALID_ARGUMENT, "null indices buffer");
-    const void* nrm = nullptr;
-    void* out = nullptr;
-    cudaError_t e = cudaSuccess;
-    if (io->target_normals) e = stg.in(io->target_normals, tr.cap * 3 * elem_size(io->target.dtype), &nrm);
-    if (e == cudaSuccess) e = stg.out(io->indices, qr.cap * 4ull, &out);
-    if (e != cudaSuccess) return fail_cuda(e, "stage nearest");
+    const void* nrm = stg.in(io->target_normals, tr.cap * 3 * elem_size(io->target.dtype));
+    int32_t* out = stg.out(io->indices, qr.cap);
+    if (cudaError_t e = stg.error()) return fail_cuda(e, "stage nearest");
     Grid g{};
+    cudaError_t e;
     if (io->target.dtype == OB_F64) {
         e = build_grid<double>(tr, nrm, io->cell_size, stg, st, &g);
         if (e == cudaSuccess)
             launch(OB_FAM_ALIGN, al_nearest_kernel<double>, blocks_for(qr.cap), 256, 0, st, qr, g, io->max_dist_sq,
-                   static_cast<int32_t*>(out));
+                   out);
     } else {
         e = build_grid<float>(tr, nrm, io->cell_size, stg, st, &g);
         if (e == cudaSuccess)
             launch(OB_FAM_ALIGN, al_nearest_kernel<float>, blocks_for(qr.cap), 256, 0, st, qr, g, io->max_dist_sq,
-                   static_cast<int32_t*>(out));
+                   out);
     }
     if (e == cudaSuccess) e = cudaGetLastError();
-    if (e == cudaSuccess) e = stg.finish();
+    stg.check(e);
+    e = stg.finish();
     if (e != cudaSuccess) return fail_cuda(e, "cloud nearest");
     return OB_OK;
 }

@@ -152,74 +152,34 @@ Staging::~Staging() {
     for (void* p : scratch_) cudaFreeAsync(p, st_);
 }
 
-cudaError_t Staging::in(const void* p, size_t bytes, const void** dev) {
-    if (bytes == 0 || p == nullptr) {
-        *dev = p;
-        return cudaSuccess;
-    }
-    if (is_device_ptr(p)) {
-        *dev = p;
-        return cudaSuccess;
-    }
-    void* d = nullptr;
-    cudaError_t e = cudaMallocAsync(&d, bytes, st_);
-    if (e != cudaSuccess) return e;
-    scratch_.push_back(d);
-    e = cudaMemcpyAsync(d, p, bytes, cudaMemcpyHostToDevice, st_);
-    *dev = d;
-    return e;
+void* Staging::stage(const void* p, size_t bytes, bool upload, bool download) {
+    if (err_ != cudaSuccess) return nullptr;
+    if (bytes == 0 || p == nullptr || is_device_ptr(p)) return const_cast<void*>(p);
+    void* d = scratch_bytes(bytes);
+    if (d && upload) check(cudaMemcpyAsync(d, p, bytes, cudaMemcpyHostToDevice, st_));
+    if (d && download) pending_.push_back({const_cast<void*>(p), d, bytes});
+    return d;
 }
 
-cudaError_t Staging::out(void* p, size_t bytes, void** dev) {
-    if (bytes == 0 || p == nullptr) {
-        *dev = p;
-        return cudaSuccess;
-    }
-    if (is_device_ptr(p)) {
-        *dev = p;
-        return cudaSuccess;
-    }
+void* Staging::scratch_bytes(size_t bytes) {
+    if (err_ != cudaSuccess) return nullptr;
     void* d = nullptr;
-    cudaError_t e = cudaMallocAsync(&d, bytes, st_);
-    if (e != cudaSuccess) return e;
+    if (check(cudaMallocAsync(&d, bytes ? bytes : 16, st_)) != cudaSuccess) return nullptr;
     scratch_.push_back(d);
-    pending_.push_back({p, d, bytes});
-    *dev = d;
-    return cudaSuccess;
-}
-
-cudaError_t Staging::inout(void* p, size_t bytes, void** dev) {
-    const void* d = nullptr;
-    cudaError_t e = in(p, bytes, &d);
-    if (e != cudaSuccess) return e;
-    if (d != p) pending_.push_back({p, const_cast<void*>(d), bytes});
-    *dev = const_cast<void*>(d);
-    return cudaSuccess;
-}
-
-cudaError_t Staging::scratch(size_t bytes, void** dev) {
-    void* d = nullptr;
-    cudaError_t e = cudaMallocAsync(&d, bytes ? bytes : 16, st_);
-    if (e != cudaSuccess) return e;
-    scratch_.push_back(d);
-    *dev = d;
-    return cudaSuccess;
+    return d;
 }
 
 cudaError_t Staging::flush() {
-    for (const Pending& q : pending_) {
-        cudaError_t e = cudaMemcpyAsync(q.host, q.dev, q.bytes, cudaMemcpyDeviceToHost, st_);
-        if (e != cudaSuccess) return e;
-    }
+    for (const Pending& q : pending_)
+        if (err_ == cudaSuccess) check(cudaMemcpyAsync(q.host, q.dev, q.bytes, cudaMemcpyDeviceToHost, st_));
     pending_.clear();
-    return cudaSuccess;
+    return err_;
 }
 
 cudaError_t Staging::finish() {
     const bool wait = !pending_.empty();
-    cudaError_t e = flush();
-    if (e == cudaSuccess && wait) e = cudaStreamSynchronize(st_);
-    return e;
+    if (flush() == cudaSuccess && wait) check(cudaStreamSynchronize(st_));
+    return err_;
 }
 
 CountedRows::CountedRows(size_t* n, size_t capacity, Staging& stg, cudaStream_t st, const char* what)
@@ -245,21 +205,17 @@ ob_status CountedRows::refuse(std::initializer_list<const void*> arrays, const c
     return OB_OK;
 }
 
-cudaError_t CountedRows::array(void* p, size_t row_bytes, void** dev) {
-    *dev = p;
-    if (!p || is_device_ptr(p)) return cudaSuccess;
-    cudaError_t e = stg_.scratch(cap_ * row_bytes, dev);
-    if (e == cudaSuccess) host_.push_back({p, *dev, row_bytes});
-    return e;
+void* CountedRows::array(void* p, size_t row_bytes) {
+    if (stg_.error()) return nullptr;
+    if (!p || is_device_ptr(p)) return p;
+    void* d = stg_.scratch<void>(cap_ * row_bytes);
+    if (d) host_.push_back({p, d, row_bytes});
+    return d;
 }
 
-cudaError_t CountedRows::word(unsigned long long** w) {
-    *w = reinterpret_cast<unsigned long long*>(n_);
-    if (dev_) return cudaSuccess;
-    void* d = nullptr;
-    cudaError_t e = stg_.scratch(8, &d);
-    *w = static_cast<unsigned long long*>(d);
-    return e;
+unsigned long long* CountedRows::word() {
+    if (dev_) return reinterpret_cast<unsigned long long*>(n_);
+    return stg_.scratch<unsigned long long>(1);
 }
 
 ob_status CountedRows::finish(const unsigned long long* end) {
@@ -755,9 +711,9 @@ static ob_status scan_to_cloud_t(const ob_lut* lut, const uint16_t* shift, const
         if (F > 1) return fs == n;
         return true;
     };
-    auto stage_out = [&](void* p, size_t fs, size_t rs, size_t n, size_t esz, void** d) {
-        const size_t bytes = extent(fs, rs, n) * esz;
-        return dense(fs, rs, n) ? stg.out(p, bytes, d) : stg.inout(p, bytes, d);
+    auto stage_out = [&](auto* p, size_t fs, size_t rs, size_t n) {
+        const size_t count = extent(fs, rs, n);
+        return dense(fs, rs, n) ? stg.out(p, count) : stg.inout(p, count);
     };
     CloudArgs<T> a;
     a.dir = static_cast<const T*>(lut->dir);
@@ -776,37 +732,30 @@ static ob_status scan_to_cloud_t(const ob_lut* lut, const uint16_t* shift, const
     a.n_returns = static_cast<int>(R);
     a.n_frames = F;
     a.shift = shift;
-    const void* din = nullptr;
-    void* dout = nullptr;
-    cudaError_t e = stg.in(io->range, extent(a.range_fs, a.range_rs, n_px) * 4, &din);
-    if (e != cudaSuccess) return fail_cuda(e, "stage range");
-    a.range = static_cast<const uint32_t*>(din);
+    a.range = stg.in(io->range, extent(a.range_fs, a.range_rs, n_px));
+    if (cudaError_t e = stg.error()) return fail_cuda(e, "stage range");
     a.xyz = nullptr;
     a.rd = nullptr;
     a.xd = nullptr;
     if (io->xyz) {
-        e = stage_out(io->xyz, a.xyz_fs, a.xyz_rs, n_px * 3, sizeof(T), &dout);
-        if (e != cudaSuccess) return fail_cuda(e, "stage xyz");
-        a.xyz = static_cast<T*>(dout);
+        a.xyz = stage_out(static_cast<T*>(io->xyz), a.xyz_fs, a.xyz_rs, n_px * 3);
+        if (cudaError_t e = stg.error()) return fail_cuda(e, "stage xyz");
     }
     if (io->range_destaggered) {
-        e = stage_out(io->range_destaggered, a.rd_fs, a.rd_rs, n_px, 4, &dout);
-        if (e != cudaSuccess) return fail_cuda(e, "stage range_destaggered");
-        a.rd = static_cast<uint32_t*>(dout);
+        a.rd = stage_out(io->range_destaggered, a.rd_fs, a.rd_rs, n_px);
+        if (cudaError_t e = stg.error()) return fail_cuda(e, "stage range_destaggered");
     }
     if (io->xyz_destaggered) {
-        e = stage_out(io->xyz_destaggered, a.xd_fs, a.xd_rs, n_px * 3, sizeof(T), &dout);
-        if (e != cudaSuccess) return fail_cuda(e, "stage xyz_destaggered");
-        a.xd = static_cast<T*>(dout);
+        a.xd = stage_out(static_cast<T*>(io->xyz_destaggered), a.xd_fs, a.xd_rs, n_px * 3);
+        if (cudaError_t e = stg.error()) return fail_cuda(e, "stage xyz_destaggered");
     }
     if (io->poses) {
         const size_t pn = static_cast<size_t>(lut->w) * 16;
-        e = stg.in(io->poses, ((F - 1) * io->poses_frame_stride + pn) * sizeof(T), &din);
-        if (e != cudaSuccess) return fail_cuda(e, "stage poses");
-        a.poses = static_cast<const T*>(din);
+        a.poses = stg.in(static_cast<const T*>(io->poses), (F - 1) * io->poses_frame_stride + pn);
+        if (cudaError_t e = stg.error()) return fail_cuda(e, "stage poses");
         a.poses_fs = io->poses_frame_stride;
     }
-    e = launch_cloud<T>(a, s->device, s->st);
+    cudaError_t e = launch_cloud<T>(a, s->device, s->st);
     if (e != cudaSuccess) return fail_cuda(e, "scan_to_cloud launch");
     e = stg.flush();
     if (e != cudaSuccess) return fail_cuda(e, "scan_to_cloud D2H");
@@ -867,13 +816,12 @@ ob_status ob_dewarp(ob_dtype dtype, const void* points, const void* poses, size_
     if (rs != OB_OK) return rs;
     const size_t esz = dtype == OB_F64 ? 8 : 4;
     Staging stg(s->st);
-    const void *dp = nullptr, *dq = nullptr;
-    void* dout = nullptr;
-    cudaError_t e = stg.in(points, n_points * 3 * esz, &dp);
-    if (e == cudaSuccess) e = stg.in(poses, n_poses * 16 * esz, &dq);
-    if (e == cudaSuccess) e = stg.out(out, n_points * 3 * esz, &dout);
-    if (e != cudaSuccess) return fail_cuda(e, "stage dewarp buffers");
+    const void* dp = stg.in(points, n_points * 3 * esz);
+    const void* dq = stg.in(poses, n_poses * 16 * esz);
+    void* dout = stg.out(out, n_points * 3 * esz);
+    if (cudaError_t e = stg.error()) return fail_cuda(e, "stage dewarp buffers");
     const size_t H = n_points / n_poses;
+    cudaError_t e;
     if (dtype == OB_F64)
         e = launch_dewarp<double>(static_cast<const double*>(dp), static_cast<const double*>(dq),
                                   static_cast<double*>(dout), H, n_poses, s->st);
@@ -898,21 +846,19 @@ static ob_status run_dewarp(std::vector<K3Frame>& hf, int dtype, uint32_t min_r,
         max_slabs = std::max(max_slabs, f.n_slabs);
     }
     const size_t esz = dtype_size(dtype);
-    void *fdev = nullptr, *scan = nullptr;
-    cudaError_t e = stg.scratch(hf.size() * sizeof(K3Frame), &fdev);
-    if (e == cudaSuccess) e = stg.scratch(dewarp_scan_scratch_bytes(n_blocks, static_cast<unsigned>(hf.size())), &scan);
+    auto* fdev = stg.scratch<K3Frame>(hf.size());
+    void* scan = stg.scratch<void>(dewarp_scan_scratch_bytes(n_blocks, static_cast<unsigned>(hf.size())));
+    cudaError_t e = stg.error();
     if (e == cudaSuccess) e = cudaMemcpyAsync(fdev, hf.data(), hf.size() * sizeof(K3Frame), cudaMemcpyHostToDevice, s->st);
     if (e != cudaSuccess) return fail_cuda(e, "frame table upload");
-    void* dpts = nullptr;
-    uint32_t *dfi = nullptr, *dci = nullptr;
-    uint64_t* dts = nullptr;
-    e = res.array(points, 3 * esz, &dpts);
-    if (e == cudaSuccess) e = res.array(frame_idx, 4, &dfi);
-    if (e == cudaSuccess) e = res.array(col_idx, 4, &dci);
-    if (e == cudaSuccess) e = res.array(timestamps_out, 8, &dts);
+    void* dpts = res.array(points, 3 * esz);
+    uint32_t* dfi = res.array(frame_idx, 4);
+    uint32_t* dci = res.array(col_idx, 4);
+    uint64_t* dts = res.array(timestamps_out, 8);
+    e = stg.error();
     if (e != cudaSuccess) return fail_cuda(e, "stage dewarp outputs");
     const unsigned long long* fend = nullptr;
-    e = launch_dewarp_fused(static_cast<const K3Frame*>(fdev), static_cast<unsigned>(hf.size()), n_blocks, max_slabs,
+    e = launch_dewarp_fused(fdev, static_cast<unsigned>(hf.size()), n_blocks, max_slabs,
                             min_r, max_r, dtype, scan, dpts, dfi, dci, dts, capacity, &fend, s->st);
     if (e != cudaSuccess) return fail_cuda(e, "dewarp launch");
     if (res.on_device()) return res.finish(fend + (hf.size() - 1));
@@ -935,18 +881,11 @@ static ob_status stage_k3_frame(const ob_lut* lut, const uint32_t* range, const 
     f.dir = lut->dir;
     f.off = lut->off;
     const size_t n_px = lut->h * lut->w;
-    const void* d = nullptr;
-    cudaError_t e = stg.in(range, n_px * 4, &d);
-    f.range = static_cast<const uint32_t*>(d);
-    if (e == cudaSuccess) e = stg.in(poses, lut->w * 16 * sizeof(double), &d);
-    f.poses = static_cast<const double*>(d);
-    if (e == cudaSuccess) e = stg.in(status, lut->w * 4, &d);
-    f.status = static_cast<const uint32_t*>(d);
-    if (e == cudaSuccess && want_ts) {
-        e = stg.in(timestamps, lut->w * 8, &d);
-        f.timestamps = static_cast<const uint64_t*>(d);
-    }
-    if (e != cudaSuccess) return fail_cuda(e, "stage dewarp inputs");
+    f.range = stg.in(range, n_px);
+    f.poses = stg.in(poses, lut->w * 16);
+    f.status = stg.in(status, lut->w);
+    if (want_ts) f.timestamps = stg.in(timestamps, lut->w);
+    if (cudaError_t e = stg.error()) return fail_cuda(e, "stage dewarp inputs");
     *out = f;
     return OB_OK;
 }
@@ -1045,14 +984,12 @@ ob_status ob_destagger(size_t elem_size, size_t k, const void* img, const int32_
     reduce_shifts(shifts, h, w, inverse, sh);
     const size_t bytes = h * w * k * elem_size;
     Staging stg(s->st);
-    const void* din = nullptr;
-    void* dout = nullptr;
-    cudaError_t e = stg.in(img, bytes, &din);
-    if (e != cudaSuccess) return fail_cuda(e, "stage image");
-    e = stg.out(out, bytes, &dout);
-    if (e != cudaSuccess) return fail_cuda(e, "stage output");
+    const void* din = stg.in(img, bytes);
+    if (cudaError_t e = stg.error()) return fail_cuda(e, "stage image");
+    void* dout = stg.out(out, bytes);
+    if (cudaError_t e = stg.error()) return fail_cuda(e, "stage output");
     if (din == dout) return fail(OB_INVALID_ARGUMENT, "image and destaggered must not alias");
-    e = launch_destagger(elem_size, k, din, sh.data(), h, w, dout, s->device, s->st);
+    cudaError_t e = launch_destagger(elem_size, k, din, sh.data(), h, w, dout, s->device, s->st);
     if (e != cudaSuccess) return fail_cuda(e, "destagger launch");
     e = stg.flush();
     if (e != cudaSuccess) return fail_cuda(e, "destagger D2H");

@@ -2,6 +2,7 @@
 #pragma once
 #include <initializer_list>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "ob_internal.h"
@@ -14,31 +15,61 @@ ob_status require_device(int device);
 bool is_device_ptr(const void* p);
 void reduce_shifts(const int32_t* shifts, size_t h, size_t w, int inverse, std::vector<uint16_t>& out);
 
-// Per-call staging of host buffers through stream-ordered device scratch.
-// in():  host -> scratch (H2D issued immediately); device pointers pass through.
-// out(): scratch now, D2H issued by flush() after the kernel; device pointers pass through.
+// Per-call staging of host buffers through stream-ordered device scratch.  Sizes count elements of T (bytes when T
+// is void); a null pointer, a device pointer or a zero-size request is returned as is.
+// in():  host -> scratch (H2D issued immediately).
+// out(): scratch now, D2H issued by flush() after the kernel.
 // inout(): as out(), but the host contents are uploaded first, so bytes the kernel leaves alone
 //          (padding between strided frames) come back unchanged.
+// scratch(): device memory for the call, freed in stream order when the Staging goes (at least 16 bytes).
+// The first CUDA error of the call is kept: error() returns it, and from then on in / out / inout / scratch return
+// null and make no CUDA call, and flush() / finish() return it.  check() records an error met outside the Staging.
 class Staging {
    public:
     explicit Staging(cudaStream_t st) : st_(st) {}
     ~Staging();
-    cudaError_t in(const void* p, size_t bytes, const void** dev);
-    cudaError_t out(void* p, size_t bytes, void** dev);
-    cudaError_t inout(void* p, size_t bytes, void** dev);
-    cudaError_t scratch(size_t bytes, void** dev);
+    cudaError_t error() const { return err_; }
+    cudaError_t check(cudaError_t e) {
+        if (err_ == cudaSuccess) err_ = e;
+        return err_;
+    }
+    template <typename T>
+    const T* in(const T* p, size_t n) {
+        return static_cast<const T*>(stage(p, n * elem_bytes<T>(), true, false));
+    }
+    template <typename T>
+    T* out(T* p, size_t n) {
+        return static_cast<T*>(stage(p, n * elem_bytes<T>(), false, true));
+    }
+    template <typename T>
+    T* inout(T* p, size_t n) {
+        return static_cast<T*>(stage(p, n * elem_bytes<T>(), true, true));
+    }
+    template <typename T>
+    T* scratch(size_t n) {
+        return static_cast<T*>(scratch_bytes(n * elem_bytes<T>()));
+    }
     cudaError_t flush();
     // flush(), then wait for the stream if that issued a D2H: host results are final on return, and a call whose
     // outputs are all device memory waits for nothing (and stays capturable in a CUDA graph)
     cudaError_t finish();
 
    private:
+    template <typename T>
+    static constexpr size_t elem_bytes() {
+        if constexpr (std::is_void_v<T>) return 1;
+        else return sizeof(T);
+    }
+    // scratch for a host buffer, filled from it (upload) and copied back to it by flush() (download)
+    void* stage(const void* p, size_t bytes, bool upload, bool download);
+    void* scratch_bytes(size_t bytes);
     struct Pending {
         void* host;
         void* dev;
         size_t bytes;
     };
     cudaStream_t st_;
+    cudaError_t err_ = cudaSuccess;
     std::vector<void*> scratch_;
     std::vector<Pending> pending_;
 };
@@ -49,7 +80,7 @@ class Staging {
 //  - A device count needs every array in device memory; refuse() turns a host array away (count 0) before anything
 //    is staged or launched.
 //  - array(): a device array is written in place, a host array through scratch of `capacity` rows, a null array is
-//    not written (count only).
+//    not written (count only).  array() and word() allocate through the call's Staging and return null after an error.
 //  - finish(): with a device count nothing waits, rows past `capacity` are cut and the count is the true total.  With
 //    a host count the call waits for the count; more rows than `capacity` fail "output capacity too small" with the
 //    count left 0 and the host rows untouched; otherwise it waits again for the rows of the host arrays.
@@ -60,16 +91,13 @@ class CountedRows {
     bool on_device() const { return dev_; }
     ob_status zero();
     ob_status refuse(std::initializer_list<const void*> arrays, const char* msg);
-    cudaError_t array(void* p, size_t row_bytes, void** dev);
+    void* array(void* p, size_t row_bytes);
     template <typename T>
-    cudaError_t array(T* p, size_t row_bytes, T** dev) {
-        void* d = nullptr;
-        cudaError_t e = array(static_cast<void*>(p), row_bytes, &d);
-        *dev = static_cast<T*>(d);
-        return e;
+    T* array(T* p, size_t row_bytes) {
+        return static_cast<T*>(array(static_cast<void*>(p), row_bytes));
     }
     // the device word the kernel writes the count to: the caller's device count, or scratch
-    cudaError_t word(unsigned long long** w);
+    unsigned long long* word();
     // after the launch; `end`: the device word holding the count
     ob_status finish(const unsigned long long* end);
     // finish() in two steps for a host count: read k device words (the last is the count) with one wait, then deliver

@@ -306,27 +306,21 @@ ob_status ob_decode_frames(const ob_decoder* dec, const ob_decode_io* frames, si
         CallLut frame_lut;
         if (io.lut && (rs = take_lut(c, io.lut, &frame_lut)) != OB_OK) return rs;
         if ((rs = check_fused(c, lut || io.lut, io.xyz, io.range_destaggered)) != OB_OK) return rs;
-        const void* d = nullptr;
-        cudaError_t e = cudaSuccess;
         if (io.n_slots > 0) {
-            e = stg.in(io.packets, (io.n_slots - 1) * io.packet_stride + L.packet_size, &d);
-            if (e != cudaSuccess) return fail_cuda(e, "stage packets");
+            f.packets = stg.in(io.packets, (io.n_slots - 1) * io.packet_stride + L.packet_size);
+            if (cudaError_t e = stg.error()) return fail_cuda(e, "stage packets");
         }
-        f.packets = static_cast<const uint8_t*>(d);
         f.packet_stride = io.packet_stride;
         f.n_slots = static_cast<uint32_t>(io.n_slots);
         if (io.col_src) {
-            e = stg.in(io.col_src, static_cast<size_t>(L.W) * 4, &d);
-            if (e != cudaSuccess) return fail_cuda(e, "stage column map");
-            f.col_src = static_cast<const int32_t*>(d);
+            f.col_src = stg.in(io.col_src, L.W);
+            if (cudaError_t e = stg.error()) return fail_cuda(e, "stage column map");
         }
         for (int k = 0; k < kOuts; ++k) {
             void* user = io_out(L, io, k);
             if (!user) continue;
-            void* o = nullptr;
-            e = stg.out(user, out_bytes(L, c.dtype, k), &o);
-            if (e != cudaSuccess) return fail_cuda(e, "stage outputs");
-            set_out(f, k, o);
+            set_out(f, k, stg.out(user, out_bytes(L, c.dtype, k)));
+            if (cudaError_t e = stg.error()) return fail_cuda(e, "stage outputs");
         }
         const bool bulk_ok = f.packets && al16(f.packets) && io.packet_stride % 16 == 0 && L.packet_size % 16 == 0;
         finish_frame(c, f, bulk_ok, io.lut ? &frame_lut : nullptr);
@@ -356,17 +350,15 @@ ob_status ob_decode_batch_run(const ob_decoder* dec, const ob_decode_batch* b, c
 
     Staging stg(stream_handle(s));
     auto span = [&](size_t stride, size_t last) { return (F - 1) * stride + last; };
-    const void* dpk = nullptr;
-    cudaError_t e = stg.in(b->packets,
-                           span(b->packets_frame_stride, (b->n_slots - 1) * b->packet_stride + L.packet_size),
-                           &dpk);
-    if (e != cudaSuccess) return fail_cuda(e, "stage packets");
+    const uint8_t* dpk =
+        stg.in(b->packets, span(b->packets_frame_stride, (b->n_slots - 1) * b->packet_stride + L.packet_size));
+    if (cudaError_t e = stg.error()) return fail_cuda(e, "stage packets");
     void* dout[kOuts] = {};  // frame 0's outputs
     for (int k = 0; k < kOuts; ++k) {
         void* user = io_out(L, *b, k);
         if (!user) continue;
-        e = stg.out(user, span(batch_stride(*b, k), out_bytes(L, c.dtype, k)), &dout[k]);
-        if (e != cudaSuccess) return fail_cuda(e, "stage outputs");
+        dout[k] = stg.out(user, span(batch_stride(*b, k), out_bytes(L, c.dtype, k)));
+        if (cudaError_t e = stg.error()) return fail_cuda(e, "stage outputs");
     }
     const bool bulk_ok = al16(dpk) && b->packet_stride % 16 == 0 && L.packet_size % 16 == 0 &&
                          b->packets_frame_stride % 16 == 0;
@@ -374,7 +366,7 @@ ob_status ob_decode_batch_run(const ob_decoder* dec, const ob_decode_batch* b, c
     for (size_t f = 0; f < F; ++f) {
         DecodeFrame& d = hf[f];
         std::memset(&d, 0, sizeof(d));
-        d.packets = static_cast<const uint8_t*>(dpk) + f * b->packets_frame_stride;
+        d.packets = dpk + f * b->packets_frame_stride;
         d.packet_stride = b->packet_stride;
         d.n_slots = static_cast<uint32_t>(b->n_slots);
         for (int k = 0; k < kOuts; ++k)
@@ -660,34 +652,19 @@ ob_status ob_encode_frames(const ob_decoder* dec, const ob_encode_io* frames, si
             return fail(OB_INVALID_ARGUMENT, "packet_stride smaller than the lidar packet size");
         if (io.packet_headers && io.packet_header_bytes < L.packet_header_size)
             return fail(OB_INVALID_ARGUMENT, "packet_header_bytes smaller than the packet header");
-        const void* d = nullptr;
-        cudaError_t e = cudaSuccess;
-        for (uint32_t k = 0; k < L.n_fields && e == cudaSuccess; ++k) {
-            if (!io.fields[k]) continue;
-            e = stg.in(io.fields[k], out_bytes(L, OB_F32, k), &d);
-            f.fields[k] = d;
-        }
-        if (e == cudaSuccess && io.timestamp) {
-            e = stg.in(io.timestamp, out_bytes(L, OB_F32, kOutTs), &d);
-            f.timestamp = static_cast<const uint64_t*>(d);
-        }
-        if (e == cudaSuccess && io.status) {
-            e = stg.in(io.status, out_bytes(L, OB_F32, kOutStatus), &d);
-            f.status = static_cast<const uint32_t*>(d);
-        }
-        if (e == cudaSuccess && io.packet_headers) {
-            e = stg.in(io.packet_headers, n_pk * io.packet_header_bytes, &d);
-            f.packet_headers = static_cast<const uint8_t*>(d);
+        for (uint32_t k = 0; k < L.n_fields; ++k)
+            if (io.fields[k]) f.fields[k] = stg.in(io.fields[k], out_bytes(L, OB_F32, k));
+        if (io.timestamp) f.timestamp = stg.in(io.timestamp, L.W);
+        if (io.status) f.status = stg.in(io.status, L.W);
+        if (io.packet_headers) {
+            f.packet_headers = stg.in(io.packet_headers, n_pk * io.packet_header_bytes);
             f.header_bytes = static_cast<uint32_t>(io.packet_header_bytes);
         }
         // the kernel writes packet_size bytes of every packet_stride; a host buffer with gaps between packets is
         // uploaded first so that its copy back leaves the gaps as the caller had them
-        void* o = nullptr;
         const size_t span = (n_pk - 1) * io.packet_stride + L.packet_size;
-        if (e == cudaSuccess)
-            e = io.packet_stride == L.packet_size ? stg.out(io.packets, span, &o) : stg.inout(io.packets, span, &o);
-        if (e != cudaSuccess) return fail_cuda(e, "stage encode buffers");
-        f.packets = static_cast<uint8_t*>(o);
+        f.packets = io.packet_stride == L.packet_size ? stg.out(io.packets, span) : stg.inout(io.packets, span);
+        if (cudaError_t e = stg.error()) return fail_cuda(e, "stage encode buffers");
         f.packet_stride = io.packet_stride;
     }
     const void* fdev = nullptr;

@@ -437,12 +437,11 @@ ob_status ob_frame_mask_fields(const ob_frame_ops_io* io, ob_stream* s) {
     if (npx == 0 || a.n_frames == 0 || a.n_fields == 0) return OB_OK;
     cudaStream_t st = stream_handle(s);
     Staging stg(st);
-    cudaError_t e = cudaSuccess;
     bool host_io = false;
     // stage host buffers: targets in and out, sources in
     std::vector<MaskEntry> ents;
     std::vector<uint32_t> fbeg(a.n_frames + 1, 0);
-    for (uint32_t f = 0; f < a.n_frames && e == cudaSuccess; ++f) {
+    for (uint32_t f = 0; f < a.n_frames && !stg.error(); ++f) {
         fbeg[f] = uint32_t(ents.size());
         for (MaskEntry m : per_frame[f]) {
             const bool src = m.role == OB_FRAME_SOURCE || m.role == OB_FRAME_SOURCE2;
@@ -451,25 +450,17 @@ ob_status ob_frame_mask_fields(const ob_frame_ops_io* io, ob_stream* s) {
                                             : m.esize);
             if (!is_device_ptr(m.data)) {
                 host_io |= !src;
-                if (src) {
-                    const void* d = nullptr;
-                    e = stg.in(m.data, bytes, &d);
-                    m.data = const_cast<void*>(d);
-                } else {
-                    void* d = nullptr;
-                    e = stg.inout(m.data, bytes, &d);
-                    m.data = d;
-                }
+                m.data = src ? const_cast<void*>(stg.in(m.data, bytes)) : stg.inout(m.data, bytes);
             }
             ents.push_back(m);
         }
     }
     fbeg[a.n_frames] = uint32_t(ents.size());
-    if (e != cudaSuccess) return fail_cuda(e, "stage frame fields");
+    if (cudaError_t e = stg.error()) return fail_cuda(e, "stage frame fields");
     const void* dposes = nullptr;
     if (a.predicate == OB_FRAME_XYZ_RANGE && a.poses) {
-        e = stg.in(a.poses, size_t(a.n_frames) * a.w * 16 * (lut.dtype == OB_F64 ? 8 : 4), &dposes);
-        if (e != cudaSuccess) return fail_cuda(e, "stage poses");
+        dposes = stg.in(a.poses, size_t(a.n_frames) * a.w * 16 * (lut.dtype == OB_F64 ? 8 : 4));
+        if (cudaError_t e = stg.error()) return fail_cuda(e, "stage poses");
     }
     std::vector<uint16_t> sh;
     if (a.predicate == OB_FRAME_COLS) reduce_shifts(a.pixel_shift_by_row, a.h, a.w, 0, sh);
@@ -492,6 +483,7 @@ ob_status ob_frame_mask_fields(const ob_frame_ops_io* io, ob_stream* s) {
         for (size_t r = 0; r < sh.size(); ++r) p.shift[r] = sh[r];
     };
     constexpr int kSmall = 32, kLarge = 512;
+    cudaError_t e = cudaSuccess;
     if (ents.size() <= size_t(kSmall) && a.n_frames <= uint32_t(kSmall)) {
         auto p = std::make_unique<MaskParams<kSmall>>();
         fill(*p);
@@ -507,7 +499,8 @@ ob_status ob_frame_mask_fields(const ob_frame_ops_io* io, ob_stream* s) {
             f0 = f1;
         }
     }
-    if (e == cudaSuccess) e = stg.flush();
+    stg.check(e);
+    e = stg.flush();
     if (e == cudaSuccess && host_io) e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail_cuda(e, "frame mask");
     return OB_OK;
@@ -530,38 +523,35 @@ ob_status ob_frame_select_rows(const ob_frame_rows_io* io, ob_stream* s) {
     if (a.n_entries == 0 || a.n_rows == 0) return OB_OK;
     cudaStream_t st = stream_handle(s);
     Staging stg(st);
-    cudaError_t e = cudaSuccess;
     bool host_io = false;
     std::vector<RowEntry> ents;
     uint32_t max_units = 0;
-    for (uint32_t i = 0; i < a.n_entries && e == cudaSuccess; ++i) {
+    for (uint32_t i = 0; i < a.n_entries && !stg.error(); ++i) {
         const ob_frame_rows_entry& r = a.entries[i];
         if (!r.row_bytes) continue;
         RowEntry x{r.src, r.dst, uint32_t(r.row_bytes), 1};
-        if (!is_device_ptr(r.src)) {
-            const void* d = nullptr;
-            e = stg.in(r.src, r.src_rows * r.row_bytes, &d);
-            x.src = d;
-        }
-        if (e == cudaSuccess && !is_device_ptr(r.dst)) {
+        if (!is_device_ptr(r.src)) x.src = stg.in(r.src, r.src_rows * r.row_bytes);
+        if (!stg.error() && !is_device_ptr(r.dst)) {
             host_io = true;
-            e = stg.out(r.dst, size_t(a.n_rows) * r.row_bytes, &x.dst);
+            x.dst = stg.out(r.dst, size_t(a.n_rows) * r.row_bytes);
         }
         const uintptr_t al = reinterpret_cast<uintptr_t>(x.src) | reinterpret_cast<uintptr_t>(x.dst) | x.row_bytes;
         x.unit = (al & 15) == 0 ? 16 : (al & 7) == 0 ? 8 : (al & 3) == 0 ? 4 : (al & 1) == 0 ? 2 : 1;
         max_units = std::max(max_units, uint32_t(std::min<size_t>(size_t(x.row_bytes / x.unit) * a.n_rows, 0xffffffffu)));
         ents.push_back(x);
     }
-    if (e != cudaSuccess) return fail_cuda(e, "stage frame rows");
+    if (cudaError_t e = stg.error()) return fail_cuda(e, "stage frame rows");
     constexpr int kCap = 768;   // 18 KB of entries + 8 KB of rows: within the 32 KB parameter limit
     auto p = std::make_unique<RowParams<kCap>>();
     p->n_rows = a.n_rows;
     for (uint32_t k = 0; k < a.n_rows; ++k) p->rows[k] = a.rows[k];
+    cudaError_t e = cudaSuccess;
     for (size_t b = 0; b < ents.size() && e == cudaSuccess; b += kCap) {
         const uint32_t n = uint32_t(std::min<size_t>(kCap, ents.size() - b));
         e = launch_rows(*p, ents.data() + b, n, st, max_units);
     }
-    if (e == cudaSuccess) e = stg.flush();
+    stg.check(e);
+    e = stg.flush();
     if (e == cudaSuccess && host_io) e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail_cuda(e, "frame select rows");
     return OB_OK;

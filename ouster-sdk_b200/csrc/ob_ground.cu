@@ -17,14 +17,12 @@
 //   fill (6)  smooth  prune  fill (6)  smooth  components  fill (3)  -- Jacobi passes, one launch each (prune: one
 //                                                                      CTA per frame, level-synchronous BFS)
 //   classify     one thread per pixel per return
-#include <cub/device/device_radix_sort.cuh>
-#include <cub/device/device_scan.cuh>
-
 #include <algorithm>
 #include <cmath>
 #include <vector>
 
 #include "ob_api_common.h"
+#include "ob_cub.cuh"
 #include "ob_project.cuh"
 
 namespace ob {
@@ -903,26 +901,6 @@ unsigned blocks_for(unsigned long long n, unsigned threads) {
     return static_cast<unsigned>(std::max<unsigned long long>(1, std::min<unsigned long long>(b, 1u << 16)));
 }
 
-int bits_for(unsigned long long v) {  // radix bits that hold 0..v
-    int b = 1;
-    while (b < 64 && (v >> b) != 0) ++b;
-    return b;
-}
-
-template <typename K, typename V>
-cudaError_t sort_pairs(Staging& stg, const K* kin, K* kout, const V* vin, V* vout, unsigned long long n, int end_bit,
-                       cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    size_t bytes = 0;
-    cudaError_t e = cub::DeviceRadixSort::SortPairs(nullptr, bytes, kin, kout, vin, vout, static_cast<int64_t>(n), 0,
-                                                    end_bit, st);
-    void* tmp = nullptr;
-    if (e == cudaSuccess) e = stg.scratch(bytes, &tmp);
-    if (e == cudaSuccess)
-        e = cub::DeviceRadixSort::SortPairs(tmp, bytes, kin, kout, vin, vout, static_cast<int64_t>(n), 0, end_bit, st);
-    return e;
-}
-
 // the root of each height-sorted cell (n_cells for cells outside every component), for the stable sort by root
 __global__ void root_keys_kernel(const unsigned long long* hk_sorted, const uint32_t* cells, const uint32_t* parent,
                                  uint32_t* roots, unsigned long long n, uint32_t n_cells) {
@@ -981,8 +959,7 @@ extern "C" ob_status ob_ground_mask(const ob_ground_item* items, size_t n_items,
     std::vector<size_t> rbase;
     unsigned long long P = 0;
     unsigned max_slots = 0, max_px = 0;
-    cudaError_t e = cudaSuccess;
-    for (size_t i = 0; i < n_items && e == cudaSuccess; ++i) {
+    for (size_t i = 0; i < n_items && !stg.error(); ++i) {
         const ob_ground_item& it = items[i];
         if (!it.lut || it.h * it.w == 0) continue;
         const LutView lv = lut_view(it.lut);
@@ -995,28 +972,17 @@ extern "C" ob_status ob_ground_mask(const ob_ground_item* items, size_t n_items,
         f.n_ret = static_cast<unsigned>(it.n_returns);
         f.n_model = it.n_returns >= 2 ? 2 : 1;
         rbase.push_back(rtab.size());
-        for (size_t r = 0; r < it.n_returns && e == cudaSuccess; ++r) {
-            const void* d = nullptr;
-            e = stg.in(it.range[r], npx * 4, &d);
-            rtab.push_back(static_cast<const uint32_t*>(d));
-            void* m = nullptr;
-            if (e == cudaSuccess) e = stg.out(it.masks[r], npx, &m);
-            mtab.push_back(static_cast<uint8_t*>(m));
+        for (size_t r = 0; r < it.n_returns; ++r) {
+            rtab.push_back(stg.in(it.range[r], npx));
+            mtab.push_back(stg.out(it.masks[r], npx));
         }
         for (unsigned r = 0; r < f.n_model; ++r) f.range[r] = rtab[rbase.back() + r];
-        const void* d = nullptr;
-        if (e == cudaSuccess) e = stg.in(it.status, it.w * 4, &d);
-        f.status = static_cast<const uint32_t*>(d);
-        if (e == cudaSuccess) e = stg.in(it.poses, it.w * 128, &d);
-        f.poses = static_cast<const double*>(d);
+        f.status = stg.in(it.status, it.w);
+        f.poses = stg.in(it.poses, it.w * 16);
         // NORMALS2 is read only alongside NORMALS, and only for a second return
-        if (e == cudaSuccess && it.normals) e = stg.in(it.normals, npx * 12, &d), f.nrm[0] = static_cast<const float*>(d);
-        if (e == cudaSuccess && it.normals && it.normals2 && f.n_model == 2)
-            e = stg.in(it.normals2, npx * 12, &d), f.nrm[1] = static_cast<const float*>(d);
-        if (e == cudaSuccess && it.compute_normals && !it.normals) {
-            e = stg.in(it.sensor_to_body, 128, &d);
-            f.sensor_to_body = static_cast<const double*>(d);
-        }
+        if (it.normals) f.nrm[0] = stg.in(it.normals, npx * 3);
+        if (it.normals && it.normals2 && f.n_model == 2) f.nrm[1] = stg.in(it.normals2, npx * 3);
+        if (it.compute_normals && !it.normals) f.sensor_to_body = stg.in(it.sensor_to_body, 16);
         f.pt_off = P;
         P += static_cast<unsigned long long>(f.n_model) * npx;
         max_slots = std::max<unsigned>(max_slots, static_cast<unsigned>(f.n_model * npx));
@@ -1024,34 +990,28 @@ extern "C" ob_status ob_ground_mask(const ob_ground_item* items, size_t n_items,
         frames.push_back(f);
         slot_of.push_back(i);
     }
-    if (e != cudaSuccess) return fail_cuda(e, "stage ground buffers");
+    if (cudaError_t e = stg.error()) return fail_cuda(e, "stage ground buffers");
     const unsigned F = static_cast<unsigned>(frames.size());
     if (F == 0) return OB_OK;
     if (F > 65535) return fail(OB_INVALID_ARGUMENT, "too many frames in one call");
     if (P >= 0xffffffffull) return fail(OB_INVALID_ARGUMENT, "frame set too large");
     // the device tables of range and mask pointers
-    const void* drt = nullptr;
-    const void* dmt = nullptr;
-    e = stg.in(rtab.data(), rtab.size() * sizeof(void*), &drt);
-    if (e == cudaSuccess) e = stg.in(mtab.data(), mtab.size() * sizeof(void*), &dmt);
+    const uint32_t* const* drt = stg.in(rtab.data(), rtab.size());
+    uint8_t* const* dmt = stg.in(mtab.data(), mtab.size());
     for (unsigned k = 0; k < F; ++k) {
-        frames[k].ranges = static_cast<const uint32_t* const*>(drt) + rbase[k];
-        frames[k].masks = static_cast<uint8_t* const*>(dmt) + rbase[k];
+        frames[k].ranges = drt + rbase[k];
+        frames[k].masks = dmt + rbase[k];
     }
-    void* dframes = nullptr;
-    void* dstate = nullptr;
-    void *pts = nullptr, *nflag = nullptr, *keys = nullptr, *keys2 = nullptr, *keys3 = nullptr, *grp = nullptr,
-         *grp2 = nullptr;
     const unsigned long long P2 = 2 * P;
-    if (e == cudaSuccess) e = stg.scratch(F * sizeof(GFrame), &dframes);
-    if (e == cudaSuccess) e = stg.scratch(F * sizeof(GState), &dstate);
-    if (e == cudaSuccess) e = stg.scratch(P * 24, &pts);
-    if (e == cudaSuccess) e = stg.scratch(P, &nflag);
-    if (e == cudaSuccess) e = stg.scratch(P2 * 8, &keys);
-    if (e == cudaSuccess) e = stg.scratch(P2 * 8, &keys2);
-    if (e == cudaSuccess) e = stg.scratch(P2 * 8, &keys3);
-    if (e == cudaSuccess) e = stg.scratch(P2 * 4, &grp);
-    if (e == cudaSuccess) e = stg.scratch(P2 * 4, &grp2);
+    auto* df = stg.scratch<GFrame>(F);
+    auto* gs = stg.scratch<GState>(F);
+    auto* pts = stg.scratch<double>(P * 3);
+    auto* nflag = stg.scratch<uint8_t>(P);
+    auto* k1 = stg.scratch<unsigned long long>(P2);
+    auto* k2 = stg.scratch<unsigned long long>(P2);
+    auto* k3 = stg.scratch<unsigned long long>(P2);
+    auto* u1 = stg.scratch<uint32_t>(P2);
+    auto* u2 = stg.scratch<uint32_t>(P2);
     // computed normals: frames of one shape and return count form one batch of ob_normals
     struct NormalsBatch {
         unsigned H, W, n_model;
@@ -1079,15 +1039,14 @@ extern "C" ob_status ob_ground_mask(const ob_ground_item* items, size_t n_items,
     }
     for (NormalsBatch& b : batches) {
         const size_t nb = b.frames.size(), hw = static_cast<size_t>(b.H) * b.W;
-        void* q = nullptr;
         for (unsigned r = 0; r < b.n_model; ++r) {
-            if (e == cudaSuccess) e = stg.scratch(nb * hw * 24, &q), b.xyz[r] = static_cast<double*>(q);
-            if (e == cudaSuccess) e = stg.scratch(nb * hw * 24, &q), b.out[r] = static_cast<double*>(q);
-            if (e == cudaSuccess) e = stg.scratch(nb * hw * 4, &q), b.range[r] = static_cast<uint32_t*>(q);
+            b.xyz[r] = stg.scratch<double>(nb * hw * 3);
+            b.out[r] = stg.scratch<double>(nb * hw * 3);
+            b.range[r] = stg.scratch<uint32_t>(nb * hw);
         }
-        if (e == cudaSuccess) e = stg.scratch(nb * b.W * 24, &q), b.origins = static_cast<double*>(q);
-        if (e == cudaSuccess) e = stg.scratch(nb * 8, &q), b.subtent = static_cast<double*>(q);
-        if (e != cudaSuccess) break;
+        b.origins = stg.scratch<double>(nb * b.W * 3);
+        b.subtent = stg.scratch<double>(nb);
+        if (stg.error()) break;
         for (size_t j = 0; j < nb; ++j) {
             GFrame& f = frames[b.frames[j]];
             for (unsigned r = 0; r < b.n_model; ++r) {
@@ -1098,11 +1057,11 @@ extern "C" ob_status ob_ground_mask(const ob_ground_item* items, size_t n_items,
             f.norigin = b.origins + j * b.W * 3;
         }
     }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(dframes, frames.data(), F * sizeof(GFrame), cudaMemcpyHostToDevice, st);
+    cudaError_t e = stg.error();
+    if (e == cudaSuccess) e = cudaMemcpyAsync(df, frames.data(), F * sizeof(GFrame), cudaMemcpyHostToDevice, st);
     if (e != cudaSuccess) return fail_cuda(e, "stage ground buffers");
     if (!batches.empty()) {
-        launch(OB_FAM_GROUND, normals_input_kernel, dim3(blocks_for(max_norm, kThreads), F), kThreads, 0, st,
-               static_cast<const GFrame*>(dframes));
+        launch(OB_FAM_GROUND, normals_input_kernel, dim3(blocks_for(max_norm, kThreads), F), kThreads, 0, st, df);
         e = cudaGetLastError();
         if (e != cudaSuccess) return fail_cuda(e, "ground normals");
         for (const NormalsBatch& b : batches) {  // the reference's normals() defaults (normals.h:23-25)
@@ -1125,23 +1084,16 @@ extern "C" ob_status ob_ground_mask(const ob_ground_item* items, size_t n_items,
             if (ns != OB_OK) return ns;
         }
     }
-    const GFrame* df = static_cast<const GFrame*>(dframes);
-    GState* gs = static_cast<GState*>(dstate);
-    auto* k1 = static_cast<unsigned long long*>(keys);
-    auto* k2 = static_cast<unsigned long long*>(keys2);
-    auto* k3 = static_cast<unsigned long long*>(keys3);
-    auto* u1 = static_cast<uint32_t*>(grp);
-    auto* u2 = static_cast<uint32_t*>(grp2);
 
     // pass 1 and 2: points, extents, the per-frame sorts, the header
     launch(OB_FAM_GROUND, span_kernel, F, kThreads, 0, st, df, gs);
-    launch(OB_FAM_GROUND, points_kernel, dim3(blocks_for(max_slots, kThreads), F), kThreads, 0, st, df, gs,
-           static_cast<double*>(pts), static_cast<uint8_t*>(nflag), k1, u1, P, F);
-    e = cudaGetLastError();
+    launch(OB_FAM_GROUND, points_kernel, dim3(blocks_for(max_slots, kThreads), F), kThreads, 0, st, df, gs, pts, nflag,
+           k1, u1, P, F);
+    stg.check(cudaGetLastError());
     // (frame, value) order: stable sort by value, then by group (z groups 0..F-1, footprint groups F..2F-1)
-    if (e == cudaSuccess) e = sort_pairs(stg, k1, k2, u1, u2, P2, 64, st);
-    if (e == cudaSuccess) e = sort_pairs(stg, u2, u1, k2, k3, P2, bits_for(2ull * F), st);
-    if (e != cudaSuccess) return fail_cuda(e, "ground points");
+    cub_run(stg, sort_pairs(k1, k2, u1, u2, static_cast<int64_t>(P2), 0, 64, st));
+    cub_run(stg, sort_pairs(u2, u1, k2, k3, static_cast<int64_t>(P2), 0, bits_for(2ull * F), st));
+    if (cudaError_t e = stg.error()) return fail_cuda(e, "ground points");
     launch(OB_FAM_GROUND, header_kernel, (F + 63) / 64, 64, 0, st, df, gs, static_cast<const unsigned long long*>(k3),
            P, F, grid_size);
     e = cudaGetLastError();
@@ -1165,35 +1117,30 @@ extern "C" ob_status ob_ground_mask(const ob_ground_item* items, size_t n_items,
         max_cells = std::max(max_cells, cells);
     }
     if (C >= 0x7fffffffull) return fail(OB_INVALID_ARGUMENT, "ground grid too large");
-    e = cudaMemcpyAsync(dframes, frames.data(), F * sizeof(GFrame), cudaMemcpyHostToDevice, st);
+    e = cudaMemcpyAsync(df, frames.data(), F * sizeof(GFrame), cudaMemcpyHostToDevice, st);
     if (e != cudaSuccess) return fail_cuda(e, "ground grid offsets");
     const uint32_t nC = static_cast<uint32_t>(C);
 
     // grids: the model, a second (Jacobi) copy of valid / height / roughness, and the pass scratch
     Grid g{}, g2{};
-    void *cbeg = nullptr, *cend = nullptr, *zs = nullptr, *fz = nullptr, *flags = nullptr, *scan = nullptr,
-         *ckeys = nullptr;
-    auto alloc = [&](size_t bytes, void** p) {
-        if (e == cudaSuccess) e = stg.scratch(bytes, p);
-    };
-    void* p = nullptr;
-    alloc(C + 1, &p), g.valid = static_cast<uint8_t*>(p);
-    alloc(C + 1, &p), g.obstacle = static_cast<uint8_t*>(p);
-    alloc((C + 1) * 8, &p), g.floor_z = static_cast<double*>(p);
-    alloc((C + 1) * 8, &p), g.height = static_cast<double*>(p);
-    alloc((C + 1) * 8, &p), g.rough = static_cast<double*>(p);
-    alloc(C + 1, &p), g2.valid = static_cast<uint8_t*>(p);
-    alloc((C + 1) * 8, &p), g2.height = static_cast<double*>(p);
-    alloc((C + 1) * 8, &p), g2.rough = static_cast<double*>(p);
+    g.valid = stg.scratch<uint8_t>(C + 1);
+    g.obstacle = stg.scratch<uint8_t>(C + 1);
+    g.floor_z = stg.scratch<double>(C + 1);
+    g.height = stg.scratch<double>(C + 1);
+    g.rough = stg.scratch<double>(C + 1);
+    g2.valid = stg.scratch<uint8_t>(C + 1);
+    g2.height = stg.scratch<double>(C + 1);
+    g2.rough = stg.scratch<double>(C + 1);
     g2.obstacle = g.obstacle;
     g2.floor_z = g.floor_z;
-    alloc((C + 1) * 4, &cbeg);
-    alloc((C + 1) * 4, &cend);
-    alloc(P * 8, &zs);
-    alloc(P * 8, &fz);
-    alloc((P + 1) * 4, &flags);
-    alloc((P + 1) * 4, &scan);
-    alloc(P * 4, &ckeys);
+    auto* cbeg = stg.scratch<uint32_t>(C + 1);
+    auto* cend = stg.scratch<uint32_t>(C + 1);
+    auto* zs = stg.scratch<double>(P);
+    auto* fz = stg.scratch<double>(P);
+    auto* flags = stg.scratch<uint32_t>(P + 1);
+    auto* scan = stg.scratch<uint32_t>(P + 1);
+    auto* ck = stg.scratch<uint32_t>(P);
+    e = stg.error();
     if (e == cudaSuccess) e = cudaMemsetAsync(cbeg, 0, (C + 1) * 4, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(cend, 0, (C + 1) * 4, st);
     if (e != cudaSuccess) return fail_cuda(e, "ground grids");
@@ -1203,43 +1150,27 @@ extern "C" ob_status ob_ground_mask(const ob_ground_item* items, size_t n_items,
     // pass 3: cells.  Sort the slots by (cell, z): by z (the zkeys still lie in k1[0, P)), then stably by cell
     uint32_t* slots = u1;        // iota
     uint32_t* zslots = u2;       // slots by z
-    uint32_t* ck = static_cast<uint32_t*>(ckeys);
     uint32_t* ck_z = u1 + P;     // cell key of each z-sorted slot
     uint32_t* ck_sorted = u2 + P;
     uint32_t* cslots = u1;       // slots by (cell, z)
-    launch(OB_FAM_GROUND, cell_keys_kernel, pgrid, kThreads, 0, st, df, gs, static_cast<const double*>(pts),
-           static_cast<const unsigned long long*>(k1), ck, slots, nC);
-    e = cudaGetLastError();
-    if (e == cudaSuccess) e = sort_pairs(stg, k1, k2, slots, zslots, P, 64, st);
-    if (e == cudaSuccess) {
-        launch(OB_FAM_GROUND, gather_kernel, flat, kThreads, 0, st, static_cast<const uint32_t*>(ck),
-               static_cast<const uint32_t*>(zslots), ck_z, P);
-        e = cudaGetLastError();
+    launch(OB_FAM_GROUND, cell_keys_kernel, pgrid, kThreads, 0, st, df, gs, pts, k1, ck, slots, nC);
+    stg.check(cudaGetLastError());
+    if (cub_run(stg, sort_pairs(k1, k2, slots, zslots, static_cast<int64_t>(P), 0, 64, st)) == cudaSuccess) {
+        launch(OB_FAM_GROUND, gather_kernel, flat, kThreads, 0, st, ck, zslots, ck_z, P);
+        stg.check(cudaGetLastError());
     }
-    if (e == cudaSuccess) e = sort_pairs(stg, ck_z, ck_sorted, zslots, cslots, P, bits_for(C), st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(static_cast<uint32_t*>(flags) + P, 0, 4, st);
+    cub_run(stg, sort_pairs(ck_z, ck_sorted, zslots, cslots, static_cast<int64_t>(P), 0, bits_for(C), st));
+    e = stg.error();
+    if (e == cudaSuccess) e = cudaMemsetAsync(flags + P, 0, 4, st);
     if (e != cudaSuccess) return fail_cuda(e, "ground cells");
-    launch(OB_FAM_GROUND, cell_segments_kernel, flat, kThreads, 0, st, static_cast<const uint32_t*>(ck_sorted),
-           static_cast<const uint32_t*>(cslots), static_cast<const unsigned long long*>(k1),
-           static_cast<const uint8_t*>(nflag), static_cast<uint32_t*>(cbeg), static_cast<uint32_t*>(cend),
-           static_cast<double*>(zs), static_cast<uint32_t*>(flags), P, nC);
-    e = cudaGetLastError();
-    if (e == cudaSuccess) {  // the normals-filtered lists: a flagged subsequence of each cell's sorted segment
-        size_t bytes = 0;
-        void* tmp = nullptr;
-        e = cub::DeviceScan::ExclusiveSum(nullptr, bytes, static_cast<uint32_t*>(flags), static_cast<uint32_t*>(scan),
-                                          static_cast<int64_t>(P + 1), st);
-        if (e == cudaSuccess) e = stg.scratch(bytes, &tmp);
-        if (e == cudaSuccess)
-            e = cub::DeviceScan::ExclusiveSum(tmp, bytes, static_cast<uint32_t*>(flags), static_cast<uint32_t*>(scan),
-                                              static_cast<int64_t>(P + 1), st);
-    }
-    if (e != cudaSuccess) return fail_cuda(e, "ground cells");
-    launch(OB_FAM_GROUND, compact_kernel, flat, kThreads, 0, st, static_cast<const uint32_t*>(flags),
-           static_cast<const uint32_t*>(scan), static_cast<const double*>(zs), static_cast<double*>(fz), P);
-    launch(OB_FAM_GROUND, cells_kernel, cgrid, kThreads, 0, st, df, gs, static_cast<const uint32_t*>(cbeg),
-           static_cast<const uint32_t*>(cend), static_cast<const double*>(zs), static_cast<const uint32_t*>(scan),
-           static_cast<const double*>(fz), g);
+    launch(OB_FAM_GROUND, cell_segments_kernel, flat, kThreads, 0, st, ck_sorted, cslots, k1, nflag, cbeg, cend, zs,
+           flags, P, nC);
+    stg.check(cudaGetLastError());
+    // the normals-filtered lists: a flagged subsequence of each cell's sorted segment
+    cub_run(stg, exclusive_sum(flags, scan, static_cast<int64_t>(P + 1), st));
+    if (cudaError_t e = stg.error()) return fail_cuda(e, "ground cells");
+    launch(OB_FAM_GROUND, compact_kernel, flat, kThreads, 0, st, flags, scan, zs, fz, P);
+    launch(OB_FAM_GROUND, cells_kernel, cgrid, kThreads, 0, st, df, gs, cbeg, cend, zs, scan, fz, g);
     e = cudaGetLastError();
     if (e != cudaSuccess) return fail_cuda(e, "ground cells");
 
@@ -1256,97 +1187,82 @@ extern "C" ob_status ob_ground_mask(const ob_ground_item* items, size_t n_items,
         launch(OB_FAM_GROUND, smooth_kernel, cgrid, kThreads, 0, st, df, static_cast<const GState*>(gs), g, g2);
         std::swap(g, g2);
     };
-    uint32_t* reach = static_cast<uint32_t*>(cbeg);  // cell segments are no longer needed
-    uint32_t* queue = static_cast<uint32_t*>(cend);
+    uint32_t* reach = cbeg;  // cell segments are no longer needed
+    uint32_t* queue = cend;
     if (stop >= OB_GROUND_FILL1) fill(6);
     if (stop >= OB_GROUND_SMOOTH1) smooth();
     if (stop >= OB_GROUND_PRUNE) launch(OB_FAM_GROUND, prune_kernel, F, 1024, 0, st, df, gs, g, reach, queue);
     if (stop >= OB_GROUND_FILL2) fill(6);
     if (stop >= OB_GROUND_SMOOTH2) smooth();
-    e = cudaGetLastError();
-    if (e == cudaSuccess && stop >= OB_GROUND_COMPONENTS) {
-        uint32_t* parent = static_cast<uint32_t*>(cbeg);
-        uint32_t* csize = static_cast<uint32_t*>(cend);
-        void *hk_p = nullptr, *hks_p = nullptr, *c1 = nullptr, *c2 = nullptr, *c3 = nullptr, *r1 = nullptr,
-             *r2 = nullptr, *med_p = nullptr;
-        alloc((C + 1) * 8, &hk_p);
-        alloc((C + 1) * 8, &hks_p);
-        alloc((C + 1) * 4, &c1);
-        alloc((C + 1) * 4, &c2);
-        alloc((C + 1) * 4, &c3);
-        alloc((C + 1) * 4, &r1);
-        alloc((C + 1) * 4, &r2);
-        alloc((C + 1) * 8, &med_p);
-        if (e != cudaSuccess) return fail_cuda(e, "ground components");
-        auto* hk = static_cast<unsigned long long*>(hk_p);
-        auto* hk_sorted = static_cast<unsigned long long*>(hks_p);
-        uint32_t* cells = static_cast<uint32_t*>(c1);
-        uint32_t* cells_h = static_cast<uint32_t*>(c2);
-        uint32_t* cells_sorted = static_cast<uint32_t*>(c3);
-        uint32_t* roots_h = static_cast<uint32_t*>(r1);
-        uint32_t* roots_sorted = static_cast<uint32_t*>(r2);
-        double* med = static_cast<double*>(med_p);
+    stg.check(cudaGetLastError());
+    if (!stg.error() && stop >= OB_GROUND_COMPONENTS) {
+        uint32_t* parent = cbeg;
+        uint32_t* csize = cend;
+        auto* hk = stg.scratch<unsigned long long>(C + 1);
+        auto* hk_sorted = stg.scratch<unsigned long long>(C + 1);
+        auto* cells = stg.scratch<uint32_t>(C + 1);
+        auto* cells_h = stg.scratch<uint32_t>(C + 1);
+        auto* cells_sorted = stg.scratch<uint32_t>(C + 1);
+        auto* roots_h = stg.scratch<uint32_t>(C + 1);
+        auto* roots_sorted = stg.scratch<uint32_t>(C + 1);
+        auto* med = stg.scratch<double>(C + 1);
+        if (cudaError_t e = stg.error()) return fail_cuda(e, "ground components");
         launch(OB_FAM_GROUND, comp_init_kernel, cgrid, kThreads, 0, st, df, static_cast<const GState*>(gs), parent,
                csize);
         launch(OB_FAM_GROUND, comp_hook_kernel, cgrid, kThreads, 0, st, df, static_cast<const GState*>(gs), g, parent);
         launch(OB_FAM_GROUND, comp_roots_kernel, cgrid, kThreads, 0, st, df, static_cast<const GState*>(gs), g, parent,
                csize, hk, cells, nC);
-        e = cudaGetLastError();
-        // (root, height) order: by height, then stably by root
-        if (e == cudaSuccess) e = sort_pairs(stg, hk, hk_sorted, cells, cells_h, C, 64, st);
-        if (e == cudaSuccess) {
-            launch(OB_FAM_GROUND, root_keys_kernel, blocks_for(C, kThreads), kThreads, 0, st,
-                   static_cast<const unsigned long long*>(hk_sorted), static_cast<const uint32_t*>(cells_h),
-                   static_cast<const uint32_t*>(parent), roots_h, static_cast<unsigned long long>(C), nC);
-            e = cudaGetLastError();
+        stg.check(cudaGetLastError());
+        // (root, height) order: by height, then stably by root (C == 0: nothing to sort)
+        if (C) cub_run(stg, sort_pairs(hk, hk_sorted, cells, cells_h, static_cast<int64_t>(C), 0, 64, st));
+        if (!stg.error()) {
+            launch(OB_FAM_GROUND, root_keys_kernel, blocks_for(C, kThreads), kThreads, 0, st, hk_sorted, cells_h,
+                   parent, roots_h, static_cast<unsigned long long>(C), nC);
+            stg.check(cudaGetLastError());
         }
-        if (e == cudaSuccess) e = sort_pairs(stg, roots_h, roots_sorted, cells_h, cells_sorted, C, bits_for(C), st);
-        if (e == cudaSuccess) {
-            launch(OB_FAM_GROUND, comp_median_kernel, blocks_for(C, kThreads), kThreads, 0, st, df, gs,
-                   static_cast<const uint32_t*>(roots_sorted), static_cast<const uint32_t*>(cells_sorted),
-                   static_cast<const uint32_t*>(csize), g, med, F, nC);
+        if (C)
+            cub_run(stg, sort_pairs(roots_h, roots_sorted, cells_h, cells_sorted, static_cast<int64_t>(C), 0,
+                                    bits_for(C), st));
+        if (!stg.error()) {
+            launch(OB_FAM_GROUND, comp_median_kernel, blocks_for(C, kThreads), kThreads, 0, st, df, gs, roots_sorted,
+                   cells_sorted, csize, g, med, F, nC);
             launch(OB_FAM_GROUND, comp_reject_kernel, cgrid, kThreads, 0, st, df, static_cast<const GState*>(gs), g,
-                   static_cast<const uint32_t*>(parent), static_cast<const uint32_t*>(csize),
-                   static_cast<const double*>(med));
-            e = cudaGetLastError();
+                   parent, csize, med);
+            stg.check(cudaGetLastError());
         }
     }
-    if (e == cudaSuccess && stop >= OB_GROUND_FILL3) fill(3);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(e, "ground passes");
+    if (!stg.error() && stop >= OB_GROUND_FILL3) fill(3);
+    if (!stg.error()) stg.check(cudaGetLastError());
+    if (cudaError_t e = stg.error()) return fail_cuda(e, "ground passes");
 
     // outputs: masks (classified at the last pass, else zeroed), model headers, grids
     launch(OB_FAM_GROUND, classify_kernel, dim3(blocks_for(max_px, kThreads), F), kThreads, 0, st, df,
            static_cast<const GState*>(gs), g, stop >= OB_GROUND_FINAL ? 1 : 0);
-    void* dmodel = nullptr;
-    e = cudaGetLastError();
-    if (e == cudaSuccess) e = stg.scratch(F * sizeof(ob_ground_model), &dmodel);
-    if (e == cudaSuccess) {
-        launch(OB_FAM_GROUND, model_kernel, (F + 63) / 64, 64, 0, st, static_cast<const GState*>(gs),
-               static_cast<ob_ground_model*>(dmodel), F);
-        e = cudaGetLastError();
+    stg.check(cudaGetLastError());
+    auto* dmodel = stg.scratch<ob_ground_model>(F);
+    if (!stg.error()) {
+        launch(OB_FAM_GROUND, model_kernel, (F + 63) / 64, 64, 0, st, static_cast<const GState*>(gs), dmodel, F);
+        stg.check(cudaGetLastError());
     }
-    for (unsigned k = 0; k < F && e == cudaSuccess; ++k) {
+    // n elements of device memory src into the caller's dst, host or device
+    auto copy_out = [&](auto* dst, const auto* src, size_t n) {
+        if (!dst || n == 0) return;
+        auto* d = stg.out(dst, n);
+        if (!stg.error()) stg.check(cudaMemcpyAsync(d, src, n * sizeof(*src), cudaMemcpyDeviceToDevice, st));
+    };
+    for (unsigned k = 0; k < F && !stg.error(); ++k) {
         const ob_ground_item& it = items[slot_of[k]];
         const size_t cells = hs[k].n_points ? static_cast<size_t>(hs[k].rows) * hs[k].cols : 0;
         const size_t off = frames[k].cell_off;
-        auto copy_out = [&](void* dst, const void* src, size_t bytes) {
-            if (!dst || bytes == 0 || e != cudaSuccess) return;
-            void* d = nullptr;
-            e = stg.out(dst, bytes, &d);
-            if (e == cudaSuccess) e = cudaMemcpyAsync(d, src, bytes, cudaMemcpyDeviceToDevice, st);
-        };
-        copy_out(it.model, static_cast<ob_ground_model*>(dmodel) + k, sizeof(ob_ground_model));
-        if (batch_of[k] >= 0)
-            copy_out(it.vertical_subtent_out, batches[batch_of[k]].subtent + index_in_batch[k], 8);
+        copy_out(it.model, dmodel + k, 1);
+        if (batch_of[k] >= 0) copy_out(it.vertical_subtent_out, batches[batch_of[k]].subtent + index_in_batch[k], 1);
         copy_out(it.valid, g.valid + off, cells);
         copy_out(it.obstacle, g.obstacle + off, cells);
-        copy_out(it.floor_z, g.floor_z + off, cells * 8);
-        copy_out(it.height, g.height + off, cells * 8);
-        copy_out(it.roughness, g.rough + off, cells * 8);
-        if (it.prune_levels) copy_out(it.prune_levels, &gs[k].prune_levels, 4);
+        copy_out(it.floor_z, g.floor_z + off, cells);
+        copy_out(it.height, g.height + off, cells);
+        copy_out(it.roughness, g.rough + off, cells);
+        copy_out(it.prune_levels, &gs[k].prune_levels, 1);
     }
-    if (e == cudaSuccess) e = stg.finish();
-    if (e != cudaSuccess) return fail_cuda(e, "ground outputs");
+    if (cudaError_t e = stg.finish()) return fail_cuda(e, "ground outputs");
     return OB_OK;
 }

@@ -681,13 +681,12 @@ ob_status ob_image_proc_update(ob_image_proc* p, int layout, int dtype, const vo
     const void* din = nullptr;
     void* dout = nullptr;
     if (f16) {
-        e = stg.in(in, n * 2, &din);
-        if (e == cudaSuccess) e = stg.out(out, n * 4, &dout);
+        din = stg.in(in, n * 2);
+        dout = stg.out(out, n * 4);
     } else {
-        e = stg.inout(out, n * esz, &dout);
-        din = dout;
+        din = dout = stg.inout(out, n * esz);
     }
-    if (e != cudaSuccess) return fail_cuda(e, "stage image");
+    if (cudaError_t e = stg.error()) return fail_cuda(e, "stage image");
     const uint32_t np = uint32_t(npx);
     const int us = update_state ? 1 : 0;
     if (p->kind == OB_IMAGE_AUTO_EXPOSURE) {
@@ -704,8 +703,8 @@ ob_status ob_image_proc_update(ob_image_proc* p, int layout, int dtype, const vo
         if (dtype == OB_F32) launch_buc<float>(p, static_cast<float*>(dout), rows, cols, us, st);
         else launch_buc<double>(p, static_cast<double*>(dout), rows, cols, us, st);
     }
-    e = cudaGetLastError();
-    if (e == cudaSuccess) e = stg.flush();
+    stg.check(cudaGetLastError());
+    e = stg.flush();
     if (e == cudaSuccess && (!is_device_ptr(out) || (f16 && !is_device_ptr(in)))) e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail_cuda(e, "image update");
     return OB_OK;

@@ -183,36 +183,30 @@ extern "C" ob_status ob_frames_to_map_rows(const ob_map_rows_item* items, size_t
         it.n_blocks = static_cast<unsigned>((n_px + kMrTile - 1) / kMrTile);
         it.n_fields = static_cast<unsigned>(io.n_fields);
         nb += it.n_blocks;
-        const void* d = nullptr;
-        cudaError_t e = stg.in(io.range, n_px * 4, &d);
-        it.range = static_cast<const uint32_t*>(d);
-        if (e == cudaSuccess) e = stg.in(io.poses, lv.w * 16 * 8, &d);
-        it.poses = static_cast<const double*>(d);
-        for (size_t k = 0; k < io.n_fields && e == cudaSuccess; ++k) {
+        it.range = stg.in(io.range, n_px);
+        it.poses = stg.in(io.poses, lv.w * 16);
+        for (size_t k = 0; k < io.n_fields; ++k) {
             const ob_map_field& fd = io.fields[k];
-            e = stg.in(fd.data, n_px * fd.channels * field_bytes(fd.type), &d);
-            it.f[k] = MrField{d, fd.type, fd.channels};
+            it.f[k] = MrField{stg.in(fd.data, n_px * fd.channels * field_bytes(fd.type)), fd.type, fd.channels};
         }
-        if (e != cudaSuccess) return fail_cuda(e, "stage map rows inputs");
+        if (cudaError_t e = stg.error()) return fail_cuda(e, "stage map rows inputs");
         hi.push_back(it);
     }
     if (hi.empty()) return OB_OK;
     const unsigned ni = static_cast<unsigned>(hi.size());
-    void *tab = nullptr, *scan = nullptr;
-    cudaError_t e = stg.scratch(hi.size() * sizeof(MrItem), &tab);
-    if (e == cudaSuccess) e = stg.scratch(state_bytes(nb) + static_cast<size_t>(nb) * 16 + ni * 8ull, &scan);
+    auto* tab = stg.scratch<MrItem>(hi.size());
+    auto* b = stg.scratch<uint8_t>(state_bytes(nb) + static_cast<size_t>(nb) * 16 + ni * 8ull);
+    double* dout = res.array(rows, cols * 8);
+    cudaError_t e = stg.error();
     if (e == cudaSuccess) e = cudaMemcpyAsync(tab, hi.data(), hi.size() * sizeof(MrItem), cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(scan, 0, state_bytes(nb), st);  // ticket + state words
-    double* dout = nullptr;
-    if (e == cudaSuccess) e = res.array(rows, cols * 8, &dout);
+    if (e == cudaSuccess) e = cudaMemsetAsync(b, 0, state_bytes(nb), st);  // ticket + state words
     if (e != cudaSuccess) return fail_cuda(e, "stage map rows");
-    uint8_t* b = static_cast<uint8_t*>(scan);
     Lookback lb;
     lb.state = reinterpret_cast<uint32_t*>(b + 16);
     lb.agg = reinterpret_cast<unsigned long long*>(b + state_bytes(nb));
     lb.incl = lb.agg + nb;
     unsigned long long* item_end = lb.incl + nb;
-    launch(OB_FAM_VOXEL_MAP, map_rows_kernel, nb, kMrThreads, 0, st, static_cast<const MrItem*>(tab), ni,
+    launch(OB_FAM_VOXEL_MAP, map_rows_kernel, nb, kMrThreads, 0, st, tab, ni,
            static_cast<unsigned>(cols), reinterpret_cast<unsigned*>(b), lb, item_end, dout, capacity);
     e = cudaGetLastError();
     if (e != cudaSuccess) return fail_cuda(e, "map rows launch");

@@ -336,42 +336,23 @@ extern "C" ob_status ob_normals(ob_dtype dtype, const ob_normals_io* io, ob_stre
     const size_t out_fs = io->normals_frame_stride ? io->normals_frame_stride : n_px * 3;
     Staging stg(st);
     NormalsParams p{};
-    const void* d = nullptr;
-    void* o = nullptr;
     // a host output with padding between frames is uploaded first so the padding survives the copy back
     const size_t out_bytes = ((F - 1) * out_fs + n_px * 3) * esz;
     const bool padded = F > 1 && out_fs != n_px * 3;
-    auto stage_out = [&](void* host, void** dev) {
-        return padded ? stg.inout(host, out_bytes, dev) : stg.out(host, out_bytes, dev);
-    };
-    cudaError_t e = stg.in(io->xyz, ((F - 1) * xyz_fs + n_px * 3) * esz, &d);
-    p.xyz[0] = d;
-    if (e == cudaSuccess) e = stg.in(io->range, ((F - 1) * range_fs + n_px) * 4, &d);
-    p.range[0] = static_cast<const uint32_t*>(d);
-    if (e == cudaSuccess) e = stage_out(io->normals, &o);
-    p.out[0] = o;
+    auto stage_out = [&](void* host) { return padded ? stg.inout(host, out_bytes) : stg.out(host, out_bytes); };
+    p.xyz[0] = stg.in(io->xyz, ((F - 1) * xyz_fs + n_px * 3) * esz);
+    p.range[0] = stg.in(io->range, (F - 1) * range_fs + n_px);
+    p.out[0] = stage_out(io->normals);
     if (dual) {
-        if (e == cudaSuccess) e = stg.in(io->xyz2, ((F - 1) * xyz_fs + n_px * 3) * esz, &d);
-        p.xyz[1] = d;
-        if (e == cudaSuccess) e = stg.in(io->range2, ((F - 1) * range_fs + n_px) * 4, &d);
-        p.range[1] = static_cast<const uint32_t*>(d);
-        if (e == cudaSuccess) e = stage_out(io->normals2, &o);
-        p.out[1] = o;
+        p.xyz[1] = stg.in(io->xyz2, ((F - 1) * xyz_fs + n_px * 3) * esz);
+        p.range[1] = stg.in(io->range2, (F - 1) * range_fs + n_px);
+        p.out[1] = stage_out(io->normals2);
     }
-    if (e == cudaSuccess && io->sensor_origins_xyz) {
-        e = stg.in(io->sensor_origins_xyz, ((F - 1) * io->origins_frame_stride + io->w * 3) * 8, &d);
-        p.origins = static_cast<const double*>(d);
-    }
-    void* sub = nullptr;
-    void* sub2 = nullptr;
-    if (e == cudaSuccess) {
-        if (io->vertical_subtent_out) e = stg.out(io->vertical_subtent_out, F * 8, &sub);
-        else e = stg.scratch(F * 8, &sub);
-    }
-    if (e == cudaSuccess && dual) e = stg.scratch(F * 8, &sub2);
-    if (e != cudaSuccess) return fail_cuda(e, "stage normals buffers");
-    p.subtent[0] = static_cast<double*>(sub);
-    p.subtent[1] = static_cast<double*>(sub2);
+    if (io->sensor_origins_xyz)
+        p.origins = stg.in(io->sensor_origins_xyz, (F - 1) * io->origins_frame_stride + io->w * 3);
+    p.subtent[0] = io->vertical_subtent_out ? stg.out(io->vertical_subtent_out, F) : stg.scratch<double>(F);
+    if (dual) p.subtent[1] = stg.scratch<double>(F);
+    if (cudaError_t e = stg.error()) return fail_cuda(e, "stage normals buffers");
     p.xyz_fs = xyz_fs;
     p.range_fs = range_fs;
     p.out_fs = out_fs;
@@ -398,7 +379,7 @@ extern "C" ob_status ob_normals(ob_dtype dtype, const ob_normals_io* io, ob_stre
         launch(OB_FAM_NORMALS, normals_kernel<float>, grid, 256, 0, st, p, 0);
         if (dual) launch(OB_FAM_NORMALS, normals_kernel<float>, grid, 256, 0, st, p, 1);
     }
-    e = cudaGetLastError();
+    cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail_cuda(e, "normals launch");
     e = stg.flush();
     if (e != cudaSuccess) return fail_cuda(e, "normals D2H");

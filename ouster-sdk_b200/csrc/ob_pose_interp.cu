@@ -478,23 +478,21 @@ extern "C" ob_status ob_interp_pose(const ob_interp_pose_io* io, ob_stream* s) {
         return fail(OB_INVALID_ARGUMENT, "a device-side error word needs device outputs");
     const size_t n = io->n, m = io->m, S = io->two_pose ? 1 : m - 1;
     Staging stg(st);
-    const void *x = nullptr, *knots = nullptr, *pk = nullptr;
-    void *out = nullptr, *work = nullptr;
-    cudaError_t e = stg.in(io->x_interp, n * 8, &x);
-    if (e == cudaSuccess) e = stg.in(io->x_known, m * 8, &knots);
-    if (e == cudaSuccess) e = stg.in(io->poses_known, m * 16 * psz, &pk);
-    if (e == cudaSuccess) e = stg.out(io->poses, n * 16 * psz, &out);
+    const void* x = stg.in(io->x_interp, n * 8);
+    const void* knots = stg.in(io->x_known, m * 8);
+    const void* pk = stg.in(io->poses_known, m * 16 * psz);
+    void* out = stg.out(io->poses, n * 16 * psz);
     // work: flags (16 B) | error words (5 x 8 B, padded to 48) | ends (S x 8 B) | segments
     const size_t ends_off = 64, seg_off = (ends_off + S * 8 + 15) & ~static_cast<size_t>(15);
-    if (e == cudaSuccess) e = stg.scratch(seg_off + S * sizeof(Seg), &work);
-    if (e != cudaSuccess) return fail_cuda(e, "stage interp_pose");
-    uint8_t* w = static_cast<uint8_t*>(work);
+    uint8_t* w = stg.scratch<uint8_t>(seg_off + S * sizeof(Seg));
+    if (cudaError_t e = stg.error()) return fail_cuda(e, "stage interp_pose");
     ScanFlags* fl = reinterpret_cast<ScanFlags*>(w);
     long long* vals = reinterpret_cast<long long*>(w + 16) + 3;
     long long* err = dev_err ? reinterpret_cast<long long*>(io->error) : reinterpret_cast<long long*>(w + 16);
     size_t* ends = reinterpret_cast<size_t*>(w + ends_off);
     Seg* segs = reinterpret_cast<Seg*>(w + seg_off);
     const bool f64 = io->x_dtype == OB_POSE_X_F64;
+    cudaError_t e;
     if (f64 && psz == 8) e = launch_interp<double, double>(io, x, knots, pk, out, fl, ends, segs, err, vals, device, st);
     else if (f64) e = launch_interp<double, float>(io, x, knots, pk, out, fl, ends, segs, err, vals, device, st);
     else if (psz == 8) e = launch_interp<long long, double>(io, x, knots, pk, out, fl, ends, segs, err, vals, device, st);
@@ -541,38 +539,30 @@ extern "C" ob_status ob_frames_interp_pose(const ob_frame_poses_item* frames, si
     Staging stg(st);
     std::vector<FrameItem> items;
     unsigned nb = 0;
-    cudaError_t e = cudaSuccess;
-    for (size_t i = 0; i < n_frames && e == cudaSuccess; ++i) {
+    for (size_t i = 0; i < n_frames && !stg.error(); ++i) {
         const ob_frame_poses_item& f = frames[i];
         if (!f.timestamps || f.w == 0) continue;
         FrameItem it{};
-        const void* d = nullptr;
-        if (x1) e = stg.in(f.timestamps, f.w * 8, &d);
-        it.ts = static_cast<const unsigned long long*>(d);
-        if (e == cudaSuccess) e = stg.in(f.status, f.w * 4, &d);
-        it.status = static_cast<const uint32_t*>(d);
-        void* pd = nullptr;
-        if (e == cudaSuccess) e = stg.inout(f.poses, f.w * 128, &pd);  // invalid columns keep their bytes
-        it.poses = static_cast<double*>(pd);
-        it.vec = (reinterpret_cast<uintptr_t>(pd) & 15u) == 0;
+        if (x1) it.ts = reinterpret_cast<const unsigned long long*>(stg.in(f.timestamps, f.w));
+        it.status = stg.in(f.status, f.w);
+        it.poses = stg.inout(f.poses, f.w * 16);  // invalid columns keep their bytes
+        it.vec = (reinterpret_cast<uintptr_t>(it.poses) & 15u) == 0;
         it.w = static_cast<unsigned>(f.w);
         it.first_block = nb;
         it.slot = static_cast<unsigned>(i);
         nb += static_cast<unsigned>((f.w + kWriteThreads - 1) / kWriteThreads);
         items.push_back(it);
     }
-    const void *dx0 = nullptr, *dx1 = nullptr;
-    if (e == cudaSuccess) e = stg.in(x0, 128, &dx0);
-    if (e == cudaSuccess && x1) e = stg.in(x1, 128, &dx1);
+    const double* dx0 = stg.in(x0, 16);
+    const double* dx1 = stg.in(x1, 16);
     // work: error words (5 x 8 B, padded to 48) | FrameState | desc.  The item table goes through the stream's
     // table cache: an unchanged set issues no host copy, so a call can be captured in a CUDA graph after one run
-    void* work = nullptr;
-    const void* tab = nullptr;
     const size_t st_off = 48, desc_off = st_off + sizeof(FrameState);
-    if (e == cudaSuccess) e = stg.scratch(desc_off + items.size() * 4, &work);
+    uint8_t* w = stg.scratch<uint8_t>(desc_off + items.size() * 4);
+    const void* tab = nullptr;
+    cudaError_t e = stg.error();
     if (e == cudaSuccess && !items.empty()) e = stream_table(s, 2, items.data(), items.size() * sizeof(FrameItem), &tab);
     if (e != cudaSuccess) return fail_cuda(e, "stage frames_interp_pose");
-    uint8_t* w = static_cast<uint8_t*>(work);
     long long* err = dev_err ? reinterpret_cast<long long*>(error) : reinterpret_cast<long long*>(w);
     long long* vals = reinterpret_cast<long long*>(w) + 3;
     FrameState* fs = reinterpret_cast<FrameState*>(w + st_off);
@@ -584,17 +574,17 @@ extern "C" ob_status ob_frames_interp_pose(const ob_frame_poses_item* frames, si
         if (e != cudaSuccess) return fail_cuda(e, "stage frames_interp_pose");
         if (x1)
             launch(OB_FAM_POSE, frame_check_kernel, static_cast<unsigned>(items.size()), kCheckThreads, 0, st, ditems,
-                   fs, desc, t0, static_cast<const double*>(dx0), t1, static_cast<const double*>(dx1));
+                   fs, desc, t0, dx0, t1, dx1);
         launch(OB_FAM_POSE, frame_write_kernel, nb, kWriteThreads, 0, st, ditems, static_cast<unsigned>(items.size()),
-               x1 ? fs : nullptr, desc, static_cast<const double*>(dx0), err, vals);
+               x1 ? fs : nullptr, desc, dx0, err, vals);
         e = cudaGetLastError();
     }
     if (e != cudaSuccess) return fail_cuda(e, "frames_interp_pose launch");
     // host error words: the call waits once, for the words and the host poses together
     long long words[5] = {0, 0, 0, 0, 0};
     const bool read = !dev_err && x1 && !items.empty();
-    if (read) e = cudaMemcpyAsync(words, w, sizeof words, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = read ? stg.flush() : stg.finish();
+    if (read) stg.check(cudaMemcpyAsync(words, w, sizeof words, cudaMemcpyDeviceToHost, st));
+    e = read ? stg.flush() : stg.finish();
     if (e == cudaSuccess && read) e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail_cuda(e, "frames_interp_pose");
     return pose_error_status(words, OB_POSE_X_F64);

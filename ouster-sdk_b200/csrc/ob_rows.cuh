@@ -54,19 +54,9 @@ ob_status stage_rows(const ob_point_rows* in, Staging& stg, Rows* r, const char*
     ob_status rs = count_rows(in->n, in->n_device, in->capacity, r);
     if (rs != OB_OK) return rs;
     if (r->cap && !in->points) return fail(OB_INVALID_ARGUMENT, "null points buffer");
-    const void* d = nullptr;
-    cudaError_t e = stg.in(in->points, r->cap * 3ull * (in->dtype == OB_F64 ? 8 : 4), &d);
-    if (e != cudaSuccess) return fail_cuda(e, what);
-    r->p = d;
+    r->p = stg.in(in->points, r->cap * 3ull * (in->dtype == OB_F64 ? 8 : 4));
+    if (cudaError_t e = stg.error()) return fail_cuda(e, what);
     return OB_OK;
-}
-
-template <typename P>
-cudaError_t scratch(Staging& stg, size_t bytes, P** p) {
-    void* d = nullptr;
-    cudaError_t e = stg.scratch(bytes, &d);
-    *p = static_cast<P*>(d);
-    return e;
 }
 
 }  // namespace

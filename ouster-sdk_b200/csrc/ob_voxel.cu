@@ -22,13 +22,10 @@
 // SHUFFLE_FIRST (core::voxel_downsample): the Fisher-Yates shuffle depends only on n; its permutation is
 // resolved without a serial loop (DESIGN 4, f-5), then the shuffled sequence goes through FIRST_N with
 // one slot per voxel.
-#include <cub/device/device_radix_sort.cuh>
-#include <cub/device/device_scan.cuh>
-
 #include <algorithm>
-#include <type_traits>
 
 #include "ob_api_common.h"
+#include "ob_cub.cuh"
 #include "ob_rows.cuh"
 #include "ob_voxel_common.cuh"
 
@@ -435,78 +432,51 @@ cudaError_t run_voxel(VoxelParams p, Staging& stg, cudaStream_t st, double* out,
                       unsigned long long* n_out_dev) {
     const unsigned cap = p.cap;
     const unsigned nb = blocks_for(cap);
-    auto alloc = [&](size_t bytes, auto** ptr) {
-        void* d = nullptr;
-        cudaError_t e = stg.scratch(bytes, &d);
-        *ptr = static_cast<std::remove_reference_t<decltype(*ptr)>>(d);
-        return e;
-    };
-    cudaError_t e = cudaSuccess;
-    size_t tmp_bytes = 0, need = 0;
-    void* tmp = nullptr;
+    const int n = static_cast<int>(cap);
     // CUB temporary storage: one block sized for the largest of the calls below
-    {
-        VKey* k = nullptr;
-        uint32_t* u = nullptr;
-        e = cub::DeviceRadixSort::SortPairs(nullptr, need, k, k, u, u, static_cast<int>(cap), VKeyDecomposer{}, 0, kKeyBits, st);
-        if (e != cudaSuccess) return e;
-        tmp_bytes = need;
-        e = cub::DeviceRadixSort::SortPairs(nullptr, need, u, u, u, u, static_cast<int>(cap), 0, 32, st);
-        if (e != cudaSuccess) return e;
-        tmp_bytes = std::max(tmp_bytes, need);
-        e = cub::DeviceScan::InclusiveSum(nullptr, need, u, u, static_cast<int>(cap), st);
-        if (e != cudaSuccess) return e;
-        tmp_bytes = std::max(tmp_bytes, need);
-        e = cub::DeviceScan::ExclusiveSum(nullptr, need, u, u, static_cast<int>(cap), st);
-        if (e != cudaSuccess) return e;
-        tmp_bytes = std::max(tmp_bytes, need);
-        e = stg.scratch(tmp_bytes, &tmp);
-        if (e != cudaSuccess) return e;
-    }
+    VKey* k = nullptr;
+    uint32_t* u = nullptr;
+    CubTemp tmp(stg, sort_pairs(k, k, u, u, n, VKeyDecomposer{}, 0, kKeyBits, st), sort_pairs(u, u, u, u, n, 0, 32, st),
+                inclusive_sum(u, u, n, st), exclusive_sum(u, u, n, st));
     if (p.mode == OB_VOXEL_SHUFFLE_FIRST) {
-        uint32_t *jkey, *step, *sj, *ss, *where, *order;
-        int32_t* last_of;
-        e = alloc(cap * 4ull, &jkey);
-        if (e == cudaSuccess) e = alloc(cap * 4ull, &step);
-        if (e == cudaSuccess) e = alloc(cap * 4ull, &sj);
-        if (e == cudaSuccess) e = alloc(cap * 4ull, &ss);
-        if (e == cudaSuccess) e = alloc(cap * 4ull, &where);
-        if (e == cudaSuccess) e = alloc(cap * 4ull, &order);
-        if (e == cudaSuccess) e = alloc(cap * 4ull, &last_of);
+        auto* jkey = stg.scratch<uint32_t>(cap);
+        auto* step = stg.scratch<uint32_t>(cap);
+        auto* sj = stg.scratch<uint32_t>(cap);
+        auto* ss = stg.scratch<uint32_t>(cap);
+        auto* where = stg.scratch<uint32_t>(cap);
+        auto* order = stg.scratch<uint32_t>(cap);
+        auto* last_of = stg.scratch<int32_t>(cap);
+        cudaError_t e = stg.error();
         if (e == cudaSuccess) e = cudaMemsetAsync(last_of, 0xff, cap * 4ull, st);
         if (e != cudaSuccess) return e;
         launch(OB_FAM_VOXEL, vx_shuffle_draw_kernel, nb, 256, 0, st, p, jkey, step);
-        int bits = 1;
-        while (bits < 32 && (1ull << bits) <= cap) ++bits;
-        e = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, jkey, sj, step, ss, static_cast<int>(cap), 0, bits, st);
+        e = tmp.run(sort_pairs(jkey, sj, step, ss, n, 0, bits_for(cap), st));
         if (e != cudaSuccess) return e;
         launch(OB_FAM_VOXEL, vx_shuffle_index_kernel, nb, 256, 0, st, cap, sj, ss, where, last_of);
         launch(OB_FAM_VOXEL, vx_shuffle_perm_kernel, nb, 256, 0, st, p, sj, ss, where, last_of, order);
         p.order = order;
     }
-    VKey *keys, *sk;
-    uint32_t *seq, *sseq, *opens, *vrank, *seg_start, *cnt, *coff;
+    auto* keys = stg.scratch<VKey>(cap);
+    auto* sk = stg.scratch<VKey>(cap);
+    auto* seq = stg.scratch<uint32_t>(cap);
+    auto* sseq = stg.scratch<uint32_t>(cap);
+    auto* opens = stg.scratch<uint32_t>(cap);
+    auto* vrank = stg.scratch<uint32_t>(cap);
+    auto* seg_start = stg.scratch<uint32_t>(cap);
+    auto* cnt = stg.scratch<uint32_t>(cap);
+    auto* coff = stg.scratch<uint32_t>(cap);
     Work w{};
-    e = alloc(cap * sizeof(VKey), &keys);
-    if (e == cudaSuccess) e = alloc(cap * sizeof(VKey), &sk);
-    if (e == cudaSuccess) e = alloc(cap * 4ull, &seq);
-    if (e == cudaSuccess) e = alloc(cap * 4ull, &sseq);
-    if (e == cudaSuccess) e = alloc(cap * 4ull, &opens);
-    if (e == cudaSuccess) e = alloc(cap * 4ull, &vrank);
-    if (e == cudaSuccess) e = alloc(cap * 4ull, &seg_start);
-    if (e == cudaSuccess) e = alloc(cap * 4ull, &cnt);
-    if (e == cudaSuccess) e = alloc(cap * 4ull, &coff);
-    if (e == cudaSuccess) e = alloc(cap * 4ull, &w.vfirst);
+    w.vfirst = stg.scratch<uint32_t>(cap);
     const bool sums = p.mode == OB_VOXEL_AVERAGE_POINT || p.mode == OB_VOXEL_POINT_NORMAL;
-    if (e == cudaSuccess && sums)
-        e = alloc(static_cast<size_t>(cap) * (p.mode == OB_VOXEL_AVERAGE_POINT ? p.cols : 6u) * 8ull, &w.vres);
-    if (e == cudaSuccess && !sums) e = alloc(cap * 4ull, &w.slot);
+    if (sums) w.vres = stg.scratch<double>(static_cast<size_t>(cap) * (p.mode == OB_VOXEL_AVERAGE_POINT ? p.cols : 6u));
+    else w.slot = stg.scratch<uint32_t>(cap);
     uint32_t* draw = nullptr;
-    if (e == cudaSuccess && p.mode == OB_VOXEL_RANDOM) {
-        e = alloc(cap * 4ull, &w.full);
-        if (e == cudaSuccess) e = alloc(cap * 4ull, &draw);
-        if (e == cudaSuccess) e = cudaMemsetAsync(w.full, 0, cap * 4ull, st);
+    if (p.mode == OB_VOXEL_RANDOM) {
+        w.full = stg.scratch<uint32_t>(cap);
+        draw = stg.scratch<uint32_t>(cap);
     }
+    cudaError_t e = stg.error();
+    if (e == cudaSuccess && p.mode == OB_VOXEL_RANDOM) e = cudaMemsetAsync(w.full, 0, cap * 4ull, st);
     if (e != cudaSuccess) return e;
     w.sk = sk;
     w.sseq = sseq;
@@ -515,24 +485,23 @@ cudaError_t run_voxel(VoxelParams p, Staging& stg, cudaStream_t st, double* out,
     w.cnt = cnt;
     w.draw = draw;
     launch(OB_FAM_VOXEL, vx_key_kernel<T>, nb, 256, 0, st, p, keys, seq);
-    e = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, sk, seq, sseq, static_cast<int>(cap), VKeyDecomposer{}, 0,
-                                        kKeyBits, st);
+    e = tmp.run(sort_pairs(keys, sk, seq, sseq, n, VKeyDecomposer{}, 0, kKeyBits, st));
     if (e != cudaSuccess) return e;
     launch(OB_FAM_VOXEL, vx_head_kernel, nb, 256, 0, st, cap, sk, sseq, opens);
-    e = cub::DeviceScan::InclusiveSum(tmp, tmp_bytes, opens, vrank, static_cast<int>(cap), st);
+    e = tmp.run(inclusive_sum(opens, vrank, n, st));
     if (e != cudaSuccess) return e;
     launch(OB_FAM_VOXEL, vx_seg_kernel, nb, 256, 0, st, cap, sk, sseq, vrank, seg_start);
     if (sums) {
         launch(OB_FAM_VOXEL, vx_reduce_sum_kernel<T>, nb, 256, 0, st, p, w);
     } else if (p.mode == OB_VOXEL_RANDOM) {
         launch(OB_FAM_VOXEL, vx_random_flags_kernel, nb, 256, 0, st, p, w);
-        e = cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, w.full, draw, static_cast<int>(cap), st);
+        e = tmp.run(exclusive_sum(w.full, draw, n, st));
         if (e != cudaSuccess) return e;
         launch(OB_FAM_VOXEL, vx_random_pick_kernel, nb, 256, 0, st, p, w);
     } else {
         launch(OB_FAM_VOXEL, vx_reduce_first_kernel<T>, nb, 256, 0, st, p, w);
     }
-    e = cub::DeviceScan::InclusiveSum(tmp, tmp_bytes, cnt, coff, static_cast<int>(cap), st);
+    e = tmp.run(inclusive_sum(cnt, coff, n, st));
     if (e != cudaSuccess) return e;
     launch(OB_FAM_VOXEL, vx_emit_kernel<T>, nb, 256, 0, st, p, w, coff, out, out_n, out_idx, n_out_dev);
     return cudaGetLastError();
@@ -579,14 +548,9 @@ extern "C" ob_status ob_voxel_downsample(const ob_voxel_io* io, ob_stream* s) {
     const size_t esz = io->dtype == OB_F64 ? 8 : 4;
     const size_t cols = io->cols, out_cols = mode == OB_VOXEL_POINT_NORMAL ? 3 : cols;
     VoxelParams p{};
-    const void* d = nullptr;
-    cudaError_t e = stg.in(io->points, cap * cols * esz, &d);
-    p.points = d;
-    if (e == cudaSuccess && mode == OB_VOXEL_POINT_NORMAL) {
-        e = stg.in(io->normals, cap * 3 * esz, &d);
-        p.normals = d;
-    }
-    if (e != cudaSuccess) return fail_cuda(e, "stage voxel inputs");
+    p.points = stg.in(io->points, cap * cols * esz);
+    if (mode == OB_VOXEL_POINT_NORMAL) p.normals = stg.in(io->normals, cap * 3 * esz);
+    if (cudaError_t e = stg.error()) return fail_cuda(e, "stage voxel inputs");
     p.n_dev = r.n_dev;
     p.n_host = r.n_host;
     p.cap = r.cap;
@@ -605,16 +569,13 @@ extern "C" ob_status ob_voxel_downsample(const ob_voxel_io* io, ob_stream* s) {
         p.min_pts = io->min_pts_threshold;
         p.res_sq = io->voxel_size * io->voxel_size / static_cast<double>(io->max_points_per_voxel);  // :39
     }
-    double *dpts = nullptr, *dnrm = nullptr;
-    uint32_t* didx = nullptr;
-    unsigned long long* dcount = nullptr;
-    e = res.array(io->points_out, out_cols * 8, &dpts);
-    if (e == cudaSuccess && mode == OB_VOXEL_POINT_NORMAL) e = res.array(io->normals_out, 3 * 8, &dnrm);
-    if (e == cudaSuccess) e = res.array(io->indices_out, 4, &didx);
-    if (e == cudaSuccess) e = res.word(&dcount);
-    if (e != cudaSuccess) return fail_cuda(e, "stage voxel outputs");
-    e = io->dtype == OB_F64 ? run_voxel<double>(p, stg, st, dpts, dnrm, didx, dcount)
-                            : run_voxel<float>(p, stg, st, dpts, dnrm, didx, dcount);
+    double* dpts = res.array(io->points_out, out_cols * 8);
+    double* dnrm = mode == OB_VOXEL_POINT_NORMAL ? res.array(io->normals_out, 3 * 8) : nullptr;
+    uint32_t* didx = res.array(io->indices_out, 4);
+    unsigned long long* dcount = res.word();
+    if (cudaError_t e = stg.error()) return fail_cuda(e, "stage voxel outputs");
+    cudaError_t e = io->dtype == OB_F64 ? run_voxel<double>(p, stg, st, dpts, dnrm, didx, dcount)
+                                        : run_voxel<float>(p, stg, st, dpts, dnrm, didx, dcount);
     if (e != cudaSuccess) return fail_cuda(e, "voxel downsample launch");
     return res.finish(dcount);
 }

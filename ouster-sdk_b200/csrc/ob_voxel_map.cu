@@ -34,8 +34,6 @@
 // device and later iterations return at once.
 #include <cub/block/block_reduce.cuh>
 #include <cub/block/block_scan.cuh>
-#include <cub/device/device_radix_sort.cuh>
-#include <cub/device/device_scan.cuh>
 
 #include <algorithm>
 #include <cfloat>
@@ -43,6 +41,7 @@
 #include <type_traits>
 
 #include "ob_api_common.h"
+#include "ob_cub.cuh"
 #include "ob_ldlt.cuh"
 #include "ob_rows.cuh"
 #include "ob_voxel_common.cuh"
@@ -808,32 +807,21 @@ template <typename T>
 cudaError_t sort_batch(const ob_voxel_map* m, Rows r, unsigned cols, Staging& stg, cudaStream_t st, AddBatch* b) {
     const unsigned cap = r.cap;
     const unsigned nb = blocks_for(cap);
-    VKey* keys;
-    uint32_t *seq, *opens;
-    cudaError_t e = scratch(stg, cap * sizeof(VKey), &keys);
-    if (e == cudaSuccess) e = scratch(stg, cap * sizeof(VKey), &b->sk);
-    if (e == cudaSuccess) e = scratch(stg, cap * 4ull, &seq);
-    if (e == cudaSuccess) e = scratch(stg, cap * 4ull, &b->sseq);
-    if (e == cudaSuccess) e = scratch(stg, cap * 4ull, &opens);
-    if (e == cudaSuccess) e = scratch(stg, cap * 4ull, &b->vrank);
-    if (e == cudaSuccess) e = scratch(stg, cap * 4ull, &b->seg_start);
-    if (e != cudaSuccess) return e;
-    size_t need = 0, tmp_bytes = 0;
-    e = cub::DeviceRadixSort::SortPairs(nullptr, need, keys, b->sk, seq, b->sseq, static_cast<int>(cap),
-                                        VKeyDecomposer{}, 0, kKeyBits, st);
-    tmp_bytes = need;
-    if (e == cudaSuccess) e = cub::DeviceScan::InclusiveSum(nullptr, need, opens, b->vrank, static_cast<int>(cap), st);
-    tmp_bytes = std::max(tmp_bytes, need);
-    void* tmp = nullptr;
-    if (e == cudaSuccess) e = stg.scratch(tmp_bytes, &tmp);
-    if (e != cudaSuccess) return e;
+    auto* keys = stg.scratch<VKey>(cap);
+    b->sk = stg.scratch<VKey>(cap);
+    auto* seq = stg.scratch<uint32_t>(cap);
+    b->sseq = stg.scratch<uint32_t>(cap);
+    auto* opens = stg.scratch<uint32_t>(cap);
+    b->vrank = stg.scratch<uint32_t>(cap);
+    b->seg_start = stg.scratch<uint32_t>(cap);
+    const auto sort = sort_pairs(keys, b->sk, seq, b->sseq, static_cast<int>(cap), VKeyDecomposer{}, 0, kKeyBits, st);
+    const auto scan = inclusive_sum(opens, b->vrank, static_cast<int>(cap), st);
+    CubTemp tmp(stg, sort, scan);
+    if (cudaError_t e = stg.error()) return e;
     launch(OB_FAM_VOXEL_MAP, vm_key_kernel<T>, nb, 256, 0, st, r, cols, m->inv, keys, seq);
-    e = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, b->sk, seq, b->sseq, static_cast<int>(cap),
-                                        VKeyDecomposer{}, 0, kKeyBits, st);
-    if (e != cudaSuccess) return e;
+    if (cudaError_t e = tmp.run(sort)) return e;
     launch(OB_FAM_VOXEL_MAP, vx_head_kernel, nb, 256, 0, st, cap, b->sk, b->sseq, opens);
-    e = cub::DeviceScan::InclusiveSum(tmp, tmp_bytes, opens, b->vrank, static_cast<int>(cap), st);
-    if (e != cudaSuccess) return e;
+    if (cudaError_t e = tmp.run(scan)) return e;
     launch(OB_FAM_VOXEL_MAP, vx_seg_kernel, nb, 256, 0, st, cap, b->sk, b->sseq, b->vrank, b->seg_start);
     return cudaGetLastError();
 }
@@ -853,31 +841,22 @@ cudaError_t run_emit(const ob_voxel_map* m, const uint32_t* sel, Staging& stg, c
                      size_t capacity, unsigned long long* n_dev) {
     const unsigned cap = m->cap;
     if (cap == 0) return cudaMemsetAsync(n_dev, 0, 8, st);
-    unsigned long long *keys, *skeys;
-    uint32_t *slots, *sslots, *c, *off;
-    cudaError_t e = scratch(stg, cap * 8ull, &keys);
-    if (e == cudaSuccess) e = scratch(stg, cap * 8ull, &skeys);
-    if (e == cudaSuccess) e = scratch(stg, cap * 4ull, &slots);
-    if (e == cudaSuccess) e = scratch(stg, cap * 4ull, &sslots);
-    if (e == cudaSuccess) e = scratch(stg, cap * 4ull, &c);
-    if (e == cudaSuccess) e = scratch(stg, cap * 4ull, &off);
-    if (e != cudaSuccess) return e;
-    size_t need = 0, tmp_bytes = 0;
-    e = cub::DeviceRadixSort::SortPairs(nullptr, need, keys, skeys, slots, sslots, static_cast<int>(cap), 0, 64, st);
-    tmp_bytes = need;
-    if (e == cudaSuccess) e = cub::DeviceScan::InclusiveSum(nullptr, need, c, off, static_cast<int>(cap), st);
-    tmp_bytes = std::max(tmp_bytes, need);
-    void* tmp = nullptr;
-    if (e == cudaSuccess) e = stg.scratch(tmp_bytes, &tmp);
-    if (e != cudaSuccess) return e;
+    auto* keys = stg.scratch<unsigned long long>(cap);
+    auto* skeys = stg.scratch<unsigned long long>(cap);
+    auto* slots = stg.scratch<uint32_t>(cap);
+    auto* sslots = stg.scratch<uint32_t>(cap);
+    auto* c = stg.scratch<uint32_t>(cap);
+    auto* off = stg.scratch<uint32_t>(cap);
+    const auto sort = sort_pairs(keys, skeys, slots, sslots, static_cast<int>(cap), 0, 64, st);
+    const auto scan = inclusive_sum(c, off, static_cast<int>(cap), st);
+    CubTemp tmp(stg, sort, scan);
+    if (cudaError_t e = stg.error()) return e;
     const Table t = table_of(m);
     const unsigned nb = blocks_for(cap);
     launch(OB_FAM_VOXEL_MAP, vm_emit_keys_kernel, nb, 256, 0, st, t, sel, keys, slots);
-    e = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, skeys, slots, sslots, static_cast<int>(cap), 0, 64, st);
-    if (e != cudaSuccess) return e;
+    if (cudaError_t e = tmp.run(sort)) return e;
     launch(OB_FAM_VOXEL_MAP, vm_emit_counts_kernel, nb, 256, 0, st, t, skeys, sslots, c);
-    e = cub::DeviceScan::InclusiveSum(tmp, tmp_bytes, c, off, static_cast<int>(cap), st);
-    if (e != cudaSuccess) return e;
+    if (cudaError_t e = tmp.run(scan)) return e;
     launch(OB_FAM_VOXEL_MAP, vm_emit_kernel, nb, 256, 0, st, t, skeys, sslots, off, out, capacity, n_dev);
     return cudaGetLastError();
 }
@@ -885,10 +864,9 @@ cudaError_t run_emit(const ob_voxel_map* m, const uint32_t* sel, Staging& stg, c
 // rows of the selected voxels of a non-empty map into `out` (null: count only), the count through `res`
 ob_status emit_rows(const ob_voxel_map* m, const uint32_t* sel, Staging& stg, cudaStream_t st, double* out,
                     size_t capacity, CountedRows& res, const char* what) {
-    double* dout = nullptr;
-    unsigned long long* dn = nullptr;
-    cudaError_t e = res.array(out, (3 + m->na) * 8, &dout);
-    if (e == cudaSuccess) e = res.word(&dn);
+    double* dout = res.array(out, (3 + m->na) * 8);
+    unsigned long long* dn = res.word();
+    cudaError_t e = stg.error();
     if (e == cudaSuccess) e = run_emit(m, sel, stg, st, dout, out ? capacity : 0, dn);
     if (e != cudaSuccess) return fail_cuda(e, what);
     return res.finish(dn);
@@ -1016,8 +994,8 @@ ob_status ob_voxel_map_add_rows(ob_voxel_map* m, const ob_map_rows* rows, ob_str
     if (r.cap == 0) return OB_OK;
     cudaStream_t st = stream_handle(s);
     Staging stg(st);
-    cudaError_t e = stg.in(rows->rows, r.cap * rows->cols * 8, &r.p);
-    if (e != cudaSuccess) return fail_cuda(e, "stage voxel map rows");
+    r.p = stg.in(rows->rows, r.cap * rows->cols);
+    if (cudaError_t e = stg.error()) return fail_cuda(e, "stage voxel map rows");
     return add_batch(m, r, static_cast<unsigned>(rows->cols), true, stg, st);
 }
 
@@ -1031,9 +1009,8 @@ ob_status ob_voxel_map_remove_far(ob_voxel_map* m, const ob_voxel_map_cull_io* i
     const bool extract = io->n_extracted != nullptr;
     // the kernel writes a device count itself: it is zeroed here only for an empty map or a refused call
     CountedRows res(io->n_extracted, io->extracted ? io->capacity : CountedRows::kCountOnly, stg, st, "voxel map cull");
-    const void* org = nullptr;
-    cudaError_t e = stg.in(io->origin, 24, &org);
-    if (e != cudaSuccess) return fail_cuda(e, "stage origin");
+    const double* org = stg.in(io->origin, 3);
+    if (cudaError_t e = stg.error()) return fail_cuda(e, "stage origin");
     if (!m->cap) return res.zero();
     if (extract) {  // refused before the cull, so a refused call leaves the map as it was
         rs = res.refuse({io->extracted}, kMixedCount);
@@ -1041,12 +1018,12 @@ ob_status ob_voxel_map_remove_far(ob_voxel_map* m, const ob_voxel_map_cull_io* i
     }
     uint32_t* removed = nullptr;
     if (extract) {
-        e = scratch(stg, m->cap * 4ull, &removed);
-        if (e != cudaSuccess) return fail_cuda(e, "voxel map cull");
+        removed = stg.scratch<uint32_t>(m->cap);
+        if (cudaError_t e = stg.error()) return fail_cuda(e, "voxel map cull");
     }
-    launch(OB_FAM_VOXEL_MAP, vm_cull_kernel, blocks_for(m->cap), 256, 0, st, table_of(m), m->ctr,
-           static_cast<const double*>(org), m->inv, cull_threshold(m->max_distance, m->inv), removed);
-    e = cudaGetLastError();
+    launch(OB_FAM_VOXEL_MAP, vm_cull_kernel, blocks_for(m->cap), 256, 0, st, table_of(m), m->ctr, org, m->inv,
+           cull_threshold(m->max_distance, m->inv), removed);
+    cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail_cuda(e, "voxel map cull");
     if (!extract) return OB_OK;
     return emit_rows(m, removed, stg, st, io->extracted, io->capacity, res, "voxel map extract");
@@ -1091,18 +1068,17 @@ ob_status ob_voxel_map_closest_neighbors(const ob_voxel_map* m, const ob_voxel_q
     rs = stage_rows(&io->queries, stg, &r, "stage queries");
     if (rs != OB_OK || r.cap == 0) return rs;
     if (!io->neighbors) return fail(OB_INVALID_ARGUMENT, "null neighbors buffer");
-    void *nb = nullptr, *d2 = nullptr;
-    cudaError_t e = stg.out(io->neighbors, r.cap * (3 + m->na) * 8ull, &nb);
-    if (e == cudaSuccess) e = stg.out(io->distances_sq, r.cap * 8ull, &d2);
-    if (e != cudaSuccess) return fail_cuda(e, "stage neighbors");
+    double* nb = stg.out(io->neighbors, r.cap * (3 + m->na));
+    double* d2 = stg.out(io->distances_sq, r.cap);
+    if (cudaError_t e = stg.error()) return fail_cuda(e, "stage neighbors");
     const Table t = table_of(m);
     const bool f64 = io->queries.dtype == OB_F64, attr = m->na != 0;
     auto kern = f64 ? (attr ? vm_closest_kernel<double, true> : vm_closest_kernel<double, false>)
                     : (attr ? vm_closest_kernel<float, true> : vm_closest_kernel<float, false>);
-    launch(OB_FAM_VOXEL_MAP, kern, blocks_for(r.cap), 256, 0, st, r, t, m->inv, m->voxel_size, io->max_distance_sq,
-           static_cast<double*>(nb), static_cast<double*>(d2));
-    e = cudaGetLastError();
-    if (e == cudaSuccess) e = stg.flush();
+    launch(OB_FAM_VOXEL_MAP, kern, blocks_for(r.cap), 256, 0, st, r, t, m->inv, m->voxel_size, io->max_distance_sq, nb,
+           d2);
+    stg.check(cudaGetLastError());
+    cudaError_t e = stg.flush();
     if (e != cudaSuccess) return fail_cuda(e, "voxel map closest neighbors");
     return OB_OK;
 }
@@ -1119,24 +1095,20 @@ ob_status ob_icp_linear_system(const ob_icp_system_io* io, ob_stream* s) {
     if (rs != OB_OK) return rs;
     const size_t cap = r.cap;
     if (cap && (!io->source || !io->target)) return fail(OB_INVALID_ARGUMENT, "null pairs buffer");
-    const void *src = nullptr, *tgt = nullptr;
-    void *jtj = nullptr, *jtr = nullptr;
-    cudaError_t e = stg.in(io->source, cap * 24, &src);
-    if (e == cudaSuccess) e = stg.in(io->target, cap * 24, &tgt);
-    if (e == cudaSuccess) e = stg.out(io->jtj, 36 * 8, &jtj);
-    if (e == cudaSuccess) e = stg.out(io->jtr, 6 * 8, &jtr);
+    const double* src = stg.in(io->source, cap * 3);
+    const double* tgt = stg.in(io->target, cap * 3);
+    double* jtj = stg.out(io->jtj, 36);
+    double* jtr = stg.out(io->jtr, 6);
     // a host count travels by value as the clamp (cap == n), a device count is read by the kernels
     const unsigned long long* n = r.n_dev;
     const unsigned slots = tree_slots(cap);
-    double* val = nullptr;
-    if (e == cudaSuccess) e = scratch(stg, slots * kSys * 8ull, &val);
-    if (e != cudaSuccess) return fail_cuda(e, "stage linear system");
-    launch(OB_FAM_ICP, icp_leaf_kernel, blocks_for(slots), 256, 0, st, static_cast<const double*>(src),
-           static_cast<const double*>(tgt), n, cap, io->kernel_scale, nullptr, slots, val);
-    launch(OB_FAM_ICP, icp_system_kernel, 1, kTreeThreads, 0, st, n, cap, val, static_cast<double*>(jtj),
-           static_cast<double*>(jtr));
-    e = cudaGetLastError();
-    if (e == cudaSuccess) e = stg.finish();
+    double* val = stg.scratch<double>(static_cast<size_t>(slots) * kSys);
+    if (cudaError_t e = stg.error()) return fail_cuda(e, "stage linear system");
+    launch(OB_FAM_ICP, icp_leaf_kernel, blocks_for(slots), 256, 0, st, src, tgt, n, cap, io->kernel_scale, nullptr,
+           slots, val);
+    launch(OB_FAM_ICP, icp_system_kernel, 1, kTreeThreads, 0, st, n, cap, val, jtj, jtr);
+    stg.check(cudaGetLastError());
+    cudaError_t e = stg.finish();
     if (e != cudaSuccess) return fail_cuda(e, "icp linear system");
     return OB_OK;
 }
@@ -1150,24 +1122,20 @@ ob_status ob_icp_align(const ob_voxel_map* m, const ob_icp_io* io, ob_stream* s)
     Rows r{};
     rs = stage_rows(&io->source, stg, &r, "stage icp source");
     if (rs != OB_OK) return rs;
-    void *pose = nullptr, *iters = nullptr;
-    IcpState* state = nullptr;
-    cudaError_t e = scratch(stg, sizeof(IcpState), &state);
-    if (e == cudaSuccess) e = stg.out(io->pose, 16 * 8, &pose);
-    if (e == cudaSuccess) e = stg.out(io->iterations, 4, &iters);
+    auto* state = stg.scratch<IcpState>(1);
+    double* pose = stg.out(io->pose, 16);
+    int32_t* iters = stg.out(io->iterations, 1);
     const unsigned cap = std::max(r.cap, 1u);
     const unsigned nb = (cap + kAssocThreads - 1) / kAssocThreads;
     const unsigned slots = tree_slots(cap);
-    double *src = nullptr, *tgt = nullptr, *ps = nullptr, *pt = nullptr, *val = nullptr;
-    uint32_t *valid = nullptr, *bc = nullptr;
-    if (e == cudaSuccess) e = scratch(stg, cap * 24ull, &src);
-    if (e == cudaSuccess) e = scratch(stg, cap * 24ull, &tgt);
-    if (e == cudaSuccess) e = scratch(stg, cap * 24ull, &ps);
-    if (e == cudaSuccess) e = scratch(stg, cap * 24ull, &pt);
-    if (e == cudaSuccess) e = scratch(stg, cap * 4ull, &valid);
-    if (e == cudaSuccess) e = scratch(stg, nb * 4ull, &bc);
-    if (e == cudaSuccess) e = scratch(stg, slots * kSys * 8ull, &val);
-    if (e != cudaSuccess) return fail_cuda(e, "icp workspace");
+    auto* src = stg.scratch<double>(cap * 3ull);
+    auto* tgt = stg.scratch<double>(cap * 3ull);
+    auto* ps = stg.scratch<double>(cap * 3ull);
+    auto* pt = stg.scratch<double>(cap * 3ull);
+    auto* valid = stg.scratch<uint32_t>(cap);
+    auto* bc = stg.scratch<uint32_t>(nb);
+    auto* val = stg.scratch<double>(static_cast<size_t>(slots) * kSys);
+    if (cudaError_t e = stg.error()) return fail_cuda(e, "icp workspace");
     const Table t = table_of(m);
     const double md2 = io->max_distance * io->max_distance;  // square(max_correspondance_distance)
     const double crit_sq = io->convergence_criterion * io->convergence_criterion;
@@ -1183,8 +1151,8 @@ ob_status ob_icp_align(const ob_voxel_map* m, const ob_icp_io* io, ob_stream* s)
                io->kernel_scale, &state->done, slots, val);
         launch(OB_FAM_ICP, icp_solve_kernel, 1, kTreeThreads, 0, st, val, crit_sq, state);
     }
-    launch(OB_FAM_ICP, icp_finish_kernel, 1, 1, 0, st, state, static_cast<double*>(pose), static_cast<int32_t*>(iters));
-    e = cudaGetLastError();
+    launch(OB_FAM_ICP, icp_finish_kernel, 1, 1, 0, st, state, pose, iters);
+    cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail_cuda(e, "icp launch");
     e = stg.finish();  // host pose / iterations: one wait; device ones: nothing waits for the GPU
     if (e != cudaSuccess) return fail_cuda(e, "icp result");

@@ -406,31 +406,27 @@ ob_status ob_zone_render(const ob_zone_render_io* io, ob_stream* s) {
         max_tri = std::max(max_tri, z.n_triangles);
     }
     Staging stg(st);
-    const void *bd = nullptr, *bo = nullptr, *sd = nullptr, *so = nullptr, *tris = nullptr, *zdev = nullptr;
-    void *near = nullptr, *far = nullptr, *flags = nullptr;
-    cudaError_t e = render_smem_opt_in(device);
-    if (e == cudaSuccess) e = stg.in(io->sensor_direction, npx * 3 * 8, &sd);
-    if (e == cudaSuccess) e = stg.in(io->sensor_offset, npx * 3 * 8, &so);
-    if (e == cudaSuccess && have_body) e = stg.in(io->body_direction, npx * 3 * 8, &bd);
-    if (e == cudaSuccess && have_body) e = stg.in(io->body_offset, npx * 3 * 8, &bo);
-    if (e == cudaSuccess) e = stg.in(packed.data(), packed.size() * 4, &tris);
-    if (e == cudaSuccess) e = stg.in(zg.data(), zg.size() * sizeof(ZoneGpu), &zdev);
-    if (e == cudaSuccess) e = stg.out(io->near_mm, npx * io->n_zones * 4, &near);
-    if (e == cudaSuccess) e = stg.out(io->far_mm, npx * io->n_zones * 4, &far);
-    if (e == cudaSuccess) e = stg.scratch(size_t(io->n_zones) * 8, &flags);  // hits, then overflow flags
-    if (e == cudaSuccess) e = cudaMemsetAsync(flags, 0, size_t(io->n_zones) * 8, st);
+    stg.check(render_smem_opt_in(device));
+    const double* sd = stg.in(io->sensor_direction, npx * 3);
+    const double* so = stg.in(io->sensor_offset, npx * 3);
+    const double* bd = have_body ? stg.in(io->body_direction, npx * 3) : nullptr;
+    const double* bo = have_body ? stg.in(io->body_offset, npx * 3) : nullptr;
+    const float* tris = stg.in(packed.data(), packed.size());
+    const ZoneGpu* zdev = stg.in(zg.data(), zg.size());
+    uint32_t* near = stg.out(io->near_mm, npx * io->n_zones);
+    uint32_t* far = stg.out(io->far_mm, npx * io->n_zones);
+    uint32_t* hits = stg.scratch<uint32_t>(size_t(io->n_zones) * 2);  // hits, then overflow flags
+    cudaError_t e = stg.error();
+    if (e == cudaSuccess) e = cudaMemsetAsync(hits, 0, size_t(io->n_zones) * 8, st);
     if (e != cudaSuccess) return fail_cuda(e, "stage zone render");
-    uint32_t* hits = static_cast<uint32_t*>(flags);
     uint32_t* ovf = hits + io->n_zones;
     const dim3 grid(unsigned((npx + kRenderTile - 1) / kRenderTile), io->n_zones);
-    launch(OB_FAM_ZONE, zone_render_kernel, grid, kRenderThreads, size_t(max_tri) * 9 * sizeof(float), st,
-           static_cast<const ZoneGpu*>(zdev), static_cast<const float*>(tris), static_cast<const double*>(bd),
-           static_cast<const double*>(bo), static_cast<const double*>(sd), static_cast<const double*>(so),
-           uint32_t(npx), static_cast<uint32_t*>(near), static_cast<uint32_t*>(far), hits, ovf);
-    e = cudaGetLastError();
+    launch(OB_FAM_ZONE, zone_render_kernel, grid, kRenderThreads, size_t(max_tri) * 9 * sizeof(float), st, zdev, tris,
+           bd, bo, sd, so, uint32_t(npx), near, far, hits, ovf);
     std::vector<uint32_t> hf(size_t(io->n_zones) * 2);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(hf.data(), flags, hf.size() * 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = stg.flush();
+    stg.check(cudaGetLastError());
+    if (!stg.error()) stg.check(cudaMemcpyAsync(hf.data(), hits, hf.size() * 4, cudaMemcpyDeviceToHost, st));
+    e = stg.flush();
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail_cuda(e, "zone render");
     for (uint32_t i = 0; i < io->n_zones; ++i) {
@@ -502,24 +498,18 @@ ob_status ob_zone_monitor_update(ob_zone_monitor* m, const uint32_t* range, uint
     if (rs != OB_OK) return rs;
     cudaStream_t st = stream_handle(s);
     Staging stg(st);
-    const void* r = nullptr;
-    void* bm = nullptr;
-    cudaError_t e = cudaSuccess;
-    if (npx) e = stg.in(range, npx * 4, &r);
+    const uint32_t* r = stg.in(range, npx);
     const bool host_bm = bitmask && !is_device_ptr(bitmask);
-    if (e == cudaSuccess && bitmask && npx) {
-        e = stg.out(bitmask, npx * 4, &bm);  // a host bitmask is read, OR-ed on the device and copied back
-        if (e == cudaSuccess && host_bm) e = cudaMemcpyAsync(bm, bitmask, npx * 4, cudaMemcpyHostToDevice, st);
-    }
-    if (e != cudaSuccess) return fail_cuda(e, "stage zone update");
+    // a host bitmask is read, OR-ed on the device and copied back
+    uint32_t* bm = npx ? stg.inout(bitmask, npx) : nullptr;
+    if (cudaError_t e = stg.error()) return fail_cuda(e, "stage zone update");
     if (npx)
-        launch(OB_FAM_ZONE, zone_occupancy_kernel, unsigned((npx + kOccTile - 1) / kOccTile), kOccThreads, 0, st,
-               static_cast<const uint32_t*>(r), m->near_mm, m->far_mm, m->n_live, uint32_t(npx),
-               static_cast<ZoneAcc*>(m->acc), static_cast<uint32_t*>(bm));
+        launch(OB_FAM_ZONE, zone_occupancy_kernel, unsigned((npx + kOccTile - 1) / kOccTile), kOccThreads, 0, st, r,
+               m->near_mm, m->far_mm, m->n_live, uint32_t(npx), static_cast<ZoneAcc*>(m->acc), bm);
     launch(OB_FAM_ZONE, zone_tail_kernel, 1, 32, 0, st, static_cast<ZoneAcc*>(m->acc), static_cast<ZoneCtl*>(m->ctl),
            m->n_live, m->states);
-    e = cudaGetLastError();
-    if (e == cudaSuccess) e = stg.flush();
+    stg.check(cudaGetLastError());
+    cudaError_t e = stg.flush();
     if (e == cudaSuccess && (host_bm || (npx && !is_device_ptr(range)))) e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail_cuda(e, "zone update");
     return OB_OK;

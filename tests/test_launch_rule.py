@@ -1,5 +1,7 @@
 """Every kernel of the library is launched through ob::launch, which counts it in its family: no `<<<` outside
-that helper's definition in ob_internal.h, and no hand-kept launch tallies."""
+that helper's definition in ob_internal.h, and no hand-kept launch tallies.  Per-call device memory comes from one
+typed Staging, and every CUB device-wide call goes through the helper in ob_cub.cuh that takes its temporary storage
+from there."""
 import os
 import re
 
@@ -25,3 +27,17 @@ def test_every_kernel_launch_goes_through_the_launch_helper():
 
 def test_no_hand_kept_launch_counts():
     assert [name for name, src in _sources() if "count_launch" in src] == []
+
+
+def test_cub_device_calls_go_through_the_cub_helper():
+    assert [name for name, src in _sources() if "cub::Device" in src] == ["ob_cub.cuh"]
+
+
+def test_one_typed_staging():
+    srcs = dict(_sources())
+    assert [name for name, src in srcs.items() if "scratch(stg," in src] == []
+    assert [name for name, src in srcs.items() if re.search(r"auto alloc = \[", src)] == []
+    common = srcs["ob_api_common.h"]
+    staging = common[common.index("class Staging {"):common.index("};", common.index("class Staging {"))]
+    assert "void**" not in staging
+    assert [name for name, src in srcs.items() if re.search(r"if \(e == cudaSuccess[^)]*\) e = (stg|res)\.", src)] == []

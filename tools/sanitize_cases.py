@@ -411,4 +411,40 @@ psp = np.zeros((100, 4, 4))
 ob.core.frames_interp_pose([(tsp, stp, psp), None], 1.0, pkp[0], 1.1, pkp[1])
 ob.core.frames_interp_pose([(tsp, stp, psp)], 0.0, pkp[0])
 print("pose ok")
+# ground segmentation: two frames of different shapes in one set, with NORMALS given and with computed normals
+from oracle import ground as og  # noqa: E402
+from tests import test_gpu_ground as tg  # noqa: E402
+ga, gb = tg._frame("box_rooftop", h=16, w=128, dual=True), tg._frame("room", h=8, w=64, seed=5)
+dg = [tg._gpu_frame(f, normals=tg._normals32(f)) for f in (ga, gb)]
+for f, d, got in zip((ga, gb), dg, ob.core.ground_mask([dg[0], None, dg[1]], model=True)[::2]):
+    tg._assert_same(got, *tg._oracle(f, d), og.FINAL)
+dg = [dict(tg._gpu_frame(f), sensor_to_body=f["sensor_to_body"]) for f in (ga, gb)]
+for f, got in zip((ga, gb), ob.core.ground_mask(dg, model=True)):
+    nrm = tg._oracle_normals(f, got["vertical_subtent"])
+    tg._assert_same(got, *og.run(f["ranges"], f["status"], f["direction"], f["offset"], f["poses"], nrm), og.FINAL)
+print("ground ok")
+# zone monitoring: render of body- and sensor-frame zones, then monitor updates with a host and a device bitmask
+import torch  # noqa: E402
+from tests import test_gpu_zone as tz  # noqa: E402
+tz.render_both(ob, tz.subsample(tz.sensor_meta("785.json"), 16, 128), [(tz.stl_tris("0.stl"), f) for f in (1, 2)],
+               tz.s2b_z1())
+tz.ZSD = ob.core.ZONE_STATE_DTYPE
+zh, zw = 8, 64
+zones = tz.random_zones(zh, zw, 3, 1)
+mon = ob.ZoneMonitor([{"id": z[0], "mode": z[1], "point_count": z[2], "frame_count": z[3], "near_mm": z[4],
+                       "far_mm": z[5]} for z in zones], zh, zw)
+ref = tz.RefZoneMon(zones)
+for f in range(4):
+    r = tz.random_range(zones, zh, zw, f)
+    want_bm = np.zeros((zh, zw), np.uint32)
+    want = ref.calc(r, want_bm)
+    if f % 2:
+        bm = torch.zeros((zh, zw), dtype=torch.int32, device="cuda")
+        mon.update(torch.from_numpy(r.view(np.int32)).cuda(), bm)
+        bm = bm.cpu().numpy().view(np.uint32)
+    else:
+        bm = np.zeros((zh, zw), np.uint32)
+        mon.update(r, bm)
+    assert np.array_equal(mon.states(), want) and np.array_equal(bm, want_bm), f
+print("zone ok")
 print("SANITIZE CASES OK")
