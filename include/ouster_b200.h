@@ -55,7 +55,7 @@ int ob_abi_version(void);
  * "ob_cloud_align_io", "ob_cloud_nearest_io", "ob_zone_desc", "ob_zone_render_io", "ob_zone_live", "ob_zone_state",
  * "ob_image_params", "ob_image_state", "ob_frame_field", "ob_frame_ops_io", "ob_frame_rows_entry",
  * "ob_frame_rows_io", "ob_map_rows", "ob_map_field", "ob_map_rows_item", "ob_interp_pose_io",
- * "ob_frame_poses_item", "ob_ground_model", "ob_ground_item");
+ * "ob_frame_poses_item", "ob_ground_model", "ob_ground_item", "ob_align_clouds_trace", "ob_align_clouds_io");
  * 0 for unknown names.  Lets FFI bindings verify their layout. */
 size_t ob_abi_sizeof(const char* struct_name);
 const char* ob_last_error(void);
@@ -644,6 +644,68 @@ typedef struct ob_cloud_nearest_io {
     int32_t* indices;
 } ob_cloud_nearest_io;
 ob_status ob_cloud_nearest(const ob_cloud_nearest_io* io, ob_stream* s);
+
+/* ---- global cloud alignment (DESIGN f-14) ---- */
+#define OB_ALIGN_COARSE_YAWS 180  /* pass 1: 2 degree steps */
+#define OB_ALIGN_FINE_YAWS 7      /* pass 2: 1 degree steps, +-3 degrees around the best coarse yaw */
+#define OB_ALIGN_Z_BINS 1024      /* Z histogram: 0.2 m bins */
+#define OB_ALIGN_MAX_FINE_BASE 481   /* largest fine grid side (60 m bound, 0.25 m pixels) */
+#define OB_ALIGN_MAX_COARSE_BASE 241 /* largest coarse grid side (60 m bound, 0.5 m pixels) */
+
+/* What one ob_align_clouds call decided, for tests and diagnostics.  Z shifts are in 0.2 m bins, dx / dy in fine
+ * pixels; scores are the peak of the normalised cross-correlation (0 for an empty grid).  Poses are row-major 4x4.
+ * With fewer than 20 feature points in either cloud only the feature counts are set (searched = 0).  The three
+ * optional host buffers receive the target's un-normalised BEV grids (row y of the grid is row y of the buffer,
+ * base_n x base_n, so they must hold OB_ALIGN_MAX_*_BASE^2 doubles) and its Z histogram. */
+typedef struct ob_align_clouds_trace {
+    size_t source_features, target_features;
+    int32_t searched, coarse_index, fine_index, pad;
+    double bound_m, fine_pixel_m, coarse_pixel_m, max_shift_m;
+    int32_t fine_base_n, fine_fft_n, fine_max_shift; /* max_shift: the window half-width in pixels */
+    int32_t coarse_base_n, coarse_fft_n, coarse_max_shift;
+    double coarse_scores[OB_ALIGN_COARSE_YAWS];
+    int32_t fine_z_bins[OB_ALIGN_FINE_YAWS], fine_dx[OB_ALIGN_FINE_YAWS], fine_dy[OB_ALIGN_FINE_YAWS], pad2;
+    double fine_scores[OB_ALIGN_FINE_YAWS];
+    double initial_pose[16]; /* the yaw search's result */
+    double icp_poses[48];    /* after the ICP passes at 2.0, 0.6 and 0.25 m */
+    double initial_confidence, refined_confidence;
+    size_t initial_matched, initial_total, refined_matched, refined_total;
+    double stage_ms[5]; /* device time (CUDA events) of features, pass 1 (with the target's grids and the Z shift),
+                           pass 2, ICP and confidence */
+    double* target_fine_grid;   /* optional */
+    double* target_coarse_grid; /* optional */
+    double* target_z_hist;      /* optional, OB_ALIGN_Z_BINS doubles */
+} ob_align_clouds_trace;
+
+/* replaces the six point-cloud overloads of algorithm::align_clouds
+ *          ouster_algorithm/src/align_clouds.cpp:396-1581, 1876-1995, 2601-2651 (declared in align_clouds.h:183-320)
+ * source / target: rows of one dtype, host or device, with n or a device-resident count (as ob_cloud_align).
+ * *_cols / *_normal_cols: the columns of the caller's arrays (must be 3).  Normals (rows x 3 of the points' dtype)
+ * are optional and must be given for both clouds or for neither.  initial_guess: 16 doubles, row-major, host or
+ * device (NULL: the identity).  pose: 16 doubles out; confidence (optional): 1 double out, 0 unless
+ * compute_confidence.  trace (optional): host ob_align_clouds_trace.
+ * The call waits once for the GPU, to read the feature counts, the footprints and the guess that size the grids
+ * and the FFT launches, so it cannot be captured in a CUDA graph.  Host outputs (and a trace) are delivered with
+ * the usual closing synchronisation.
+ * errors (OB_INVALID_ARGUMENT, checked in this order): "source_points must have shape (N, 3)",
+ * "source_normals must have shape (N, 3)", "source_points and source_normals must have the same number of rows",
+ * the same three for the target, "source_normals and target_normals must both be given or both be omitted";
+ * then OB_NO_DEVICE without a GPU. */
+typedef struct ob_align_clouds_io {
+    ob_point_rows source;
+    ob_point_rows target;
+    size_t source_cols, target_cols;
+    const void* source_normals; /* optional */
+    size_t source_normal_rows, source_normal_cols;
+    const void* target_normals; /* optional */
+    size_t target_normal_rows, target_normal_cols;
+    const double* initial_guess;
+    int32_t compute_confidence;
+    double* pose;
+    double* confidence;
+    ob_align_clouds_trace* trace;
+} ob_align_clouds_io;
+ob_status ob_align_clouds(const ob_align_clouds_io* io, ob_stream* s);
 
 /* ---- zone monitoring (DESIGN f-8) ---- */
 #define OB_ZONE_MAX_TRIANGLES 2048 /* Zone::MAX_TRIANGLES */

@@ -138,6 +138,37 @@ class CloudAlignIO(C.Structure):
                 ("pose", vp), ("iterations", vp)]
 
 
+OB_ALIGN_COARSE_YAWS, OB_ALIGN_FINE_YAWS, OB_ALIGN_Z_BINS = 180, 7, 1024
+OB_ALIGN_MAX_FINE_BASE, OB_ALIGN_MAX_COARSE_BASE = 481, 241
+
+
+class AlignCloudsTrace(C.Structure):
+    """ob_align_clouds_trace"""
+    _fields_ = [("source_features", sz), ("target_features", sz),
+                ("searched", C.c_int32), ("coarse_index", C.c_int32), ("fine_index", C.c_int32), ("pad", C.c_int32),
+                ("bound_m", C.c_double), ("fine_pixel_m", C.c_double), ("coarse_pixel_m", C.c_double),
+                ("max_shift_m", C.c_double),
+                ("fine_base_n", C.c_int32), ("fine_fft_n", C.c_int32), ("fine_max_shift", C.c_int32),
+                ("coarse_base_n", C.c_int32), ("coarse_fft_n", C.c_int32), ("coarse_max_shift", C.c_int32),
+                ("coarse_scores", C.c_double * OB_ALIGN_COARSE_YAWS),
+                ("fine_z_bins", C.c_int32 * OB_ALIGN_FINE_YAWS), ("fine_dx", C.c_int32 * OB_ALIGN_FINE_YAWS),
+                ("fine_dy", C.c_int32 * OB_ALIGN_FINE_YAWS), ("pad2", C.c_int32),
+                ("fine_scores", C.c_double * OB_ALIGN_FINE_YAWS),
+                ("initial_pose", C.c_double * 16), ("icp_poses", C.c_double * 48),
+                ("initial_confidence", C.c_double), ("refined_confidence", C.c_double),
+                ("initial_matched", sz), ("initial_total", sz), ("refined_matched", sz), ("refined_total", sz),
+                ("stage_ms", C.c_double * 5), ("target_fine_grid", vp), ("target_coarse_grid", vp), ("target_z_hist", vp)]
+
+
+class AlignCloudsIO(C.Structure):
+    """ob_align_clouds_io"""
+    _fields_ = [("source", PointRows), ("target", PointRows), ("source_cols", sz), ("target_cols", sz),
+                ("source_normals", vp), ("source_normal_rows", sz), ("source_normal_cols", sz),
+                ("target_normals", vp), ("target_normal_rows", sz), ("target_normal_cols", sz),
+                ("initial_guess", vp), ("compute_confidence", C.c_int32), ("pose", vp), ("confidence", vp),
+                ("trace", C.POINTER(AlignCloudsTrace))]
+
+
 class CloudNearestIO(C.Structure):
     _fields_ = [("target", PointRows), ("target_normals", vp), ("queries", PointRows), ("cell_size", C.c_double),
                 ("max_dist_sq", C.c_double), ("indices", vp)]
@@ -313,6 +344,7 @@ _sig("ob_icp_align", i32, vp, C.POINTER(IcpIO), vp)
 _sig("ob_icp_linear_system", i32, C.POINTER(IcpSystemIO), vp)
 _sig("ob_cloud_align", i32, C.POINTER(CloudAlignIO), vp)
 _sig("ob_cloud_nearest", i32, C.POINTER(CloudNearestIO), vp)
+_sig("ob_align_clouds", i32, C.POINTER(AlignCloudsIO), vp)
 _sig("ob_zone_render", i32, C.POINTER(ZoneRenderIO), vp)
 _sig("ob_zone_monitor_create", i32, i32, u32, u32, C.POINTER(ZoneLive), u32, C.POINTER(vp))
 _sig("ob_zone_monitor_update", i32, vp, vp, vp, vp)

@@ -900,6 +900,100 @@ def cloud_nearest(target, queries, cell_size, max_dist_sq, target_normals=None, 
     return out
 
 
+def _align_clouds_input(a, ref=None):
+    """(array kept for the call, its columns): numpy or torch rows of float32 / float64; with `ref`, in ref's dtype
+    and memory."""
+    if ref is not None:
+        if _is_torch(ref):
+            import torch
+            a = torch.as_tensor(a, device=ref.device)
+        elif _is_torch(a):
+            a = a.cpu().numpy()
+        a = _contig(a, _np_dtype(ref))
+    else:
+        a = _contig(a, floats=True)
+    cols = int(a.shape[1]) if len(a.shape) == 2 else 0
+    return a, cols
+
+
+def align_clouds(source, target, source_normals=None, target_normals=None, initial_guess=None,
+                 compute_confidence=False, n_source=None, n_target=None, trace=False, stream=None):
+    """The point-cloud overloads of algorithm::align_clouds on the GPU (ob_align_clouds): (pose [4, 4] float64,
+    confidence), plus a dict of ob_align_clouds_trace (with the target's raw BEV grids and Z histogram) when
+    trace=True.  Normals are optional, for both clouds or neither.  CUDA-tensor clouds give a CUDA pose [4, 4] and
+    confidence [1] (both float64); n_source / n_target: optional device-resident row counts (e.g. voxel_downsample's
+    count), the arrays then holding `capacity` rows.  initial_guess (identity when None) may be a CUDA tensor."""
+    from ._capi import AlignCloudsIO, AlignCloudsTrace
+    s, s_cols = _align_clouds_input(source)
+    if _is_torch(s) != _is_torch(target):
+        raise ValueError("source and target must live in the same memory")
+    t, t_cols = _align_clouds_input(target, s)
+    io = AlignCloudsIO()
+    io.source_cols, io.target_cols = s_cols, t_cols
+    keep = [s, t]
+    for rows, arr, n in ((io.source, s, n_source), (io.target, t, n_target)):
+        rows.dtype = _capi.OB_F64 if _np_dtype(arr) == np.float64 else _capi.OB_F32
+        rows.points = _ptr(arr)
+        if n is None:
+            rows.n = int(arr.shape[0]) if len(arr.shape) else 0
+        else:
+            rows.n_device, rows.capacity = _device_rows(n, arr), int(arr.shape[0])
+    if source_normals is not None:
+        sn, io.source_normal_cols = _align_clouds_input(source_normals, s)
+        io.source_normals, io.source_normal_rows = _ptr(sn), int(sn.shape[0]) if len(sn.shape) else 0
+        keep.append(sn)
+    if target_normals is not None:
+        tn, io.target_normal_cols = _align_clouds_input(target_normals, t)
+        io.target_normals, io.target_normal_rows = _ptr(tn), int(tn.shape[0]) if len(tn.shape) else 0
+        keep.append(tn)
+    g = None
+    if initial_guess is not None:
+        g = _contig(initial_guess, np.float64)
+        if _numel(g) != 16:
+            raise ValueError("initial_guess must be 4x4")
+        io.initial_guess = _ptr(g)
+    io.compute_confidence = int(bool(compute_confidence))
+    pose, conf = _empty(s, (4, 4), np.float64), _empty(s, (1,), np.float64)
+    io.pose, io.confidence = _ptr(pose), _ptr(conf)
+    tr, bufs = None, None
+    if trace:
+        tr = AlignCloudsTrace()
+        bufs = (np.zeros(_capi.OB_ALIGN_MAX_FINE_BASE ** 2), np.zeros(_capi.OB_ALIGN_MAX_COARSE_BASE ** 2),
+                np.zeros(_capi.OB_ALIGN_Z_BINS))
+        tr.target_fine_grid, tr.target_coarse_grid, tr.target_z_hist = (b.ctypes.data for b in bufs)
+        io.trace = C.pointer(tr)
+    # ob_align_clouds checks these too, in this order; here they also hold on a machine without a GPU (no stream to
+    # create yet)
+    for p, nrm, pc, nc, rows in (("source", source_normals, s_cols, io.source_normal_cols, io.source_normal_rows),
+                                 ("target", target_normals, t_cols, io.target_normal_cols, io.target_normal_rows)):
+        if pc != 3:
+            raise ValueError(f"{p}_points must have shape (N, 3)")
+        if nrm is not None and nc != 3:
+            raise ValueError(f"{p}_normals must have shape (N, 3)")
+        pr = io.source if p == "source" else io.target
+        if nrm is not None and rows != (pr.capacity if pr.n_device else pr.n):
+            raise ValueError(f"{p}_points and {p}_normals must have the same number of rows")
+    if (source_normals is None) != (target_normals is None):
+        raise ValueError("source_normals and target_normals must both be given or both be omitted")
+    check(lib.ob_align_clouds(C.byref(io), _stream_for(s, stream).h))
+    out = (pose, conf) if _is_torch(conf) else (pose, float(conf[0]))
+    if not trace:
+        return out
+    d = {name: getattr(tr, name) for name, _ in AlignCloudsTrace._fields_
+         if not name.startswith("pad") and not name.endswith(("_grid", "_hist"))}
+    for k in ("coarse_scores", "fine_scores", "initial_pose", "icp_poses", "stage_ms"):
+        d[k] = np.array(d[k][:], np.float64)
+    for k in ("fine_z_bins", "fine_dx", "fine_dy"):
+        d[k] = np.array(d[k][:], np.int32)
+    d["initial_pose"] = d["initial_pose"].reshape(4, 4)
+    d["icp_poses"] = d["icp_poses"].reshape(3, 4, 4)
+    fb, cb = tr.fine_base_n, tr.coarse_base_n
+    d["target_fine_grid"] = bufs[0][:fb * fb].reshape(fb, fb).copy() if tr.searched else None
+    d["target_coarse_grid"] = bufs[1][:cb * cb].reshape(cb, cb).copy() if tr.searched else None
+    d["target_z_hist"] = bufs[2].copy() if tr.searched else None
+    return out + (d,)
+
+
 def icp_linear_system(source, target, kernel_scale, stream=None, device=0):
     """build_linear_system(correspondences, kernel_scale) (icp_registration.cpp) on the GPU with the reference's
     deterministic-reduce tree: (jtj [6, 6], lower triangle, jtr [6]) float64 numpy arrays."""

@@ -386,6 +386,8 @@ size_t ob_abi_sizeof(const char* name) {
     if (n == "ob_frame_poses_item") return sizeof(ob_frame_poses_item);
     if (n == "ob_ground_model") return sizeof(ob_ground_model);
     if (n == "ob_ground_item") return sizeof(ob_ground_item);
+    if (n == "ob_align_clouds_trace") return sizeof(ob_align_clouds_trace);
+    if (n == "ob_align_clouds_io") return sizeof(ob_align_clouds_io);
     return 0;
 }
 

@@ -755,7 +755,32 @@ def point_to_plane_align(source_points, target_points, source_normals, target_no
     return pose
 
 
-# ---- zone monitoring (DESIGN f-8) -----------------------------------------------------------------------------
+def align_clouds(*args, initial_guess=None, compute_confidence=False):
+    """source_to_target_transform between two point clouds without a usable initial guess (DESIGN f-14):
+    align_clouds(source_points, target_points, initial_guess=None, compute_confidence=False) or
+    align_clouds(source_points, source_normals, target_points, target_normals, initial_guess=None,
+    compute_confidence=False), dispatched on the number of arrays as the reference's two bindings are.  A yaw search
+    by BEV cross-correlation, three ICP passes, and the overlap confidence as a guard.  Returns the 4x4 pose, or
+    (pose, confidence) with compute_confidence."""
+    # (sp, tp, initial_guess, compute_confidence) has a flag where (sp, sn, tp, tn) has an array
+    n_arrays = 4 if len(args) >= 4 and getattr(args[3], "ndim", np.ndim(args[3])) >= 1 else 2
+    if len(args) < 2 or len(args) > n_arrays + 2:
+        raise TypeError("align_clouds() takes 2 or 4 point arrays, then initial_guess and compute_confidence")
+    rest = list(args[n_arrays:])
+    if rest:
+        initial_guess = rest.pop(0)
+    if rest:
+        compute_confidence = rest.pop(0)
+    if n_arrays == 4:
+        sp, sn, tp, tn = args[:4]
+    else:
+        (sp, tp), sn, tn = args[:2], None, None
+    pose, conf = _c.align_clouds(sp, tp, sn, tn, initial_guess=initial_guess,
+                                 compute_confidence=compute_confidence)
+    return (pose, conf) if compute_confidence else pose
+
+
+# ---- zone monitoring (DESIGN f-8)-----------------------------------------------------------------------------
 # ouster.sdk.core's Mesh / Stl / Zone / ZoneSet / Zrb (python/src/cpp/client/zone_monitor.cpp) and EmulatedZoneMon
 # (python/src/ouster/sdk/core/zone_common.py).  Rendering and the per-frame occupancy run on the GPU; STL parsing
 # is host code.  ZRB / ZoneSet files, hashes and JSON are not provided (DESIGN 9).
