@@ -29,7 +29,6 @@
 
 #include <algorithm>
 #include <cfloat>
-#include <climits>
 #include <cmath>
 
 #include "ob_api_common.h"
@@ -51,20 +50,6 @@ constexpr unsigned kLeaf = 32;                    // pairs per leaf of the summa
 constexpr unsigned kTreeThreads = 256;
 constexpr unsigned long long kPadKey = ~0ull;     // sorts after every |r|
 constexpr int kPair = 7;                          // x (3), q or n_tgt (3), r
-
-__device__ __forceinline__ bool finite3(const double* v) { return isfinite(v[0]) && isfinite(v[1]) && isfinite(v[2]); }
-__device__ __forceinline__ double dot3(const double* a, const double* b) {
-    return add(add(mul(a[0], b[0]), mul(a[1], b[1])), mul(a[2], b[2]));
-}
-__device__ __forceinline__ double max_d(double a, double b) { return a < b ? b : a; }  // std::max
-__device__ __forceinline__ double min_d(double a, double b) { return b < a ? b : a; }  // std::min
-
-// static_cast<int64_t>(std::floor(v)) as x86 cvttsd2si evaluates it (the device conversion saturates instead)
-__device__ __forceinline__ int64_t cell_coord(double v) {
-    const double f = floor(v);
-    if (!(f >= -9223372036854775808.0 && f < 9223372036854775808.0)) return INT64_MIN;
-    return static_cast<int64_t>(f);
-}
 
 // ---- SpatialHashGrid3D ----
 struct GKey {
@@ -116,7 +101,9 @@ __global__ void gr_key_kernel(Rows t, const void* normals, double inv, GKey* key
             load3<T>(normals, i, nn);
             ok = finite3(nn) && norm3(nn) > kNormalEps;
         }
-        if (ok) k = GKey{0u, cell_coord(mul(p[0], inv)), cell_coord(mul(p[1], inv)), cell_coord(mul(p[2], inv))};
+        if (ok)
+            k = GKey{0u, floor_cast<int64_t>(mul(p[0], inv)), floor_cast<int64_t>(mul(p[1], inv)),
+                     floor_cast<int64_t>(mul(p[2], inv))};
     }
     keys[i] = k;
     seq[i] = i;
@@ -163,7 +150,8 @@ __device__ __forceinline__ int grid_find(const Grid& g, int64_t x, int64_t y, in
 // a cell's rows in ascending index, the first strictly smaller squared distance kept
 __device__ int grid_nearest(const Grid& g, const double* q, double max_dist_sq) {
     if (!finite3(q) || !isfinite(max_dist_sq) || max_dist_sq <= 0.0) return -1;
-    const int64_t c[3] = {cell_coord(mul(q[0], g.inv)), cell_coord(mul(q[1], g.inv)), cell_coord(mul(q[2], g.inv))};
+    const int64_t c[3] = {floor_cast<int64_t>(mul(q[0], g.inv)), floor_cast<int64_t>(mul(q[1], g.inv)),
+                          floor_cast<int64_t>(mul(q[2], g.inv))};
     int best = -1;
     double best_d2 = max_dist_sq;
     for (int dx = -1; dx <= 1; ++dx)
@@ -196,14 +184,6 @@ __global__ void al_nearest_kernel(Rows q, Grid g, double max_dist_sq, int32_t* o
 }
 
 // ---- small dense pieces (DESIGN 2: products sum over k in index order, norms are sqrt of sqn3) ----
-// x = R p + t, and R p, for the top 3 x 4 of a row-major pose
-__device__ __forceinline__ void transform(const double* P, const double* p, double* x) {
-    for (int d = 0; d < 3; ++d)
-        x[d] = add(add(add(mul(P[4 * d], p[0]), mul(P[4 * d + 1], p[1])), mul(P[4 * d + 2], p[2])), P[4 * d + 3]);
-}
-__device__ __forceinline__ void rotate(const double* P, const double* p, double* x) {
-    for (int d = 0; d < 3; ++d) x[d] = add(add(mul(P[4 * d], p[0]), mul(P[4 * d + 1], p[1])), mul(P[4 * d + 2], p[2]));
-}
 // a = b * a, row-major 4 x 4 (PoseH(delta) * current_pose)
 __device__ void pose_premul(const double* b, double* a) {
     double r[16];
@@ -262,13 +242,13 @@ __device__ bool svd3(const double* A, double u[3][3], double v[3][3]) {
             u[i][j] = v[i][j] = i == j ? 1.0 : 0.0;
         }
     const double precision = mul(2.0, DBL_EPSILON);
-    double max_diag = max_d(max_d(fabs(w[0][0]), fabs(w[1][1])), fabs(w[2][2]));
+    double max_diag = smax(smax(fabs(w[0][0]), fabs(w[1][1])), fabs(w[2][2]));
     bool finished = false;
     for (int sweep = 0; !finished && sweep < kJacobiMaxSweeps; ++sweep) {
         finished = true;
         for (int p = 1; p < 3; ++p)
             for (int q = 0; q < p; ++q) {
-                const double threshold = max_d(DBL_MIN, mul(precision, max_diag));
+                const double threshold = smax(DBL_MIN, mul(precision, max_diag));
                 if (!(fabs(w[p][q]) > threshold || fabs(w[q][p]) > threshold)) continue;
                 finished = false;
                 const double m00 = w[p][p], m01 = w[p][q], m10 = w[q][p], m11 = w[q][q];
@@ -292,7 +272,7 @@ __device__ bool svd3(const double* A, double u[3][3], double v[3][3]) {
                 rot_cols(u, p, q, cl, sl);
                 rot_cols(w, p, q, cr, -sr);
                 rot_cols(v, p, q, cr, -sr);
-                max_diag = max_d(max_diag, max_d(fabs(w[p][p]), fabs(w[q][q])));
+                max_diag = smax(max_diag, smax(fabs(w[p][p]), fabs(w[q][q])));
             }
     }
     double s[3];
@@ -366,7 +346,7 @@ __global__ void al_assoc_kernel(Rows src, const void* snrm, const void* tgt, con
         }
         if (use) {
             double x[3];
-            transform(P, p, x);
+            mat4_transform(P, p, x);
             const int j = grid_nearest(g, x, max_d2);
             if (j >= 0) {
                 double q[3], v[3];
@@ -378,7 +358,7 @@ __global__ void al_assoc_kernel(Rows src, const void* snrm, const void* tgt, con
                     for (int d = 0; d < 3; ++d) v[d] = q[d];
                 } else {
                     double nw[3];
-                    rotate(P, ns, nw);
+                    mat4_rotate(P, ns, nw);
                     load3<T>(tnrm, j, v);
                     const double tn = norm3(v);
                     if (finite3(v) && tn > kNormalEps) {
@@ -413,27 +393,9 @@ __global__ void al_assoc_kernel(Rows src, const void* snrm, const void* tgt, con
 __global__ void al_compact_kernel(unsigned kcap, const double* rows, const uint32_t* valid, const uint32_t* block_count,
                                   double* pairs, AlignState* st) {
     if (st->done) return;
-    using BR = cub::BlockReduce<unsigned, kThreads>;
-    using BS = cub::BlockScan<unsigned, kThreads>;
-    __shared__ union {
-        typename BR::TempStorage r;
-        typename BS::TempStorage s;
-    } tmp;
-    __shared__ unsigned base;
-    unsigned part = 0;
-    for (unsigned b = threadIdx.x; b < blockIdx.x; b += blockDim.x) part += block_count[b];
-    const unsigned before = BR(tmp.r).Sum(part);
-    if (threadIdx.x == 0) base = before;
-    __syncthreads();
-    const unsigned i = tid_global();
-    const unsigned f = i < kcap ? valid[i] : 0u;
-    unsigned pos, total;
-    BS(tmp.s).ExclusiveSum(f, pos, total);
-    if (f) {
-        const size_t o = static_cast<size_t>(base) + pos;
+    compact_rows<kThreads>(kcap, valid, block_count, &st->n_pairs, [&](unsigned i, size_t o) {
         for (int d = 0; d < kPair; ++d) pairs[kPair * o + d] = rows[kPair * static_cast<size_t>(i) + d];
-    }
-    if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) st->n_pairs = base + total;
+    });
 }
 
 // median_abs over the sorted keys, then the MAD-scaled Huber threshold (align_clouds.cpp:1650-1655)
@@ -442,7 +404,7 @@ __device__ double huber_delta(unsigned long long n, const unsigned long long* sk
     const double hi = __longlong_as_double(static_cast<long long>(skeys[mid]));
     const double mad = (n & 1ull) ? hi : mul(0.5, add(__longlong_as_double(static_cast<long long>(skeys[mid - 1])), hi));
     double sigma = mul(1.4826, mad);
-    if (!isfinite(sigma) || sigma < 1e-4) sigma = max_d(1e-3, mul(0.25, max_corr_dist));
+    if (!isfinite(sigma) || sigma < 1e-4) sigma = smax(1e-3, mul(0.25, max_corr_dist));
     return mul(1.5, sigma);
 }
 __device__ __forceinline__ double huber_w(double r, double delta) {
@@ -582,7 +544,7 @@ __global__ void __launch_bounds__(kTreeThreads, 1) al_p2p_solve_kernel(double* v
     }
     const double D[16] = {R[0], R[1], R[2], dt[0], R[3], R[4], R[5], dt[1], R[6], R[7], R[8], dt[2], 0.0, 0.0, 0.0, 1.0};
     pose_premul(D, st->pose);
-    const double trace_term = max_d(-1.0, min_d(mul(0.5, sub(add(add(R[0], R[4]), R[8]), 1.0)), 1.0));
+    const double trace_term = smax(-1.0, smin(mul(0.5, sub(add(add(R[0], R[4]), R[8]), 1.0)), 1.0));
     if (acos(trace_term) < 1e-4 && norm3(dt) < 1e-3) st->done = 1;
 }
 

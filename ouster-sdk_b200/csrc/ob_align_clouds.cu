@@ -76,25 +76,6 @@ constexpr double kCoarsePixel = 0.5;
 constexpr size_t kMinPoints = 20;
 constexpr unsigned kConfSamples = 16000;
 
-__device__ __forceinline__ bool finite3(const double* v) { return isfinite(v[0]) && isfinite(v[1]) && isfinite(v[2]); }
-__device__ __forceinline__ double max_d(double a, double b) { return a < b ? b : a; }  // std::max
-__device__ __forceinline__ double min_d(double a, double b) { return b < a ? b : a; }  // std::min
-// order-preserving uint64 image of a double (-0.0 sorts below +0.0) and back
-__device__ __forceinline__ unsigned long long okey(double v) {
-    const unsigned long long b = static_cast<unsigned long long>(__double_as_longlong(v));
-    return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
-}
-__device__ __forceinline__ double okey_value(unsigned long long k) {
-    return __longlong_as_double(static_cast<long long>((k >> 63) ? (k & 0x7fffffffffffffffull) : ~k));
-}
-__device__ __forceinline__ void transform(const double* P, const double* p, double* x) {
-    for (int d = 0; d < 3; ++d)
-        x[d] = add(add(add(mul(P[4 * d], p[0]), mul(P[4 * d + 1], p[1])), mul(P[4 * d + 2], p[2])), P[4 * d + 3]);
-}
-__device__ __forceinline__ void rotate(const double* P, const double* p, double* x) {
-    for (int d = 0; d < 3; ++d) x[d] = add(add(mul(P[4 * d], p[0]), mul(P[4 * d + 1], p[1])), mul(P[4 * d + 2], p[2]));
-}
-
 // ---- device state of one call ----
 struct Filter {  // build_xy_bev_grid's floor / ceiling band
     int on;
@@ -186,7 +167,7 @@ __global__ void ac_keys_kernel(const double* fp, const unsigned long long* nf, u
     }
     const double* p = fp + 3 * static_cast<size_t>(i);
     dist[i] = norm3(p);
-    ekey[i] = okey(max_d(fabs(p[0]), fabs(p[1])));
+    ekey[i] = okey(smax(fabs(p[0]), fabs(p[1])));
     zkey[i] = okey(p[2]);
 }
 
@@ -239,8 +220,8 @@ __global__ void ac_items_kernel(const double* fp, const double* fn, const double
     const double* p = fp + 3 * static_cast<size_t>(i);
     const double* q = fn ? fn + 3 * static_cast<size_t>(i) : nullptr;
     if (poses) {
-        transform(poses + 16 * g, p, x);
-        if (q) rotate(poses + 16 * g, q, m);
+        mat4_transform(poses + 16 * g, p, x);
+        if (q) mat4_rotate(poses + 16 * g, q, m);
     } else {
         for (int d = 0; d < 3; ++d) {
             x[d] = p[d];
@@ -528,7 +509,7 @@ __global__ void __launch_bounds__(kThreads) ac_zshift_kernel(const double* hm, c
         }
     }
     st->zbins = best_shift;
-    st->dz = max_d(-4.0, min_d(mul(kPitch, static_cast<double>(best_shift)), 4.0));
+    st->dz = smax(-4.0, smin(mul(kPitch, static_cast<double>(best_shift)), 4.0));
     st->filt_s = filter_of(st->zstat[0], add(g23, st->dz));
 }
 

@@ -692,14 +692,8 @@ cudaError_t launch_cloud(const CloudArgs<T>& a, int device, cudaStream_t st) {
 // dewarp / transform: out[i*W + w] = R_w * p[i*W + w] + t_w  (pose_util.h:37-59, 118-131).
 // A CTA stages the 3x4 parts of 128 consecutive column poses in shared memory and sweeps a band of
 // rows; lane = column, so point loads/stores are contiguous 384-byte runs per warp.
-// Products are rounded separately and summed as x0 + (x1 + x2), then + t (no FMA contraction).
+// Each row is ob_project.cuh's pose_row: products rounded separately, summed as x0 + (x1 + x2), then + t.
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ float madd3(float a0, float b0, float a1, float b1, float a2, float b2, float t) {
-    return __fadd_rn(__fadd_rn(__fmul_rn(a0, b0), __fadd_rn(__fmul_rn(a1, b1), __fmul_rn(a2, b2))), t);
-}
-__device__ __forceinline__ double madd3(double a0, double b0, double a1, double b1, double a2, double b2, double t) {
-    return __dadd_rn(__dadd_rn(__dmul_rn(a0, b0), __dadd_rn(__dmul_rn(a1, b1), __dmul_rn(a2, b2))), t);
-}
 
 template <typename T>
 __global__ void __launch_bounds__(256) dewarp_kernel(const T* __restrict__ pts, const T* __restrict__ poses,
@@ -720,9 +714,9 @@ __global__ void __launch_bounds__(256) dewarp_kernel(const T* __restrict__ pts, 
     for (unsigned long long row = r0 + rsub; row < r1; row += 2) {
         const unsigned long long ix = (row * W + c0 + lc) * 3ull;
         const T x = pts[ix], y = pts[ix + 1], z = pts[ix + 2];
-        out[ix] = madd3(m[0], x, m[1], y, m[2], z, m[3]);
-        out[ix + 1] = madd3(m[4], x, m[5], y, m[6], z, m[7]);
-        out[ix + 2] = madd3(m[8], x, m[9], y, m[10], z, m[11]);
+        out[ix] = pose_row(m, x, y, z);
+        out[ix + 1] = pose_row(m + 4, x, y, z);
+        out[ix + 2] = pose_row(m + 8, x, y, z);
     }
 }
 

@@ -22,6 +22,7 @@
 #include <vector>
 
 #include "ob_api_common.h"
+#include "ob_project.cuh"
 
 namespace ob {
 namespace {
@@ -52,21 +53,6 @@ struct MaskParams {
     MaskEntry e[CAP];
     uint16_t shift[kMaxShiftRows];  // COLS: shift[r] mod w
 };
-
-// K1's projection (ob_cloud.cu): r == 0 gives 0, else r * d + o, each operation rounded on its own
-__device__ __forceinline__ float project(uint32_t r, float d, float o) {
-    return r == 0 ? 0.0f : __fadd_rn(__fmul_rn(static_cast<float>(r), d), o);
-}
-__device__ __forceinline__ double project(uint32_t r, double d, double o) {
-    return r == 0 ? 0.0 : __dadd_rn(__dmul_rn(static_cast<double>(r), d), o);
-}
-// ob_dewarp's row of R * p + t: (m0 x + (m1 y + m2 z)) + m3
-__device__ __forceinline__ float pose_row(const float* m, float x, float y, float z) {
-    return __fadd_rn(__fadd_rn(__fmul_rn(m[0], x), __fadd_rn(__fmul_rn(m[1], y), __fmul_rn(m[2], z))), m[3]);
-}
-__device__ __forceinline__ double pose_row(const double* m, double x, double y, double z) {
-    return __dadd_rn(__dadd_rn(__dmul_rn(m[0], x), __dadd_rn(__dmul_rn(m[1], y), __dmul_rn(m[2], z))), m[3]);
-}
 
 // axis coordinate of lut(range) at pixel i of frame f, posed by column c when poses are given; compared in T
 template <typename T, int CAP>

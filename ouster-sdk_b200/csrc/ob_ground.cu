@@ -5,11 +5,11 @@
 // Every step is double arithmetic with one rounding per operation (explicit __dmul_rn / __dadd_rn, no contraction),
 // and every statistic is a selection in the total order "<, then -0.0 before +0.0" (DESIGN §9), so each grid after
 // each pass is bit-identical to oracle/orc_ground.c given the same normals.  Selections sort the order-preserving
-// uint64 image of the double (ord()) as an unsigned key: CUB's floating-point radix digits fold -0.0 onto +0.0.
+// uint64 image of the double (okey()) as an unsigned key: CUB's floating-point radix digits fold -0.0 onto +0.0.
 //
 // Passes (launch family "ground"; CUB's own sort and scan kernels are not counted):
 //   span         first / last column with status bit 0, per frame
-//   points       dewarped model points (first two returns), extents (atomicMin/Max on ord()), z and footprint keys
+//   points       dewarped model points (first two returns), extents (atomicMin/Max on okey()), z and footprint keys
 //   [sort]       per frame: z and max(|x|, |y|) ascending
 //   header       footprint bound, fallback z (sequential ascending sum, one thread per frame), origin, shape
 //   -- the one host wait: grid shapes, then the grids are allocated --
@@ -22,6 +22,7 @@
 #include <vector>
 
 #include "ob_api_common.h"
+#include "ob_arith.cuh"
 #include "ob_cub.cuh"
 #include "ob_project.cuh"
 
@@ -52,30 +53,6 @@ constexpr int kThreads = 256;
 constexpr int kFillWarps = 8;
 constexpr unsigned long long kNoKey = ~0ull;
 
-__device__ __forceinline__ double mul(double a, double b) { return __dmul_rn(a, b); }
-__device__ __forceinline__ double add(double a, double b) { return __dadd_rn(a, b); }
-__device__ __forceinline__ double sub(double a, double b) { return __dsub_rn(a, b); }
-
-// order-preserving image of a double: unsigned order = "<, then -0.0 before +0.0" (NaN never enters)
-__host__ __device__ __forceinline__ unsigned long long ord(double d) {
-    unsigned long long b;
-    memcpy(&b, &d, 8);
-    return (b >> 63) ? ~b : (b | (1ull << 63));
-}
-__host__ __device__ __forceinline__ double unord(unsigned long long k) {
-    const unsigned long long b = (k >> 63) ? (k & ~(1ull << 63)) : ~k;
-    double d;
-    memcpy(&d, &b, 8);
-    return d;
-}
-
-__device__ __forceinline__ bool finite3(double x, double y, double z) {
-    return isfinite(x) && isfinite(y) && isfinite(z);
-}
-__device__ __forceinline__ double norm3(double x, double y, double z) {
-    return sqrt(add(add(mul(x, x), mul(y, y)), mul(z, z)));
-}
-
 // one frame of the call, device memory
 struct GFrame {
     const double* dir;    // h*w x 3, the item's f64 LUT
@@ -101,7 +78,7 @@ struct GFrame {
 // per-frame state written by the kernels; the host reads it once (the grid shapes)
 struct GState {
     int first, last;
-    unsigned long long min_x, min_y, max_x, max_y;  // ord() images
+    unsigned long long min_x, min_y, max_x, max_y;  // okey() images
     unsigned long long n_points;
     double origin_x, origin_y, fallback_z, footprint_bound, cell, inv;
     int rows, cols, valid, has_columns;
@@ -217,12 +194,12 @@ __global__ void points_kernel(const GFrame* frames, GState* gs, double* pts, uin
                 pts[slot * 3 + 0] = p[0];
                 pts[slot * 3 + 1] = p[1];
                 pts[slot * 3 + 2] = p[2];
-                zk = ord(p[2]);
-                fk = ord(fmax(fabs(p[0]), fabs(p[1])));
-                atomicMin(&s.min_x, ord(p[0]));
-                atomicMin(&s.min_y, ord(p[1]));
-                atomicMax(&s.max_x, ord(p[0]));
-                atomicMax(&s.max_y, ord(p[1]));
+                zk = okey(p[2]);
+                fk = okey(fmax(fabs(p[0]), fabs(p[1])));
+                atomicMin(&s.min_x, okey(p[0]));
+                atomicMin(&s.min_y, okey(p[1]));
+                atomicMax(&s.max_x, okey(p[0]));
+                atomicMax(&s.max_y, okey(p[1]));
                 atomicAdd(&s.n_points, 1ull);
                 double x, y, z;
                 if (normal_at(f, static_cast<int>(ret), px, x, y, z)) {
@@ -253,21 +230,21 @@ __global__ void header_kernel(const GFrame* frames, GState* gs, const unsigned l
     const unsigned long long* fp = sorted + P + f.pt_off;
     unsigned long long k = static_cast<unsigned long long>(floor(kXyBoundsPct * static_cast<double>(n - 1)));
     if (k > n - 1) k = n - 1;
-    s.footprint_bound = unord(fp[k]);
+    s.footprint_bound = okey_value(fp[k]);
     unsigned long long lo = static_cast<unsigned long long>(floor(kTailLow * static_cast<double>(n - 1)));
     unsigned long long hi = static_cast<unsigned long long>(ceil(kTailHigh * static_cast<double>(n - 1)));
     if (lo > n - 1) lo = n - 1;
     if (hi > n - 1) hi = n - 1;
     if (hi < lo) hi = lo;
     double sum = 0.0;
-    for (unsigned long long i = lo; i <= hi; ++i) sum = add(sum, unord(zs[i]));  // ascending, as pinned in §9
+    for (unsigned long long i = lo; i <= hi; ++i) sum = add(sum, okey_value(zs[i]));  // ascending, as pinned in §9
     s.fallback_z = sum / static_cast<double>(hi - lo + 1);
     s.cell = grid_size;
     s.inv = 1.0 / grid_size;
-    s.origin_x = mul(floor(mul(unord(s.min_x), s.inv)), s.cell);
-    s.origin_y = mul(floor(mul(unord(s.min_y), s.inv)), s.cell);
-    const double cols = ceil(sub(unord(s.max_x), s.origin_x) / s.cell) + 1.0;
-    const double rows = ceil(sub(unord(s.max_y), s.origin_y) / s.cell) + 1.0;
+    s.origin_x = mul(floor(mul(okey_value(s.min_x), s.inv)), s.cell);
+    s.origin_y = mul(floor(mul(okey_value(s.min_y), s.inv)), s.cell);
+    const double cols = ceil(sub(okey_value(s.max_x), s.origin_x) / s.cell) + 1.0;
+    const double rows = ceil(sub(okey_value(s.max_y), s.origin_y) / s.cell) + 1.0;
     // the oracle's (int) conversion; a shape beyond int range is refused on the host
     s.cols = cols > 1.0 ? (cols < 2147483647.0 ? static_cast<int>(cols) : 0x7fffffff) : 1;
     s.rows = rows > 1.0 ? (rows < 2147483647.0 ? static_cast<int>(rows) : 0x7fffffff) : 1;
@@ -321,7 +298,7 @@ __global__ void cell_segments_kernel(const uint32_t* skeys, const uint32_t* sslo
             if (i == 0 || skeys[i - 1] != key) cbeg[key] = static_cast<uint32_t>(i);
             if (i + 1 == P || skeys[i + 1] != key) cend[key] = static_cast<uint32_t>(i + 1);
             const uint32_t slot = sslots[i];
-            zs[i] = unord(zkeys[slot]);
+            zs[i] = okey_value(zkeys[slot]);
             fl = nflag[slot];
         }
         flags[i] = fl;
@@ -434,10 +411,10 @@ __global__ void cells_kernel(const GFrame* frames, GState* gs, const uint32_t* c
 // k-th smallest (total order) of v[0, n) in shared memory, by rank counting across the warp
 __device__ double warp_kth(const double* v, unsigned n, unsigned kk, double* slot, unsigned lane) {
     for (unsigned i = lane; i < n; i += 32) {
-        const unsigned long long ki = ord(v[i]);
+        const unsigned long long ki = okey(v[i]);
         unsigned less = 0, eq = 0;
         for (unsigned j = 0; j < n; ++j) {
-            const unsigned long long kj = ord(v[j]);
+            const unsigned long long kj = okey(v[j]);
             less += kj < ki;
             eq += kj == ki;
         }
@@ -517,9 +494,9 @@ __global__ void __launch_bounds__(kFillWarps * 32) fill_kernel(const GFrame* fra
 __device__ __forceinline__ double small_median(double* v, unsigned n) {  // insertion sort in the total order
     for (unsigned i = 1; i < n; ++i) {
         const double x = v[i];
-        const unsigned long long kx = ord(x);
+        const unsigned long long kx = okey(x);
         unsigned j = i;
-        while (j > 0 && ord(v[j - 1]) > kx) {
+        while (j > 0 && okey(v[j - 1]) > kx) {
             v[j] = v[j - 1];
             --j;
         }
@@ -705,7 +682,7 @@ __global__ void comp_roots_kernel(const GFrame* frames, const GState* gs, Grid g
             const uint32_t root = find_root(parent, static_cast<uint32_t>(ci));
             parent[ci] = root;
             atomicAdd(&csize[root], 1u);
-            hk = ord(g.height[ci]);
+            hk = okey(g.height[ci]);
         }
         hkeys[ci] = hk;
         cells[ci] = static_cast<uint32_t>(ci);

@@ -10,6 +10,7 @@
 #include <cstring>
 
 #include "ob_api_common.h"
+#include "ob_arith.cuh"
 
 namespace ob {
 namespace {
@@ -41,26 +42,10 @@ struct HostParams {
     int32_t update_every, color_correct;
 };
 
-// ---- rounded arithmetic in T ----
-__device__ __forceinline__ float radd(float a, float b) { return __fadd_rn(a, b); }
-__device__ __forceinline__ double radd(double a, double b) { return __dadd_rn(a, b); }
-__device__ __forceinline__ float rsub(float a, float b) { return __fsub_rn(a, b); }
-__device__ __forceinline__ double rsub(double a, double b) { return __dsub_rn(a, b); }
-__device__ __forceinline__ float rmul(float a, float b) { return __fmul_rn(a, b); }
-__device__ __forceinline__ double rmul(double a, double b) { return __dmul_rn(a, b); }
-__device__ __forceinline__ float rdiv(float a, float b) { return __fdiv_rn(a, b); }
-__device__ __forceinline__ double rdiv(double a, double b) { return __ddiv_rn(a, b); }
-
-// std::max(a, b) / std::min(a, b): (a < b) ? b : a and (b < a) ? b : a
-template <typename T>
-__device__ __forceinline__ T smax(T a, T b) { return (a < b) ? b : a; }
-template <typename T>
-__device__ __forceinline__ T smin(T a, T b) { return (b < a) ? b : a; }
-
 // (r * R + g * G) + b * B in T, each constant rounded to T once
 template <typename T>
 __device__ __forceinline__ T lum3(T r, T g, T b) {
-    return radd(radd(rmul(r, T(kRLum)), rmul(g, T(kGLum))), rmul(b, T(kBLum)));
+    return add(add(mul(r, T(kRLum)), mul(g, T(kGLum))), mul(b, T(kBLum)));
 }
 
 // f16_bits_to_f32_bits_fast_nan_zero (image_processing.cpp:59-65): a bias shift, not an IEEE conversion
@@ -74,28 +59,6 @@ __device__ __forceinline__ float fast_log10(float x) {
     const int32_t bits = __float_as_int(x);
     return __fmul_rn(__fmul_rn(__int2float_rn(bits - 0x3F800000), 1.1920929e-7f), 0.30103f);
 }
-
-// ---- order-preserving keys ----
-template <typename T>
-struct Key;
-template <>
-struct Key<float> {
-    using K = uint32_t;
-    __device__ static K of(float x) {
-        const uint32_t u = __float_as_uint(x);
-        return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-    }
-    __device__ static float val(K k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k); }
-};
-template <>
-struct Key<double> {
-    using K = unsigned long long;
-    __device__ static K of(double x) {
-        const K u = (K)__double_as_longlong(x);
-        return (u >> 63) ? ~u : (u | (1ull << 63));
-    }
-    __device__ static double val(K k) { return __longlong_as_double((long long)((k >> 63) ? (k & ~(1ull << 63)) : ~k)); }
-};
 
 // Number of items for which get(i, k) holds; every thread of the block gets the count.
 template <class Get, typename K>
@@ -172,8 +135,7 @@ __device__ __forceinline__ T load(const void* p, size_t i) {
 template <typename T, int L>
 __global__ void __launch_bounds__(kSelectThreads) ae_select_kernel(const void* img, uint32_t npx, DevState* st,
                                                                     HostParams p, int update_state, int ltm) {
-    using KT = Key<T>;
-    using K = typename KT::K;
+    using K = decltype(okey(T()));
     __shared__ uint32_t hist[2 * 256];
     __shared__ int select;
     // one read of the counter, shared before anyone branches on it: thread 0 writes it back further down
@@ -187,7 +149,7 @@ __global__ void __launch_bounds__(kSelectThreads) ae_select_kernel(const void* i
             if constexpr (L == 0) v = load<T, L>(img, px);
             else v = lum3<T>(load<T, L>(img, 3 * px), load<T, L>(img, 3 * px + 1), load<T, L>(img, 3 * px + 2));
             if (!(v > T(0))) return false;
-            k = KT::of(v);
+            k = okey(v);
             return true;
         };
         const uint32_t n = block_count<decltype(get), K>(get, n_items);
@@ -201,8 +163,8 @@ __global__ void __launch_bounds__(kSelectThreads) ae_select_kernel(const void* i
         __shared__ K res[2];
         block_select<K, 2>(get, n_items, ranks, res, hist);
         if (threadIdx.x == 0) {
-            st->lo = double(KT::val(res[0]));
-            st->hi = double(KT::val(res[1]));
+            st->lo = double(okey_value(res[0]));
+            st->hi = double(okey_value(res[1]));
             if (!st->initialized) {
                 st->initialized = 1;
                 st->lo_state = st->lo;
@@ -243,8 +205,8 @@ __global__ void __launch_bounds__(kSelectThreads) ae_select_kernel(const void* i
 
 template <typename T>
 __device__ __forceinline__ T affine(T v, const DevState& s) {
-    if (s.branch == 1) return radd(rmul(rsub(v, T(s.sub)), T(s.mul)), T(s.add));
-    return rmul(v, T(s.mul));
+    if (s.branch == 1) return add(mul(sub(v, T(s.sub)), T(s.mul)), T(s.add));
+    return mul(v, T(s.mul));
 }
 
 // AutoExposure: the affine map and the clamp to [0, 1]; the float16 layout always writes the converted input
@@ -277,17 +239,17 @@ __global__ void ltm_pixel_kernel(const void* in, T* out, T* lum_ae, uint32_t npx
                 const T lum = lum3(c[0], c[1], c[2]);
                 if (lum > thresh) {
                     // lum - thresh + 1.0 is a double expression, narrowed to float for fast_log10
-                    const float arg = __double2float_rn(__dadd_rn(double(rsub(lum, thresh)), 1.0));
-                    const T new_lum = radd(thresh, T(fast_log10(arg)));
-                    const T scale = rdiv(new_lum, lum);
+                    const float arg = __double2float_rn(__dadd_rn(double(sub(lum, thresh)), 1.0));
+                    const T new_lum = add(thresh, T(fast_log10(arg)));
+                    const T scale = div(new_lum, lum);
 #pragma unroll
-                    for (int k = 0; k < 3; ++k) c[k] = rmul(c[k], scale);
+                    for (int k = 0; k < 3; ++k) c[k] = mul(c[k], scale);
                 }
             }
 #pragma unroll
             for (int k = 0; k < 3; ++k) {
                 const T x = smax(c[k], T(0));
-                c[k] = rdiv(x, radd(T(1), x));
+                c[k] = div(x, add(T(1), x));
             }
             lum_ae[px] = lum3(c[0], c[1], c[2]);
         }
@@ -354,7 +316,7 @@ __global__ void ltm_apply_kernel(T* img, const T* lum_ae, int h, int w, const fl
     const DevState s = *st;
     if (!s.apply) return;
     T cf = T(0.75);
-    if (s.hi_state < 1.0) cf = rmul(cf, smax(T(0), T(__ddiv_rn(__dsub_rn(s.hi_state, 0.5), 0.5))));
+    if (s.hi_state < 1.0) cf = mul(cf, smax(T(0), T(__ddiv_rn(__dsub_rn(s.hi_state, 0.5), 0.5))));
     const bool plain = !color_correct || cf == T(0);
     const uint32_t npx = uint32_t(h) * uint32_t(w);
     for (uint32_t px = blockIdx.x * blockDim.x + threadIdx.x; px < npx; px += gridDim.x * blockDim.x) {
@@ -371,15 +333,15 @@ __global__ void ltm_apply_kernel(T* img, const T* lum_ae, int h, int w, const fl
         const float a = __fadd_rn(__fmul_rn(gx, l0[tx0 * kBins + bin]), __fmul_rn(fx, l0[tx1 * kBins + bin]));
         const float b = __fadd_rn(__fmul_rn(gx, l1[tx0 * kBins + bin]), __fmul_rn(fx, l1[tx1 * kBins + bin]));
         const T lum_new = T(__fadd_rn(__fmul_rn(__fsub_rn(1.0f, fy), a), __fmul_rn(fy, b)));
-        const T scale = (lum_old > T(1e-6)) ? rdiv(lum_new, lum_old) : T(1);
+        const T scale = (lum_old > T(1e-6)) ? div(lum_new, lum_old) : T(1);
         T* c = img + 3 * size_t(px);
 #pragma unroll
         for (int k = 0; k < 3; ++k) {
-            const T v = rmul(c[k], scale);
+            const T v = mul(c[k], scale);
             if (plain) {
                 c[k] = smin(v, T(1));
             } else {
-                const T u = radd(rmul(-lum_new, cf), rmul(v, radd(T(1), cf)));
+                const T u = add(mul(-lum_new, cf), mul(v, add(T(1), cf)));
                 c[k] = smax(T(0), smin(u, T(1)));
             }
         }
@@ -408,8 +370,7 @@ template <typename T>
 __global__ void __launch_bounds__(kMedianThreads) buc_median_kernel(const T* img, uint32_t rows, uint32_t cols,
                                                                      const uint8_t* mask, T* med, const DevState* st,
                                                                      int update_state) {
-    using KT = Key<T>;
-    using K = typename KT::K;
+    using K = decltype(okey(T()));
     if (!buc_recompute(st, rows, update_state)) return;
     __shared__ uint32_t hist[256];
     __shared__ K res;
@@ -418,14 +379,14 @@ __global__ void __launch_bounds__(kMedianThreads) buc_median_kernel(const T* img
     const T* b = a - cols;
     auto get = [&](uint32_t c, K& k) -> bool {
         if (!mask[c]) return false;
-        k = KT::of(rsub(a[c], b[c]));
+        k = okey(sub(a[c], b[c]));
         return true;
     };
     const uint32_t n = block_count<decltype(get), K>(get, cols);
     if (n == 0) return;
     const uint32_t rank = n / 2;
     block_select<K, 1>(get, cols, &rank, &res, hist);
-    if (threadIdx.x == 0) med[i] = KT::val(res);
+    if (threadIdx.x == 0) med[i] = okey_value(res);
 }
 
 // compute_dark_count after the medians: the cumulative sum, the FullPivLU "fit" (restated below), the minimum, then
@@ -442,7 +403,7 @@ __global__ void buc_tail_kernel(uint32_t rows, uint32_t cols, const uint8_t* mas
             for (int i = 0; i < h; ++i) dc[i] = T(0);
         } else {
             dc[0] = T(0);
-            for (int i = 1; i < h; ++i) dc[i] = radd(dc[i - 1], dc[i]);  // dc[i] held the median of pair i
+            for (int i = 1; i < h; ++i) dc[i] = add(dc[i - 1], dc[i]);  // dc[i] held the median of pair i
             // image_array.fullPivLu().solve(dc) for image_array = [1, i] (h x 2), lu column-major
             T* c0 = lu;
             T* c1 = lu + h;
@@ -486,12 +447,12 @@ __global__ void buc_tail_kernel(uint32_t rows, uint32_t cols, const uint8_t* mas
                     col[k] = col[bc];
                     col[bc] = t;
                 }
-                for (int r = k + 1; r < h; ++r) col[k][r] = rdiv(col[k][r], col[k][k]);
+                for (int r = k + 1; r < h; ++r) col[k][r] = div(col[k][r], col[k][k]);
                 if (k < size - 1)
                     for (int j = k + 1; j < 2; ++j)
-                        for (int r = k + 1; r < h; ++r) col[j][r] = rsub(col[j][r], rmul(col[k][r], col[j][k]));
+                        for (int r = k + 1; r < h; ++r) col[j][r] = sub(col[j][r], mul(col[k][r], col[j][k]));
             }
-            const T thr = rmul(maxpivot, rmul(T(sizeof(T) == 4 ? 1.1920928955078125e-07 : 2.220446049250313e-16),
+            const T thr = mul(maxpivot, mul(T(sizeof(T) == 4 ? 1.1920928955078125e-07 : 2.220446049250313e-16),
                                               T(size)));
             int rank = 0;
             for (int q = 0; q < nonzero; ++q) rank += fabs(col[q][q]) > thr;
@@ -505,13 +466,13 @@ __global__ void buc_tail_kernel(uint32_t rows, uint32_t cols, const uint8_t* mas
                     cv[rowt[k]] = t;
                 }
                 T c[2] = {cv[0], size > 1 ? cv[1] : T(0)};
-                if (size > 1) c[1] = rsub(c[1], rmul(c[0], col[0][1]));  // unit lower
+                if (size > 1) c[1] = sub(c[1], mul(c[0], col[0][1]));  // unit lower
                 // upper, rank x rank, back substitution
                 if (rank > 1) {
-                    c[1] = rdiv(c[1], col[1][1]);
-                    c[0] = rsub(c[0], rmul(c[1], col[1][0]));
+                    c[1] = div(c[1], col[1][1]);
+                    c[0] = sub(c[0], mul(c[1], col[1][0]));
                 }
-                c[0] = rdiv(c[0], col[0][0]);
+                c[0] = div(c[0], col[0][0]);
                 int q[2] = {0, 1};
                 for (int k = 0; k < size; ++k) {
                     const int t = colt[k], s = q[k];
@@ -522,10 +483,10 @@ __global__ void buc_tail_kernel(uint32_t rows, uint32_t cols, const uint8_t* mas
             }
             T m = T(0);
             for (int i = 0; i < h; ++i) {
-                dc[i] = rsub(dc[i], radd(rmul(T(1), x[0]), rmul(T(i), x[1])));
+                dc[i] = sub(dc[i], add(mul(T(1), x[0]), mul(T(i), x[1])));
                 m = (i == 0) ? dc[i] : smin(m, dc[i]);
             }
-            for (int i = 0; i < h; ++i) dc[i] = rsub(dc[i], m);
+            for (int i = 0; i < h; ++i) dc[i] = sub(dc[i], m);
         }
         for (int i = 0; i < h; ++i)
             dark[i] = reset ? double(dc[i])
@@ -539,7 +500,7 @@ __global__ void buc_tail_kernel(uint32_t rows, uint32_t cols, const uint8_t* mas
 template <typename T>
 __global__ void buc_apply_kernel(T* img, uint32_t cols, size_t n, const double* dark) {
     for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += size_t(gridDim.x) * blockDim.x)
-        img[i] = smax(rsub(img[i], T(dark[i / cols])), T(0));
+        img[i] = smax(sub(img[i], T(dark[i / cols])), T(0));
 }
 
 unsigned ew_blocks(size_t n) { return unsigned(std::max<size_t>(1, std::min<size_t>((n + kEwThreads - 1) / kEwThreads, 4096))); }

@@ -3,7 +3,7 @@
 #pragma once
 #include <cfloat>
 
-#include "ob_voxel_common.cuh"
+#include "ob_arith.cuh"
 
 namespace ob {
 namespace {

@@ -4,6 +4,8 @@
 #pragma once
 #include <cstdint>
 
+#include "ob_arith.cuh"
+
 namespace ob {
 
 __device__ __forceinline__ uint32_t ld_acquire_u32(const uint32_t* p) {
@@ -13,11 +15,6 @@ __device__ __forceinline__ uint32_t ld_acquire_u32(const uint32_t* p) {
 }
 __device__ __forceinline__ void st_release_u32(uint32_t* p, uint32_t v) {
     asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ unsigned long long warp_sum_u64(unsigned long long v) {
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
-    return v;
 }
 
 // Per logical CTA a state word (0 = nothing yet, 1 = aggregate published, 2 = inclusive prefix published) and the

@@ -22,6 +22,7 @@
 #include <cmath>
 
 #include "ob_api_common.h"
+#include "ob_arith.cuh"
 
 namespace ob {
 
@@ -41,13 +42,6 @@ struct NormalsParams {
     double desired_sq, tan_safe, h_subtent, subtent_override;
     int dual;
 };
-
-__device__ __forceinline__ double mul(double a, double b) { return __dmul_rn(a, b); }
-__device__ __forceinline__ double add(double a, double b) { return __dadd_rn(a, b); }
-__device__ __forceinline__ double sub(double a, double b) { return __dsub_rn(a, b); }
-__device__ __forceinline__ double dot3(const double (&a)[3], const double (&b)[3]) {
-    return add(add(mul(a[0], b[0]), mul(a[1], b[1])), mul(a[2], b[2]));
-}
 
 template <typename T>
 __device__ __forceinline__ void load3(const T* base, size_t idx, double (&v)[3]) {

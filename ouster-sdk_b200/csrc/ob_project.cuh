@@ -1,5 +1,6 @@
-// ob_project.cuh -- the per-pixel arithmetic of range -> XYZ and of the per-column pose, shared by K1 (ob_cloud.cu),
-// K3 (ob_dewarp_frame.cu) and the map-row ingest (ob_map_rows.cu), so that every path rounds exactly alike.
+// ob_project.cuh -- the per-pixel arithmetic of range -> XYZ and of the per-column pose, shared by K1 and the
+// stand-alone dewarp (ob_cloud.cu), K3 (ob_dewarp_frame.cu), the map-row ingest (ob_map_rows.cu), the frame
+// operations (ob_frame_ops.cu) and ground segmentation (ob_ground.cu), so that every path rounds exactly alike.
 #pragma once
 #include <cstdint>
 

@@ -1,7 +1,11 @@
 // ob_rows.cuh -- point rows of the C ABI (ob_point_rows) as the device sees them, shared by the voxel map / ICP
 // (ob_voxel_map.cu) and cloud-to-cloud ICP (ob_align.cu): a host row count or a device word clamped to the
-// capacity, float32 or float64 rows widened to double on load, and the host-side check and staging.
+// capacity, float32 or float64 rows widened to double on load, the order-preserving compaction of the rows an
+// association kept, and the host-side check and staging.
 #pragma once
+#include <cub/block/block_reduce.cuh>
+#include <cub/block/block_scan.cuh>
+
 #include <cstdint>
 
 #include "ob_api_common.h"
@@ -27,6 +31,32 @@ __device__ __forceinline__ void load3(const void* base, size_t row, double* v) {
     v[0] = static_cast<double>(p[0]);
     v[1] = static_cast<double>(p[1]);
     v[2] = static_cast<double>(p[2]);
+}
+
+// Order-preserving compaction of the rows i < cap with valid[i] set, one thread per row in blocks of kThreads whose
+// flags sum to block_count[b]: keep(i, o) for each such row, o its position among them; the last block writes their
+// number to *n.
+template <int kThreads, class Keep>
+__device__ __forceinline__ void compact_rows(unsigned cap, const uint32_t* valid, const uint32_t* block_count,
+                                             unsigned long long* n, Keep keep) {
+    using BR = cub::BlockReduce<unsigned, kThreads>;
+    using BS = cub::BlockScan<unsigned, kThreads>;
+    __shared__ union {
+        typename BR::TempStorage r;
+        typename BS::TempStorage s;
+    } tmp;
+    __shared__ unsigned base;
+    unsigned part = 0;
+    for (unsigned b = threadIdx.x; b < blockIdx.x; b += blockDim.x) part += block_count[b];
+    const unsigned before = BR(tmp.r).Sum(part);
+    if (threadIdx.x == 0) base = before;
+    __syncthreads();
+    const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+    const unsigned f = i < cap ? valid[i] : 0u;
+    unsigned pos, total;
+    BS(tmp.s).ExclusiveSum(f, pos, total);
+    if (f) keep(i, static_cast<size_t>(base) + pos);
+    if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) *n = base + total;
 }
 
 // ---- host side ----

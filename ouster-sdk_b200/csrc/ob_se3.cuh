@@ -1,5 +1,6 @@
-// ob_se3.cuh -- SE(3) pieces in pinned double arithmetic, shared by cloud-to-cloud ICP (ob_align.cu) and pose
-// interpolation (ob_pose_interp.cu): PoseV::exp, PoseH::log, the 3 x 3 and 4 x 4 inverses and the 4 x 4 product.
+// ob_se3.cuh -- SE(3) pieces in pinned double arithmetic, shared by cloud-to-cloud ICP (ob_align.cu), global cloud
+// alignment (ob_align_clouds.cu) and pose interpolation (ob_pose_interp.cu): PoseV::exp, PoseH::log, the 3 x 3 and
+// 4 x 4 inverses, the 4 x 4 product and a 4 x 4 pose applied to a point or a direction.
 //
 // What it restates (reference paths relative to the reference tree):
 //   PoseV::exp, RotV::exp, RotV::vee          ouster_core/src/transform_vector.cpp:40-60, 96-104
@@ -11,15 +12,10 @@
 #pragma once
 #include <cfloat>
 
+#include "ob_arith.cuh"
+
 namespace ob {
 namespace {
-
-__device__ __forceinline__ double mul(double a, double b) { return __dmul_rn(a, b); }
-__device__ __forceinline__ double add(double a, double b) { return __dadd_rn(a, b); }
-__device__ __forceinline__ double sub(double a, double b) { return __dsub_rn(a, b); }
-// squaredNorm of a 3-vector, (x0*x0 + x1*x1) + x2*x2 as in ob_normals.cu (DESIGN 2)
-__device__ __forceinline__ double sqn3(double a, double b, double c) { return add(add(mul(a, a), mul(b, b)), mul(c, c)); }
-__device__ __forceinline__ double norm3(const double* a) { return sqrt(sqn3(a[0], a[1], a[2])); }
 
 __device__ void mat3_mul(const double a[3][3], const double b[3][3], double c[3][3]) {
     for (int i = 0; i < 3; ++i)
@@ -113,6 +109,16 @@ __device__ __forceinline__ void mat4_mul(const double* a, const double* b, doubl
         for (int j = 0; j < 4; ++j)
             c[4 * i + j] = add(add(add(mul(a[4 * i], b[j]), mul(a[4 * i + 1], b[4 + j])), mul(a[4 * i + 2], b[8 + j])),
                                mul(a[4 * i + 3], b[12 + j]));
+}
+
+// x = R p + t and x = R p for the top 3 x 4 of a row-major pose, summed left to right: ((r0 p0 + r1 p1) + r2 p2) + t.
+// ob_project.cuh's pose_row sums the dewarp's order, r0 p0 + (r1 p1 + r2 p2), instead.
+__device__ __forceinline__ void mat4_transform(const double* P, const double* p, double* x) {
+    for (int d = 0; d < 3; ++d)
+        x[d] = add(add(add(mul(P[4 * d], p[0]), mul(P[4 * d + 1], p[1])), mul(P[4 * d + 2], p[2])), P[4 * d + 3]);
+}
+__device__ __forceinline__ void mat4_rotate(const double* P, const double* p, double* x) {
+    for (int d = 0; d < 3; ++d) x[d] = add(add(mul(P[4 * d], p[0]), mul(P[4 * d + 1], p[1])), mul(P[4 * d + 2], p[2]));
 }
 
 // ---- PoseH::log (transform_homogeneous.cpp:31-62): row-major 4 x 4 -> v = (rotation vector, translation) ----

@@ -102,8 +102,6 @@ __device__ __forceinline__ double ld(const void* base, size_t i) {
     return static_cast<double>(static_cast<const T*>(base)[i]);
 }
 
-__device__ __forceinline__ bool finite3(double a, double b, double c) { return isfinite(a) && isfinite(b) && isfinite(c); }
-
 // ---- Fisher-Yates without the serial loop (SHUFFLE_FIRST) ----
 // step s < n-1 swaps positions s and j_s = s + ((u64)rand_s * (n - s)) >> 32, rand_s the (s+1)-th draw;
 // step n-1 is treated as j = n-1.  Padding steps get the key `cap` (sorts last).
@@ -178,7 +176,9 @@ __global__ void vx_key_kernel(VoxelParams p, VKey* keys, uint32_t* seq) {
             const double a = ld<T>(p.normals, row * 3), b = ld<T>(p.normals, row * 3 + 1), c = ld<T>(p.normals, row * 3 + 2);
             ok = finite3(x, y, z) && finite3(a, b, c) && sqrt(sqn3(a, b, c)) > 1e-12;
         }
-        if (ok) k = VKey{0u, voxel_coord(mul(x, p.inv)), voxel_coord(mul(y, p.inv)), voxel_coord(mul(z, p.inv))};
+        if (ok)
+            k = VKey{0u, floor_cast<int32_t>(mul(x, p.inv)), floor_cast<int32_t>(mul(y, p.inv)),
+                     floor_cast<int32_t>(mul(z, p.inv))};
     }
     keys[t] = k;
     seq[t] = t;

@@ -5,10 +5,9 @@
 #pragma once
 #include <cuda/std/tuple>
 
-#include <climits>
 #include <cstdint>
 
-#include "ob_se3.cuh"  // mul / add / sub / sqn3
+#include "ob_arith.cuh"
 
 namespace ob {
 namespace {
@@ -30,14 +29,6 @@ constexpr int kKeyBits = 97;  // x, y, z and the low bit of pad
 
 __device__ __forceinline__ bool same_key(const VKey& a, const VKey& b) {
     return a.pad == b.pad && a.x == b.x && a.y == b.y && a.z == b.z;
-}
-
-// static_cast<int>(std::floor(v)) as x86 cvttsd2si evaluates it: NaN and out-of-range give INT_MIN
-// (the device conversion would saturate instead)
-__device__ __forceinline__ int32_t voxel_coord(double v) {
-    const double f = floor(v);
-    if (!(f >= -2147483648.0 && f < 2147483648.0)) return INT_MIN;
-    return static_cast<int32_t>(f);
 }
 
 // first_n_point's rejection test (voxel_hash_map.h:293-296): a kept point q is within the map resolution of p

@@ -156,7 +156,8 @@ __global__ void vm_key_kernel(Rows r, unsigned cols, double inv, VKey* keys, uin
     if (t < rows_n(r)) {
         double v[3];
         load_xyz<T>(r.p, t, cols, v);
-        k = VKey{0u, voxel_coord(mul(v[0], inv)), voxel_coord(mul(v[1], inv)), voxel_coord(mul(v[2], inv))};
+        k = VKey{0u, floor_cast<int32_t>(mul(v[0], inv)), floor_cast<int32_t>(mul(v[1], inv)),
+                 floor_cast<int32_t>(mul(v[2], inv))};
     }
     keys[t] = k;
     seq[t] = t;
@@ -243,9 +244,9 @@ __global__ void vm_cull_kernel(Table t, unsigned long long* ctr, const double* o
     if (i >= t.cap) return;
     uint32_t out = 0;
     if (t.state[i] == kLive) {
-        const uint32_t ox = static_cast<uint32_t>(voxel_coord(mul(origin[0], inv)));
-        const uint32_t oy = static_cast<uint32_t>(voxel_coord(mul(origin[1], inv)));
-        const uint32_t oz = static_cast<uint32_t>(voxel_coord(mul(origin[2], inv)));
+        const uint32_t ox = static_cast<uint32_t>(floor_cast<int32_t>(mul(origin[0], inv)));
+        const uint32_t oy = static_cast<uint32_t>(floor_cast<int32_t>(mul(origin[1], inv)));
+        const uint32_t oz = static_cast<uint32_t>(floor_cast<int32_t>(mul(origin[2], inv)));
         const uint32_t dx = static_cast<uint32_t>(t.key[3 * i]) - ox, dy = static_cast<uint32_t>(t.key[3 * i + 1]) - oy,
                        dz = static_cast<uint32_t>(t.key[3 * i + 2]) - oz;
         const int32_t d2 = static_cast<int32_t>((dx * dx + dy * dy) + dz * dz);
@@ -303,7 +304,8 @@ __constant__ int8_t kShift[27][3] = {
 template <bool kAt = false>
 __device__ double closest(const Table& t, double inv, double vs, const double* q, double max_d2, double* nb,
                           long long* at = nullptr) {
-    const int32_t v[3] = {voxel_coord(mul(q[0], inv)), voxel_coord(mul(q[1], inv)), voxel_coord(mul(q[2], inv))};
+    const int32_t v[3] = {floor_cast<int32_t>(mul(q[0], inv)), floor_cast<int32_t>(mul(q[1], inv)),
+                          floor_cast<int32_t>(mul(q[2], inv))};
     double best = max_d2;
     nb[0] = nb[1] = nb[2] = 0.0;
     if (kAt) *at = -1;
@@ -629,30 +631,12 @@ __global__ void icp_assoc_kernel(Rows r, Table t, double inv, double vs, double 
 __global__ void icp_compact_kernel(unsigned cap, const double* src, const double* tgt, const uint32_t* valid,
                                    const uint32_t* block_count, double* ps, double* pt, IcpState* s) {
     if (s->done) return;
-    using BR = cub::BlockReduce<unsigned, kAssocThreads>;
-    using BS = cub::BlockScan<unsigned, kAssocThreads>;
-    __shared__ union {
-        typename BR::TempStorage r;
-        typename BS::TempStorage s;
-    } tmp;
-    __shared__ unsigned base;
-    unsigned part = 0;
-    for (unsigned b = threadIdx.x; b < blockIdx.x; b += blockDim.x) part += block_count[b];
-    const unsigned before = BR(tmp.r).Sum(part);
-    if (threadIdx.x == 0) base = before;
-    __syncthreads();
-    const unsigned i = tid_global();
-    const unsigned f = i < cap ? valid[i] : 0u;
-    unsigned pos, total;
-    BS(tmp.s).ExclusiveSum(f, pos, total);
-    if (f) {
-        const size_t o = static_cast<size_t>(base) + pos;
+    compact_rows<kAssocThreads>(cap, valid, block_count, &s->n_pairs, [&](unsigned i, size_t o) {
         for (int d = 0; d < 3; ++d) {
             ps[3 * o + d] = src[3 * static_cast<size_t>(i) + d];
             pt[3 * o + d] = tgt[3 * static_cast<size_t>(i) + d];
         }
-    }
-    if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) s->n_pairs = base + total;
+    });
 }
 
 // the tree's parents, then (thread 0) the LDLT solve, SE3::exp, t_icp = estimation * t_icp and the stop test

@@ -14,6 +14,7 @@
 #include <vector>
 
 #include "ob_api_common.h"
+#include "ob_arith.cuh"
 
 struct ob_zone_monitor {
     int device;
@@ -184,12 +185,6 @@ __global__ void zone_max_count_kernel(const uint32_t* __restrict__ near_mm, cons
     if ((threadIdx.x & 31) == 0 && c) atomicAdd(&ctl[z].max_count, c);
 }
 
-__device__ __forceinline__ unsigned long long warp_sum64(unsigned long long v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
 // _calc_counts (zone_common.py:47-78): integer counts and atomics, so the result does not depend on scheduling
 __global__ void __launch_bounds__(kOccThreads) zone_occupancy_kernel(
     const uint32_t* __restrict__ range, const uint32_t* __restrict__ near_mm, const uint32_t* __restrict__ far_mm,
@@ -228,7 +223,7 @@ __global__ void __launch_bounds__(kOccThreads) zone_occupancy_kernel(
         inv = __reduce_add_sync(0xffffffffu, inv);
         mn = __reduce_min_sync(0xffffffffu, mn);
         mx = __reduce_max_sync(0xffffffffu, mx);
-        sum = warp_sum64(sum);
+        sum = warp_sum_u64(sum);
         if ((threadIdx.x & 31) == 0) {
             if (cnt) {
                 atomicAdd(&s_acc[z].count, cnt);
