@@ -43,6 +43,10 @@ typedef enum ob_status {
 
 typedef enum ob_dtype { OB_F32 = 0, OB_F64 = 1 } ob_dtype;
 
+/* Handles (ob_stream, ob_lut, ob_decoder, ob_decode_job, ob_voxel_map, ob_zone_monitor, ob_image_proc) live on the
+ * device they were created for.  Every *_destroy frees the handle's memory on that device and leaves the caller's
+ * current device as it was, so a handle may be destroyed from anywhere (a garbage collector, another device's code).
+ * Passing NULL to a *_destroy is OB_OK. */
 typedef struct ob_stream ob_stream;   /* CUDA stream + device arena + pinned staging */
 typedef struct ob_lut ob_lut;         /* device-resident XYZLutT<T> (direction/offset tables) */
 typedef struct ob_decoder ob_decoder; /* device-resident PacketFormat decode table */

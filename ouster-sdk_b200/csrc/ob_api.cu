@@ -288,8 +288,7 @@ struct ob_stream {
     // a steady-state caller passes the same pointers again and again, and re-uploading an identical
     // table costs a host-staged H2D copy per launch during which the GPU idles
     struct Table {
-        void* dev{nullptr};
-        size_t cap{0};
+        DeviceBlock dev;
         std::vector<uint8_t> host;
     } tables[3];
 };
@@ -298,48 +297,41 @@ struct ob_lut {
     int device;
     int dtype;
     size_t h, w;
-    void* dir;
-    void* off;
+    DeviceBlock dir, off;
     // LUT-free mode (LUTs built from per-beam intrinsics only): device LutAnalyticT<T> + its tables
-    void* an{nullptr};
-    void* an_row{nullptr};
-    void* an_col{nullptr};
+    DeviceBlock an, an_row, an_col;
     bool analytic_on{false};
 };
 
 namespace ob {
 LutView lut_view(const ob_lut* lut) {
-    return LutView{lut->dir, lut->off, lut->dtype, lut->h, lut->w, lut->device, lut->analytic_on ? lut->an : nullptr};
+    return LutView{lut->dir.get(), lut->off.get(), lut->dtype, lut->h, lut->w, lut->device,
+                   lut->analytic_on ? lut->an.get() : nullptr};
 }
 cudaStream_t stream_handle(ob_stream* s) { return s->st; }
 
 cudaError_t stream_table(ob_stream* s, int which, const void* host, size_t bytes, const void** dev) {
     ob_stream::Table& t = s->tables[which];
-    if (t.dev != nullptr && t.host.size() == bytes && std::memcmp(t.host.data(), host, bytes) == 0) {
-        *dev = t.dev;  // identical to what the device already holds
+    if (t.dev.get() && t.host.size() == bytes && std::memcmp(t.host.data(), host, bytes) == 0) {
+        *dev = t.dev.get();  // identical to what the device already holds
         return cudaSuccess;
     }
-    if (bytes > t.cap) {
-        if (t.dev) {
+    if (bytes > t.dev.bytes()) {
+        if (t.dev.get()) {
             cudaError_t e = cudaStreamSynchronize(s->st);  // a running launch may still read the old table
             if (e != cudaSuccess) return e;
-            cudaFree(t.dev);
-            t.dev = nullptr;
-            t.cap = 0;
         }
-        const size_t cap = std::max<size_t>(bytes * 2, 4096);
-        cudaError_t e = cudaMalloc(&t.dev, cap);
+        cudaError_t e = t.dev.alloc(std::max<size_t>(bytes * 2, 4096));
         if (e != cudaSuccess) return e;
-        t.cap = cap;
     }
     t.host.assign(static_cast<const uint8_t*>(host), static_cast<const uint8_t*>(host) + bytes);
     // stream-ordered: lands after every earlier launch of this stream that reads the previous contents
-    cudaError_t e = cudaMemcpyAsync(t.dev, t.host.data(), bytes, cudaMemcpyHostToDevice, s->st);
+    cudaError_t e = cudaMemcpyAsync(t.dev.get(), t.host.data(), bytes, cudaMemcpyHostToDevice, s->st);
     if (e != cudaSuccess) {
         t.host.clear();
         return e;
     }
-    *dev = t.dev;
+    *dev = t.dev.get();
     return cudaSuccess;
 }
 int stream_device(ob_stream* s) { return s->device; }
@@ -470,11 +462,10 @@ void* ob_stream_cuda_handle(ob_stream* s) { return s ? static_cast<void*>(s->st)
 
 ob_status ob_stream_destroy(ob_stream* s) {
     if (!s) return OB_OK;
+    DeviceScope on(s->device);
     bool have_tables = false;
-    for (auto& t : s->tables) have_tables |= t.dev != nullptr;
+    for (auto& t : s->tables) have_tables |= t.dev.get() != nullptr;
     if (s->owned || have_tables) cudaStreamSynchronize(s->st);
-    for (auto& t : s->tables)
-        if (t.dev) cudaFree(t.dev);
     if (s->owned) cudaStreamDestroy(s->st);
     delete s;
     return OB_OK;
@@ -531,21 +522,20 @@ static cudaError_t build_analytic(ob_lut* l, double range_unit, const double* b2
     a.b23 = static_cast<T>(b23);
     for (int j = 0; j < 3; ++j)
         for (int k = 0; k < 4; ++k) a.m[4 * j + k] = static_cast<T>(tr[4 * j + k] * range_unit);
-    cudaError_t e = cudaMalloc(&l->an_row, row.size() * sizeof(T));
-    if (e == cudaSuccess) e = cudaMalloc(&l->an_col, col.size() * sizeof(T));
-    if (e == cudaSuccess) e = cudaMalloc(&l->an, sizeof(a));
-    if (e == cudaSuccess) e = cudaMemcpy(l->an_row, row.data(), row.size() * sizeof(T), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(l->an_col, col.data(), col.size() * sizeof(T), cudaMemcpyHostToDevice);
-    a.row = static_cast<const T*>(l->an_row);
-    a.col = static_cast<const T*>(l->an_col);
-    if (e == cudaSuccess) e = cudaMemcpy(l->an, &a, sizeof(a), cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) {
-        cudaFree(l->an);
-        cudaFree(l->an_row);
-        cudaFree(l->an_col);
-        l->an = l->an_row = l->an_col = nullptr;
-    }
-    return e;
+    DeviceBlock an, an_row, an_col;
+    cudaError_t e = an_row.alloc(row.size() * sizeof(T));
+    if (e == cudaSuccess) e = an_col.alloc(col.size() * sizeof(T));
+    if (e == cudaSuccess) e = an.alloc(sizeof(a));
+    if (e == cudaSuccess) e = cudaMemcpy(an_row.get(), row.data(), row.size() * sizeof(T), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(an_col.get(), col.data(), col.size() * sizeof(T), cudaMemcpyHostToDevice);
+    a.row = an_row.get<const T>();
+    a.col = an_col.get<const T>();
+    if (e == cudaSuccess) e = cudaMemcpy(an.get(), &a, sizeof(a), cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) return e;
+    l->an = std::move(an);
+    l->an_row = std::move(an_row);
+    l->an_col = std::move(an_col);
+    return cudaSuccess;
 }
 
 extern "C" {
@@ -559,22 +549,14 @@ ob_status ob_lut_create(ob_dtype dtype, const void* direction, const void* offse
     ob_status rs = require_device(device);
     if (rs != OB_OK) return rs;
     const size_t bytes = h * w * 3 * dtype_size(dtype);
-    void *d = nullptr, *o = nullptr;
-    cudaError_t e = cudaMalloc(&d, bytes);
+    std::unique_ptr<ob_lut> l(new ob_lut{device, static_cast<int>(dtype), h, w});
+    cudaError_t e = l->dir.alloc(bytes);
+    if (e == cudaSuccess) e = l->off.alloc(bytes);
     if (e != cudaSuccess) return fail_cuda(e, "cudaMalloc(lut)");
-    e = cudaMalloc(&o, bytes);
-    if (e != cudaSuccess) {
-        cudaFree(d);
-        return fail_cuda(e, "cudaMalloc(lut)");
-    }
-    e = cudaMemcpy(d, direction, bytes, cudaMemcpyDefault);
-    if (e == cudaSuccess) e = cudaMemcpy(o, offset, bytes, cudaMemcpyDefault);
-    if (e != cudaSuccess) {
-        cudaFree(d);
-        cudaFree(o);
-        return fail_cuda(e, "cudaMemcpy(lut)");
-    }
-    *out = new ob_lut{device, static_cast<int>(dtype), h, w, d, o};
+    e = cudaMemcpy(l->dir.get(), direction, bytes, cudaMemcpyDefault);
+    if (e == cudaSuccess) e = cudaMemcpy(l->off.get(), offset, bytes, cudaMemcpyDefault);
+    if (e != cudaSuccess) return fail_cuda(e, "cudaMemcpy(lut)");
+    *out = l.release();
     return OB_OK;
 }
 
@@ -594,43 +576,35 @@ ob_status ob_lut_from_intrinsics(ob_dtype dtype, size_t w, size_t h, double rang
     if (rs != OB_OK) return rs;
 
     const size_t n3 = w * h * 3;
-    double *daz = nullptr, *dalt = nullptr, *dd = nullptr, *doff = nullptr;
-    cudaError_t e = cudaMalloc(&daz, n_az * 8);
-    if (e == cudaSuccess) e = cudaMalloc(&dalt, n_alt * 8);
-    if (e == cudaSuccess) e = cudaMalloc(&dd, n3 * 8);
-    if (e == cudaSuccess) e = cudaMalloc(&doff, n3 * 8);
-    if (e == cudaSuccess) e = cudaMemcpy(daz, az, n_az * 8, cudaMemcpyDefault);
-    if (e == cudaSuccess) e = cudaMemcpy(dalt, alt, n_alt * 8, cudaMemcpyDefault);
-    if (e == cudaSuccess)
-        e = launch_make_lut(w, h, range_unit, b2l, transform, daz, n_az, dalt, n_alt, dd, doff, 0);
-    void *rd = dd, *ro = doff;
-    if (e == cudaSuccess && dtype == OB_F32) {
-        float *fd = nullptr, *fo = nullptr;
-        e = cudaMalloc(&fd, n3 * 4);
-        if (e == cudaSuccess) e = cudaMalloc(&fo, n3 * 4);
-        if (e == cudaSuccess) e = launch_cast_f64_f32(dd, fd, n3, 0);
-        if (e == cudaSuccess) e = launch_cast_f64_f32(doff, fo, n3, 0);
-        if (e == cudaSuccess) e = cudaDeviceSynchronize();
-        if (e == cudaSuccess) {
-            cudaFree(dd);
-            cudaFree(doff);
-            dd = doff = nullptr;
-            rd = fd;
-            ro = fo;
-        } else {
-            cudaFree(fd);
-            cudaFree(fo);
+    DeviceBlock dd, doff;  // the finished tables
+    cudaError_t e;
+    {  // the angles' device copies go before the LUT-free tables are allocated
+        DeviceBlock daz, dalt;
+        e = daz.alloc(n_az * 8);
+        if (e == cudaSuccess) e = dalt.alloc(n_alt * 8);
+        if (e == cudaSuccess) e = dd.alloc(n3 * 8);
+        if (e == cudaSuccess) e = doff.alloc(n3 * 8);
+        if (e == cudaSuccess) e = cudaMemcpy(daz.get(), az, n_az * 8, cudaMemcpyDefault);
+        if (e == cudaSuccess) e = cudaMemcpy(dalt.get(), alt, n_alt * 8, cudaMemcpyDefault);
+        if (e == cudaSuccess)
+            e = launch_make_lut(w, h, range_unit, b2l, transform, daz.get<double>(), n_az, dalt.get<double>(), n_alt,
+                                dd.get<double>(), doff.get<double>(), 0);
+        if (e == cudaSuccess && dtype == OB_F32) {
+            DeviceBlock fd, fo;
+            e = fd.alloc(n3 * 4);
+            if (e == cudaSuccess) e = fo.alloc(n3 * 4);
+            if (e == cudaSuccess) e = launch_cast_f64_f32(dd.get<double>(), fd.get<float>(), n3, 0);
+            if (e == cudaSuccess) e = launch_cast_f64_f32(doff.get<double>(), fo.get<float>(), n3, 0);
+            if (e == cudaSuccess) e = cudaDeviceSynchronize();
+            if (e == cudaSuccess) {
+                dd = std::move(fd);
+                doff = std::move(fo);
+            }
         }
+        if (e == cudaSuccess) e = cudaDeviceSynchronize();
     }
-    if (e == cudaSuccess) e = cudaDeviceSynchronize();
-    cudaFree(daz);
-    cudaFree(dalt);
-    if (e != cudaSuccess) {
-        cudaFree(dd);
-        cudaFree(doff);
-        return fail_cuda(e, "ob_lut_from_intrinsics");
-    }
-    ob_lut* l = new ob_lut{device, static_cast<int>(dtype), h, w, rd, ro};
+    if (e != cudaSuccess) return fail_cuda(e, "ob_lut_from_intrinsics");
+    ob_lut* l = new ob_lut{device, static_cast<int>(dtype), h, w, std::move(dd), std::move(doff)};
     if (n_az == h && n_alt == h) {  // per-beam angles: the LUT-free tables exist (off until ob_lut_set_analytic)
         cudaError_t ea = dtype == OB_F64 ? build_analytic<double>(l, range_unit, b2l, transform, az, alt)
                                          : build_analytic<float>(l, range_unit, b2l, transform, az, alt);
@@ -642,7 +616,7 @@ ob_status ob_lut_from_intrinsics(ob_dtype dtype, size_t w, size_t h, double rang
 
 ob_status ob_lut_set_analytic(ob_lut* lut, int enable) {
     if (!lut) return fail(OB_INVALID_ARGUMENT, "null lut");
-    if (enable && !lut->an)
+    if (enable && !lut->an.get())
         return fail(OB_INVALID_ARGUMENT, "LUT-free projection needs a lut built from per-beam intrinsics");
     lut->analytic_on = enable != 0;
     return OB_OK;
@@ -654,8 +628,8 @@ ob_status ob_lut_download(const ob_lut* lut, void* direction, void* offset) {
     if (!lut || !direction || !offset) return fail(OB_INVALID_ARGUMENT, "null pointer");
     const size_t bytes = lut->h * lut->w * 3 * dtype_size(lut->dtype);
     cudaSetDevice(lut->device);
-    cudaError_t e = cudaMemcpy(direction, lut->dir, bytes, cudaMemcpyDefault);
-    if (e == cudaSuccess) e = cudaMemcpy(offset, lut->off, bytes, cudaMemcpyDefault);
+    cudaError_t e = cudaMemcpy(direction, lut->dir.get(), bytes, cudaMemcpyDefault);
+    if (e == cudaSuccess) e = cudaMemcpy(offset, lut->off.get(), bytes, cudaMemcpyDefault);
     if (e != cudaSuccess) return fail_cuda(e, "ob_lut_download");
     return OB_OK;
 }
@@ -671,20 +645,15 @@ ob_status ob_lut_info(const ob_lut* lut, size_t* h, size_t* w, int* dtype, int* 
 
 ob_status ob_lut_device_ptrs(const ob_lut* lut, void** direction, void** offset) {
     if (!lut) return fail(OB_INVALID_ARGUMENT, "null lut");
-    if (direction) *direction = lut->dir;
-    if (offset) *offset = lut->off;
+    if (direction) *direction = lut->dir.get();
+    if (offset) *offset = lut->off.get();
     return OB_OK;
 }
 
 ob_status ob_lut_destroy(ob_lut* lut) {
     if (!lut) return OB_OK;
-    cudaSetDevice(lut->device);
-    forget_lut_tensor_maps(lut->dir);
-    cudaFree(lut->dir);
-    cudaFree(lut->off);
-    cudaFree(lut->an);
-    cudaFree(lut->an_row);
-    cudaFree(lut->an_col);
+    DeviceScope on(lut->device);
+    forget_lut_tensor_maps(lut->dir.get());
     delete lut;
     return OB_OK;
 }
@@ -718,9 +687,9 @@ static ob_status scan_to_cloud_t(const ob_lut* lut, const uint16_t* shift, const
         return dense(fs, rs, n) ? stg.out(p, count) : stg.inout(p, count);
     };
     CloudArgs<T> a;
-    a.dir = static_cast<const T*>(lut->dir);
-    a.off = static_cast<const T*>(lut->off);
-    a.analytic = lut->analytic_on ? static_cast<const LutAnalyticT<T>*>(lut->an) : nullptr;
+    a.dir = lut->dir.get<const T>();
+    a.off = lut->off.get<const T>();
+    a.analytic = lut->analytic_on ? lut->an.get<const LutAnalyticT<T>>() : nullptr;
     a.range_fs = io->range_frame_stride;
     a.range_rs = io->range_return_stride;
     a.xyz_fs = io->xyz_frame_stride;
@@ -880,8 +849,8 @@ static ob_status stage_k3_frame(const ob_lut* lut, const uint32_t* range, const 
     f.n_cg = (f.W + 31) / 32;
     f.n_slabs = (f.H + 15) / 16;
     f.index = index;
-    f.dir = lut->dir;
-    f.off = lut->off;
+    f.dir = lut->dir.get();
+    f.off = lut->off.get();
     const size_t n_px = lut->h * lut->w;
     f.range = stg.in(range, n_px);
     f.poses = stg.in(poses, lut->w * 16);

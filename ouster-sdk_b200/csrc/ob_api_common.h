@@ -1,8 +1,10 @@
 // ob_api_common.h -- helpers shared by the C-ABI translation units.
 #pragma once
 #include <initializer_list>
+#include <memory>
 #include <string>
 #include <type_traits>
+#include <utility>
 #include <vector>
 
 #include "ob_internal.h"
@@ -72,6 +74,84 @@ class Staging {
     cudaError_t err_ = cudaSuccess;
     std::vector<void*> scratch_;
     std::vector<Pending> pending_;
+};
+
+// Memory a handle keeps across calls: one cudaMalloc block (cudaHostAlloc when Pinned) and its size, freed when the
+// owner goes or takes another block.  Move-only.  Frees are not stream-ordered: cudaFree waits for the device.
+template <bool Pinned>
+class Block {
+   public:
+    Block() = default;
+    Block(Block&& o) noexcept : p_(std::exchange(o.p_, nullptr)), bytes_(std::exchange(o.bytes_, 0)) {}
+    Block& operator=(Block&& o) noexcept {
+        if (this != &o) {
+            release();
+            p_ = std::exchange(o.p_, nullptr);
+            bytes_ = std::exchange(o.bytes_, 0);
+        }
+        return *this;
+    }
+    ~Block() { release(); }
+    // frees the block, then allocates one of `bytes`; on failure the owner is left empty
+    cudaError_t alloc(size_t bytes) {
+        release();
+        void* p = nullptr;
+        cudaError_t e = Pinned ? cudaHostAlloc(&p, bytes, cudaHostAllocDefault) : cudaMalloc(&p, bytes);
+        if (e == cudaSuccess) {
+            p_ = p;
+            bytes_ = bytes;
+        }
+        return e;
+    }
+    // alloc(bytes) unless the block already has that many; the contents are not kept
+    cudaError_t reserve(size_t bytes) { return bytes <= bytes_ ? cudaSuccess : alloc(bytes); }
+    template <typename T = void>
+    T* get() const {
+        return static_cast<T*>(p_);
+    }
+    size_t bytes() const { return bytes_; }
+
+   private:
+    void release() {
+        if (p_) Pinned ? cudaFreeHost(p_) : cudaFree(p_);
+        p_ = nullptr;
+        bytes_ = 0;
+    }
+    void* p_ = nullptr;
+    size_t bytes_ = 0;
+};
+using DeviceBlock = Block<false>;
+using PinnedBlock = Block<true>;
+
+// A cudaEvent_t (timing disabled) a handle keeps across calls, destroyed with its owner.
+class Event {
+   public:
+    Event() = default;
+    Event(const Event&) = delete;
+    Event& operator=(const Event&) = delete;
+    ~Event() {
+        if (ev_) cudaEventDestroy(ev_);
+    }
+    cudaError_t create() { return cudaEventCreateWithFlags(&ev_, cudaEventDisableTiming); }
+    cudaEvent_t get() const { return ev_; }
+
+   private:
+    cudaEvent_t ev_ = nullptr;
+};
+
+// Makes `device` current for the scope and gives the caller's current device back when it ends.
+class DeviceScope {
+   public:
+    explicit DeviceScope(int device) {
+        cudaGetDevice(&prev_);
+        cudaSetDevice(device);
+    }
+    ~DeviceScope() { cudaSetDevice(prev_); }
+    DeviceScope(const DeviceScope&) = delete;
+    DeviceScope& operator=(const DeviceScope&) = delete;
+
+   private:
+    int prev_ = 0;
 };
 
 // A result whose length the GPU decides: rows in one or more arrays plus their count, each in host or device memory.

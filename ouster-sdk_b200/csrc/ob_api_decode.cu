@@ -388,39 +388,32 @@ struct ob_decode_job {
     ob_stream* s;
     cudaStream_t st;
     int device;
-    size_t stride;             // bytes per packet slot on the device (multiple of 16)
-    uint8_t* d_pk{nullptr};    // packet slots
+    size_t stride;        // bytes per packet slot on the device (multiple of 16)
+    DeviceBlock pk;       // packet slots
     size_t cap_slots{0};
-    size_t up_slots{0};        // highest uploaded slot + 1
-    uint8_t* d_out{nullptr};   // output slab (fields, headers, xyz, destaggered ranges)
-    size_t out_bytes{0};
-    int32_t* d_colsrc{nullptr};
-    int32_t* h_colsrc{nullptr};     // pinned
-    DecodeFrame* d_frame{nullptr};
-    DecodeFrame* h_frame{nullptr};  // pinned
-    cudaEvent_t ev_up{nullptr}, ev_done{nullptr};
+    size_t up_slots{0};   // highest uploaded slot + 1
+    DeviceBlock out;      // output slab (fields, headers, xyz, destaggered ranges)
+    DeviceBlock colsrc;   // int32 x W
+    PinnedBlock h_colsrc;
+    DeviceBlock frame;    // one DecodeFrame
+    PinnedBlock h_frame;
+    Event ev_up, ev_done;
     bool up_pending{false}, busy{false};
 };
 
 static cudaError_t job_reserve(ob_decode_job* j, size_t slots) {
     if (slots <= j->cap_slots) return cudaSuccess;
     const size_t cap = std::max(slots, j->cap_slots ? j->cap_slots * 2 : static_cast<size_t>(16));
-    uint8_t* p = nullptr;
-    cudaError_t e = cudaMalloc(&p, cap * j->stride + 16);
+    DeviceBlock p;
+    cudaError_t e = p.alloc(cap * j->stride + 16);
     if (e != cudaSuccess) return e;
-    if (j->d_pk) {  // rare: more packets than the frame was sized for (duplicates, retransmits)
+    if (j->pk.get()) {  // rare: more packets than the frame was sized for (duplicates, retransmits)
         e = cudaStreamSynchronize(j->st);
         if (e == cudaSuccess && j->up_slots)
-            e = cudaMemcpy(p, j->d_pk, j->up_slots * j->stride, cudaMemcpyDeviceToDevice);
-        cudaFree(j->d_pk);
-        if (e != cudaSuccess) {
-            cudaFree(p);
-            j->d_pk = nullptr;
-            j->cap_slots = 0;
-            return e;
-        }
+            e = cudaMemcpy(p.get(), j->pk.get(), j->up_slots * j->stride, cudaMemcpyDeviceToDevice);
+        if (e != cudaSuccess) return e;
     }
-    j->d_pk = p;
+    j->pk = std::move(p);
     j->cap_slots = cap;
     return cudaSuccess;
 }
@@ -438,33 +431,22 @@ ob_status ob_decode_job_create(const ob_decoder* dec, size_t reserve_slots, ob_s
     j->st = stream_handle(s);
     j->device = device;
     j->stride = (static_cast<size_t>(dec->L.packet_size) + 15) & ~static_cast<size_t>(15);
-    cudaError_t e = cudaEventCreateWithFlags(&j->ev_up, cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&j->ev_done, cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaMalloc(&j->d_colsrc, static_cast<size_t>(dec->L.W) * 4);
-    if (e == cudaSuccess) e = cudaHostAlloc(&j->h_colsrc, static_cast<size_t>(dec->L.W) * 4, cudaHostAllocDefault);
-    if (e == cudaSuccess) e = cudaMalloc(&j->d_frame, sizeof(DecodeFrame));
-    if (e == cudaSuccess) e = cudaHostAlloc(&j->h_frame, sizeof(DecodeFrame), cudaHostAllocDefault);
+    cudaError_t e = j->ev_up.create();
+    if (e == cudaSuccess) e = j->ev_done.create();
+    if (e == cudaSuccess) e = j->colsrc.alloc(static_cast<size_t>(dec->L.W) * 4);
+    if (e == cudaSuccess) e = j->h_colsrc.alloc(static_cast<size_t>(dec->L.W) * 4);
+    if (e == cudaSuccess) e = j->frame.alloc(sizeof(DecodeFrame));
+    if (e == cudaSuccess) e = j->h_frame.alloc(sizeof(DecodeFrame));
     if (e == cudaSuccess && reserve_slots) e = job_reserve(j.get(), reserve_slots);
-    if (e != cudaSuccess) {
-        ob_decode_job_destroy(j.release());
-        return fail_cuda(e, "decode job allocation");
-    }
+    if (e != cudaSuccess) return fail_cuda(e, "decode job allocation");
     *out = j.release();
     return OB_OK;
 }
 
 ob_status ob_decode_job_destroy(ob_decode_job* j) {
     if (!j) return OB_OK;
-    cudaSetDevice(j->device);
+    DeviceScope on(j->device);
     cudaStreamSynchronize(j->st);
-    if (j->ev_up) cudaEventDestroy(j->ev_up);
-    if (j->ev_done) cudaEventDestroy(j->ev_done);
-    cudaFree(j->d_pk);
-    cudaFree(j->d_out);
-    cudaFree(j->d_colsrc);
-    cudaFree(j->d_frame);
-    if (j->h_colsrc) cudaFreeHost(j->h_colsrc);
-    if (j->h_frame) cudaFreeHost(j->h_frame);
     delete j;
     return OB_OK;
 }
@@ -487,13 +469,13 @@ ob_status ob_decode_job_upload(ob_decode_job* j, const uint8_t* src, size_t src_
     }
     cudaError_t e = job_reserve(j, first_slot + count);
     if (e != cudaSuccess) return fail_cuda(e, "decode job packet slots");
-    uint8_t* dst = j->d_pk + first_slot * j->stride;
+    uint8_t* dst = j->pk.get<uint8_t>() + first_slot * j->stride;
     if (count == 1 || src_stride == j->stride)
         e = cudaMemcpyAsync(dst, src, (count - 1) * j->stride + psize, cudaMemcpyDefault, j->st);
     else
         e = cudaMemcpy2DAsync(dst, j->stride, src, src_stride, psize, count, cudaMemcpyDefault, j->st);
     if (e != cudaSuccess) return fail_cuda(e, "packet upload");
-    e = cudaEventRecord(j->ev_up, j->st);
+    e = cudaEventRecord(j->ev_up.get(), j->st);
     if (e != cudaSuccess) return fail_cuda(e, "packet upload event");
     j->up_pending = true;
     // an upload at slot 0 begins a new frame: slots of the previous one are no longer valid
@@ -504,7 +486,7 @@ ob_status ob_decode_job_upload(ob_decode_job* j, const uint8_t* src, size_t src_
 ob_status ob_decode_job_uploads_done(ob_decode_job* j) {
     if (!j) return fail(OB_INVALID_ARGUMENT, "null pointer");
     if (!j->up_pending) return OB_OK;
-    cudaError_t e = cudaEventSynchronize(j->ev_up);
+    cudaError_t e = cudaEventSynchronize(j->ev_up.get());
     j->up_pending = false;
     if (e != cudaSuccess) return fail_cuda(e, "packet upload");
     return OB_OK;
@@ -513,7 +495,7 @@ ob_status ob_decode_job_uploads_done(ob_decode_job* j) {
 ob_status ob_decode_job_wait(ob_decode_job* j) {
     if (!j) return fail(OB_INVALID_ARGUMENT, "null pointer");
     if (!j->busy) return OB_OK;
-    cudaError_t e = cudaEventSynchronize(j->ev_done);
+    cudaError_t e = cudaEventSynchronize(j->ev_done.get());
     j->busy = false;
     j->up_pending = false;
     if (e != cudaSuccess) return fail_cuda(e, "decode job");
@@ -570,33 +552,28 @@ ob_status ob_decode_job_submit(ob_decode_job* j, const ob_decode_io* io, const o
         o.off = need;
         need += o.bytes;
     }
-    cudaError_t e = cudaSuccess;
-    if (need > j->out_bytes) {  // job is idle here
-        cudaFree(j->d_out);
-        j->d_out = nullptr;
-        j->out_bytes = 0;
-        e = cudaMalloc(&j->d_out, need);
-        if (e != cudaSuccess) return fail_cuda(e, "decode job output slab");
-        j->out_bytes = need;
-    }
+    cudaError_t e = j->out.reserve(need);  // job is idle here
+    if (e != cudaSuccess) return fail_cuda(e, "decode job output slab");
+    uint8_t* slab = j->out.get<uint8_t>();
     DecodeFrame f;
     std::memset(&f, 0, sizeof(f));
-    for (size_t i = 0; i < n_out; ++i) set_out(f, outs[i].k, outs[i].host ? j->d_out + outs[i].off : outs[i].user);
-    f.packets = j->d_pk;
+    for (size_t i = 0; i < n_out; ++i) set_out(f, outs[i].k, outs[i].host ? slab + outs[i].off : outs[i].user);
+    f.packets = j->pk.get<uint8_t>();
     f.packet_stride = j->stride;
     f.n_slots = static_cast<uint32_t>(io->n_slots);
     if (io->col_src) {
-        std::memcpy(j->h_colsrc, io->col_src, static_cast<size_t>(L.W) * 4);
-        e = cudaMemcpyAsync(j->d_colsrc, j->h_colsrc, static_cast<size_t>(L.W) * 4, cudaMemcpyHostToDevice, j->st);
+        std::memcpy(j->h_colsrc.get(), io->col_src, static_cast<size_t>(L.W) * 4);
+        e = cudaMemcpyAsync(j->colsrc.get(), j->h_colsrc.get(), static_cast<size_t>(L.W) * 4, cudaMemcpyHostToDevice,
+                            j->st);
         if (e != cudaSuccess) return fail_cuda(e, "stage column map");
-        f.col_src = j->d_colsrc;
+        f.col_src = j->colsrc.get<int32_t>();
     }
     finish_frame(c, f, L.packet_size % 16 == 0, nullptr);  // slots are 16-byte aligned by construction
-    *j->h_frame = f;
-    e = cudaMemcpyAsync(j->d_frame, j->h_frame, sizeof(DecodeFrame), cudaMemcpyHostToDevice, j->st);
+    *j->h_frame.get<DecodeFrame>() = f;
+    e = cudaMemcpyAsync(j->frame.get(), j->h_frame.get(), sizeof(DecodeFrame), cudaMemcpyHostToDevice, j->st);
     if (e != cudaSuccess) return fail_cuda(e, "frame table upload");
     const void* xyz_base[OB_MAX_RETURNS] = {f.xyz[0], f.xyz[1]};  // a one-frame batch
-    e = launch(c, j->d_frame, 1, j->st, xyz_base, out_bytes(L, c.dtype, kOutReturns));  // kOutReturns: XYZ of return 0
+    e = launch(c, j->frame.get<DecodeFrame>(), 1, j->st, xyz_base, out_bytes(L, c.dtype, kOutReturns));  // kOutReturns: XYZ of return 0
     if (e != cudaSuccess) return fail_cuda(e, "decode launch");
     for (size_t k = 0; k < n_host;) {  // one D2H per run of outputs contiguous on both sides
         const Out& first = outs[order[k]];
@@ -606,11 +583,11 @@ ob_status ob_decode_job_submit(ob_decode_job* j, const ob_decode_io* io, const o
             bytes += outs[order[m]].bytes;
             ++m;
         }
-        e = cudaMemcpyAsync(first.user, j->d_out + first.off, bytes, cudaMemcpyDeviceToHost, j->st);
+        e = cudaMemcpyAsync(first.user, slab + first.off, bytes, cudaMemcpyDeviceToHost, j->st);
         if (e != cudaSuccess) return fail_cuda(e, "decode D2H");
         k = m;
     }
-    e = cudaEventRecord(j->ev_done, j->st);
+    e = cudaEventRecord(j->ev_done.get(), j->st);
     if (e != cudaSuccess) return fail_cuda(e, "decode job event");
     j->busy = true;
     return OB_OK;

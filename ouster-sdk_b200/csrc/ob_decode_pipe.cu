@@ -28,6 +28,7 @@
 #include <unordered_map>
 #include <vector>
 
+#include "ob_api_common.h"
 #include "ob_decode_tile.cuh"
 
 namespace ob {
@@ -915,9 +916,7 @@ const void* lut_tensor_maps(const void* dir, const void* off, int dtype, size_t 
                      CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
         if (ok) {
-            int cur = 0;
-            cudaGetDevice(&cur);
-            cudaSetDevice(device);
+            DeviceScope on(device);
             if (cudaMalloc(&dev, sizeof(maps)) == cudaSuccess) {
                 if (cudaMemcpy(dev, maps, sizeof(maps), cudaMemcpyHostToDevice) != cudaSuccess) {
                     cudaFree(dev);
@@ -927,7 +926,6 @@ const void* lut_tensor_maps(const void* dir, const void* off, int dtype, size_t 
                 dev = nullptr;
             }
             cudaGetLastError();
-            cudaSetDevice(cur);
         }
     }
     g_maps.emplace(key, dev);

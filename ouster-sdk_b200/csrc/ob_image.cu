@@ -511,60 +511,52 @@ unsigned ew_blocks(size_t n) { return unsigned(std::max<size_t>(1, std::min<size
 struct ob_image_proc {
     int device, kind;
     ob::HostParams p;
-    ob::DevState* st;
-    void* scratch;
-    size_t scratch_bytes;
-    double* dark;
-    uint32_t dark_cap;
+    ob::DeviceBlock st;       // one DevState
+    ob::DeviceBlock scratch;  // per-update scratch of BUC and LTM
+    ob::DeviceBlock dark;     // BUC's dark count, double x rows
 };
 
 using namespace ob;
 
 namespace {
 
-cudaError_t grow(void** buf, size_t* have, size_t need) {
-    if (need <= *have) return cudaSuccess;
-    cudaFree(*buf);
-    *buf = nullptr;
-    *have = 0;
-    cudaError_t e = cudaMalloc(buf, need);
-    if (e == cudaSuccess) *have = need;
-    return e;
-}
-
 template <typename T, int L>
 void launch_ae(ob_image_proc* p, const void* in, T* out, uint32_t npx, int update_state, cudaStream_t st) {
-    launch(OB_FAM_IMAGE, ae_select_kernel<T, L>, 1, kSelectThreads, 0, st, in, npx, p->st, p->p, update_state, 0);
+    DevState* ds = p->st.get<DevState>();
+    launch(OB_FAM_IMAGE, ae_select_kernel<T, L>, 1, kSelectThreads, 0, st, in, npx, ds, p->p, update_state, 0);
     const size_t n = size_t(npx) * (L == 0 ? 1 : 3);
-    launch(OB_FAM_IMAGE, ae_apply_kernel<T, L>, ew_blocks(n), kEwThreads, 0, st, in, out, n, p->st);
+    launch(OB_FAM_IMAGE, ae_apply_kernel<T, L>, ew_blocks(n), kEwThreads, 0, st, in, out, n, ds);
 }
 
 template <typename T, int L>
 void launch_ltm(ob_image_proc* p, const void* in, T* out, uint32_t rows, uint32_t cols, int update_state,
                 cudaStream_t st) {
     const uint32_t npx = rows * cols;
-    T* lum = static_cast<T*>(p->scratch);
-    float* luts = reinterpret_cast<float*>(static_cast<char*>(p->scratch) + ((size_t(npx) * sizeof(T) + 255) & ~size_t(255)));
-    launch(OB_FAM_IMAGE, ae_select_kernel<T, L>, 1, kSelectThreads, 0, st, in, npx, p->st, p->p, update_state, 1);
-    launch(OB_FAM_IMAGE, ltm_pixel_kernel<T, L>, ew_blocks(npx), kEwThreads, 0, st, in, out, lum, npx, p->st);
-    launch(OB_FAM_IMAGE, clahe_lut_kernel<T>, kTiles * kTiles, 1024, 0, st, lum, int(rows), int(cols), luts, p->st);
+    DevState* ds = p->st.get<DevState>();
+    T* lum = p->scratch.get<T>();
+    float* luts = reinterpret_cast<float*>(p->scratch.get<char>() + ((size_t(npx) * sizeof(T) + 255) & ~size_t(255)));
+    launch(OB_FAM_IMAGE, ae_select_kernel<T, L>, 1, kSelectThreads, 0, st, in, npx, ds, p->p, update_state, 1);
+    launch(OB_FAM_IMAGE, ltm_pixel_kernel<T, L>, ew_blocks(npx), kEwThreads, 0, st, in, out, lum, npx, ds);
+    launch(OB_FAM_IMAGE, clahe_lut_kernel<T>, kTiles * kTiles, 1024, 0, st, lum, int(rows), int(cols), luts, ds);
     launch(OB_FAM_IMAGE, ltm_apply_kernel<T>, ew_blocks(npx), kEwThreads, 0, st, out, lum, int(rows), int(cols), luts,
-           p->st, p->p.color_correct);
+           ds, p->p.color_correct);
 }
 
 template <typename T>
 void launch_buc(ob_image_proc* p, T* img, uint32_t rows, uint32_t cols, int update_state, cudaStream_t st) {
-    uint8_t* mask = static_cast<uint8_t*>(p->scratch);
-    T* dc = reinterpret_cast<T*>(static_cast<char*>(p->scratch) + ((size_t(cols) + 255) & ~size_t(255)));
+    DevState* ds = p->st.get<DevState>();
+    double* dark = p->dark.get<double>();
+    uint8_t* mask = p->scratch.get<uint8_t>();
+    T* dc = reinterpret_cast<T*>(p->scratch.get<char>() + ((size_t(cols) + 255) & ~size_t(255)));
     T* lu = dc + rows;
-    launch(OB_FAM_IMAGE, buc_mask_kernel<T>, ew_blocks(cols), kEwThreads, 0, st, img, rows, cols, mask, p->st,
+    launch(OB_FAM_IMAGE, buc_mask_kernel<T>, ew_blocks(cols), kEwThreads, 0, st, img, rows, cols, mask, ds,
            update_state);
     if (rows > 1)
-        launch(OB_FAM_IMAGE, buc_median_kernel<T>, rows - 1, kMedianThreads, 0, st, img, rows, cols, mask, dc, p->st,
+        launch(OB_FAM_IMAGE, buc_median_kernel<T>, rows - 1, kMedianThreads, 0, st, img, rows, cols, mask, dc, ds,
                update_state);
-    launch(OB_FAM_IMAGE, buc_tail_kernel<T>, 1, 1, 0, st, rows, cols, mask, dc, lu, p->dark, p->st, update_state);
+    launch(OB_FAM_IMAGE, buc_tail_kernel<T>, 1, 1, 0, st, rows, cols, mask, dc, lu, dark, ds, update_state);
     const size_t n = size_t(rows) * cols;
-    launch(OB_FAM_IMAGE, buc_apply_kernel<T>, ew_blocks(n), kEwThreads, 0, st, img, cols, n, p->dark);
+    launch(OB_FAM_IMAGE, buc_apply_kernel<T>, ew_blocks(n), kEwThreads, 0, st, img, cols, n, dark);
 }
 
 }  // namespace
@@ -587,17 +579,13 @@ ob_status ob_image_proc_create(int device, int kind, const ob_image_params* para
     }
     ob_status rs = require_device(device);
     if (rs != OB_OK) return rs;
-    cudaError_t e = cudaSetDevice(device);
-    ob_image_proc* p = new ob_image_proc{device, kind, hp, nullptr, nullptr, 0, nullptr, 0};
-    if (e == cudaSuccess) e = cudaMalloc(&p->st, sizeof(DevState));
+    std::unique_ptr<ob_image_proc> p(new ob_image_proc{device, kind, hp});
+    cudaError_t e = p->st.alloc(sizeof(DevState));
     DevState s0{};
     s0.lo = s0.hi = s0.lo_state = s0.hi_state = -1.0;
-    if (e == cudaSuccess) e = cudaMemcpy(p->st, &s0, sizeof(s0), cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) {
-        ob_image_proc_destroy(p);
-        return fail_cuda(e, "ob_image_proc_create");
-    }
-    *out = p;
+    if (e == cudaSuccess) e = cudaMemcpy(p->st.get(), &s0, sizeof(s0), cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) return fail_cuda(e, "ob_image_proc_create");
+    *out = p.release();
     return OB_OK;
 }
 
@@ -624,18 +612,12 @@ ob_status ob_image_proc_update(ob_image_proc* p, int layout, int dtype, const vo
     const size_t esz = dtype == OB_F64 ? 8 : 4;
     cudaError_t e = cudaSuccess;
     if (p->kind == OB_IMAGE_BEAM_UNIFORMITY) {
-        e = grow(&p->scratch, &p->scratch_bytes, ((size_t(cols) + 255) & ~size_t(255)) + 4 * size_t(rows) * esz);
-        if (e == cudaSuccess && rows > p->dark_cap) {
-            // the dark count keeps its values across calls only while the height stays the same; a new height
-            // recomputes it, so a larger buffer need not carry the old one over
-            cudaFree(p->dark);
-            p->dark = nullptr;
-            p->dark_cap = 0;
-            e = cudaMalloc(&p->dark, size_t(rows) * 8);
-            if (e == cudaSuccess) p->dark_cap = rows;
-        }
+        e = p->scratch.reserve(((size_t(cols) + 255) & ~size_t(255)) + 4 * size_t(rows) * esz);
+        // the dark count keeps its values across calls only while the height stays the same; a new height
+        // recomputes it, so a larger buffer need not carry the old one over
+        if (e == cudaSuccess) e = p->dark.reserve(size_t(rows) * 8);
     } else if (p->kind == OB_IMAGE_LOCAL_TONE_MAP) {
-        e = grow(&p->scratch, &p->scratch_bytes, ((npx * esz + 255) & ~size_t(255)) + size_t(kTiles * kTiles * kBins) * 4);
+        e = p->scratch.reserve(((npx * esz + 255) & ~size_t(255)) + size_t(kTiles * kTiles * kBins) * 4);
     }
     if (e != cudaSuccess) return fail_cuda(e, "image scratch");
     Staging stg(st);
@@ -680,12 +662,12 @@ ob_status ob_image_proc_state(const ob_image_proc* p, ob_image_state* state, dou
     if (rs != OB_OK) return rs;
     cudaStream_t st = stream_handle(s);
     DevState d;
-    cudaError_t e = cudaMemcpyAsync(&d, p->st, sizeof(d), cudaMemcpyDeviceToHost, st);
+    cudaError_t e = cudaMemcpyAsync(&d, p->st.get(), sizeof(d), cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     size_t nd = 0;
-    if (e == cudaSuccess && dark_count && p->dark) {
+    if (e == cudaSuccess && dark_count && p->dark.get()) {
         nd = std::min<size_t>(d.dc_rows, cap);
-        if (nd) e = cudaMemcpyAsync(dark_count, p->dark, nd * 8, cudaMemcpyDeviceToHost, st);
+        if (nd) e = cudaMemcpyAsync(dark_count, p->dark.get(), nd * 8, cudaMemcpyDeviceToHost, st);
         if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     }
     if (e != cudaSuccess) return fail_cuda(e, "image state");
@@ -695,13 +677,7 @@ ob_status ob_image_proc_state(const ob_image_proc* p, ob_image_state* state, dou
 
 ob_status ob_image_proc_destroy(ob_image_proc* p) {
     if (!p) return OB_OK;
-    int prev = 0;
-    cudaGetDevice(&prev);
-    cudaSetDevice(p->device);
-    cudaFree(p->st);
-    cudaFree(p->scratch);
-    cudaFree(p->dark);
-    cudaSetDevice(prev);
+    DeviceScope on(p->device);
     delete p;
     return OB_OK;
 }

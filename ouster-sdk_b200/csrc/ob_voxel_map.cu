@@ -46,20 +46,25 @@
 #include "ob_rows.cuh"
 #include "ob_voxel_common.cuh"
 
+// the slot arrays of the hash table
+struct VoxelSlots {
+    unsigned cap = 0;          // slots (power of two), 0 before the first insertion
+    ob::DeviceBlock key;       // int32 cap x 3
+    ob::DeviceBlock state;     // uint32 cap
+    ob::DeviceBlock stamp;     // uint64 cap
+    ob::DeviceBlock cnt;       // uint32 cap
+    ob::DeviceBlock pts;       // double cap x max_pts x 3
+    ob::DeviceBlock attr;      // double cap x max_pts x na, empty when na == 0
+};
+
 struct ob_voxel_map {
     int device;
     double voxel_size, max_distance, inv, res_sq;
     size_t max_pts, min_pts;
-    unsigned cap;                // slots (power of two), 0 before the first insertion
-    int32_t* key;                // cap x 3
-    uint32_t* state;             // cap
-    unsigned long long* stamp;   // cap
-    uint32_t* cnt;               // cap
-    double* pts;                 // cap x max_pts x 3
-    size_t na;                   // attributes per point (VoxelHashMapXd; 0 for VoxelHashMap3d)
-    double* attr;                // cap x max_pts x na, null when na == 0
-    unsigned long long* ctr;     // device counters, see Ctr
-    size_t occupied_bound;       // host upper bound of live + tombstone slots
+    size_t na;                 // attributes per point (VoxelHashMapXd; 0 for VoxelHashMap3d)
+    VoxelSlots slots;
+    ob::DeviceBlock ctr;       // device counters, see Ctr
+    size_t occupied_bound;     // host upper bound of live + tombstone slots
 };
 
 namespace ob {
@@ -81,10 +86,13 @@ struct Table {
     unsigned na;
 };
 
-Table table_of(const ob_voxel_map* m) {
-    return Table{m->cap,  m->key, m->state, m->stamp, m->cnt, m->pts, static_cast<unsigned>(m->max_pts),
-                 m->attr, static_cast<unsigned>(m->na)};
+Table table_of(const ob_voxel_map* m, const VoxelSlots& s) {
+    return Table{s.cap, s.key.get<int32_t>(), s.state.get<uint32_t>(), s.stamp.get<unsigned long long>(),
+                 s.cnt.get<uint32_t>(), s.pts.get<double>(), static_cast<unsigned>(m->max_pts), s.attr.get<double>(),
+                 static_cast<unsigned>(m->na)};
 }
+Table table_of(const ob_voxel_map* m) { return table_of(m, m->slots); }
+unsigned long long* counters(const ob_voxel_map* m) { return m->ctr.get<unsigned long long>(); }
 
 // columns 0-2 of row `row` of a rows x cols input
 template <typename T>
@@ -683,44 +691,18 @@ using namespace ob;
 
 namespace {
 
-void free_table(ob_voxel_map* m) {
-    cudaFree(m->key);
-    cudaFree(m->state);
-    cudaFree(m->stamp);
-    cudaFree(m->cnt);
-    cudaFree(m->pts);
-    cudaFree(m->attr);
-    m->key = nullptr;
-    m->state = nullptr;
-    m->stamp = nullptr;
-    m->cnt = nullptr;
-    m->pts = nullptr;
-    m->attr = nullptr;
-    m->cap = 0;
-}
-
 size_t table_bytes(size_t cap, size_t max_pts, size_t na) { return cap * (12 + 4 + 8 + 4 + (24 + 8 * na) * max_pts); }
 
-// a new, empty table in `t` (only its arrays and cap); on failure everything allocated here is freed again
-cudaError_t alloc_table(ob_voxel_map* t, unsigned cap, cudaStream_t st) {
-    t->key = nullptr;
-    t->state = nullptr;
-    t->stamp = nullptr;
-    t->cnt = nullptr;
-    t->pts = nullptr;
-    t->attr = nullptr;
+// a new, empty table of `cap` slots for the map `m` in `t`
+cudaError_t alloc_table(const ob_voxel_map* m, unsigned cap, cudaStream_t st, VoxelSlots* t) {
     t->cap = cap;
-    cudaError_t e = cudaMalloc(&t->key, cap * 12ull);
-    if (e == cudaSuccess) e = cudaMalloc(&t->state, cap * 4ull);
-    if (e == cudaSuccess) e = cudaMalloc(&t->stamp, cap * 8ull);
-    if (e == cudaSuccess) e = cudaMalloc(&t->cnt, cap * 4ull);
-    if (e == cudaSuccess) e = cudaMalloc(&t->pts, cap * t->max_pts * 24ull);
-    if (e == cudaSuccess && t->na) e = cudaMalloc(&t->attr, cap * t->max_pts * t->na * 8ull);
-    if (e == cudaSuccess) e = cudaMemsetAsync(t->state, 0, cap * 4ull, st);
-    if (e != cudaSuccess) {
-        cudaGetLastError();
-        free_table(t);
-    }
+    cudaError_t e = t->key.alloc(cap * 12ull);
+    if (e == cudaSuccess) e = t->state.alloc(cap * 4ull);
+    if (e == cudaSuccess) e = t->stamp.alloc(cap * 8ull);
+    if (e == cudaSuccess) e = t->cnt.alloc(cap * 4ull);
+    if (e == cudaSuccess) e = t->pts.alloc(cap * m->max_pts * 24ull);
+    if (e == cudaSuccess && m->na) e = t->attr.alloc(cap * m->max_pts * m->na * 8ull);
+    if (e == cudaSuccess) e = cudaMemsetAsync(t->state.get(), 0, cap * 4ull, st);
     return e;
 }
 
@@ -734,16 +716,16 @@ constexpr unsigned kMinSlots = 1024;
 // add to the occupied slots (rows, or the exact nv once it was read).
 ob_status reserve(ob_voxel_map* m, size_t rows, const uint32_t* nv_dev, cudaStream_t st, size_t* added) {
     *added = rows;
-    if (m->cap && m->occupied_bound + rows <= m->cap / 2) return OB_OK;
+    if (m->slots.cap && m->occupied_bound + rows <= m->slots.cap / 2) return OB_OK;
     unsigned long long c[C_WORDS] = {};
     uint32_t nv = 0;
-    cudaError_t e = cudaMemcpyAsync(c, m->ctr, sizeof(c), cudaMemcpyDeviceToHost, st);
+    cudaError_t e = cudaMemcpyAsync(c, counters(m), sizeof(c), cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaMemcpyAsync(&nv, nv_dev, 4, cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail_cuda(e, "voxel map counters");
     *added = nv;
     m->occupied_bound = static_cast<size_t>(c[C_OCCUPIED]);
-    if (m->cap && m->occupied_bound + nv <= m->cap / 2) return OB_OK;
+    if (m->slots.cap && m->occupied_bound + nv <= m->slots.cap / 2) return OB_OK;
     const size_t live = static_cast<size_t>(c[C_LIVE]);
     const size_t need = 4 * (live + nv);
     size_t cap = kMinSlots;
@@ -755,28 +737,18 @@ ob_status reserve(ob_voxel_map* m, size_t rows, const uint32_t* nv_dev, cudaStre
         return fail(OB_RUNTIME_ERROR, "voxel map: a table of " + std::to_string(cap) + " slots (" +
                                           std::to_string(table_bytes(cap, m->max_pts, m->na)) +
                                           " bytes) does not fit in free device memory");
-    ob_voxel_map nt = *m;
-    e = alloc_table(&nt, static_cast<unsigned>(cap), st);
+    VoxelSlots nt;
+    e = alloc_table(m, static_cast<unsigned>(cap), st, &nt);
     if (e != cudaSuccess) return fail_cuda(e, "voxel map allocation");
-    if (m->cap) {
-        launch(OB_FAM_VOXEL_MAP, vm_rehash_kernel, blocks_for(m->cap), 256, 0, st, table_of(m), table_of(&nt));
+    if (m->slots.cap) {
+        launch(OB_FAM_VOXEL_MAP, vm_rehash_kernel, blocks_for(m->slots.cap), 256, 0, st, table_of(m), table_of(m, nt));
         e = cudaGetLastError();
     }
     const unsigned long long occ = live;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(m->ctr + C_OCCUPIED, &occ, 8, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(counters(m) + C_OCCUPIED, &occ, 8, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);  // the old table is freed below, `occ` is on this stack
-    if (e != cudaSuccess) {
-        free_table(&nt);
-        return fail_cuda(e, "voxel map rehash");
-    }
-    free_table(m);
-    m->cap = nt.cap;
-    m->key = nt.key;
-    m->state = nt.state;
-    m->stamp = nt.stamp;
-    m->cnt = nt.cnt;
-    m->pts = nt.pts;
-    m->attr = nt.attr;
+    if (e != cudaSuccess) return fail_cuda(e, "voxel map rehash");
+    m->slots = std::move(nt);
     m->occupied_bound = live;
     return OB_OK;
 }
@@ -813,9 +785,9 @@ cudaError_t sort_batch(const ob_voxel_map* m, Rows r, unsigned cols, Staging& st
 // the second half: every distinct voxel of the batch into the table
 template <typename T>
 cudaError_t insert_batch(ob_voxel_map* m, Rows r, unsigned cols, const AddBatch& b, cudaStream_t st) {
-    launch(OB_FAM_VOXEL_MAP, vm_insert_kernel<T>, blocks_for(r.cap), 256, 0, st, r, cols, table_of(m), m->ctr, b.sk,
-           b.sseq, b.vrank, b.seg_start, m->res_sq);
-    launch(OB_FAM_VOXEL_MAP, vm_advance_stamp_kernel, 1, 1, 0, st, r.cap, b.vrank, m->ctr);
+    launch(OB_FAM_VOXEL_MAP, vm_insert_kernel<T>, blocks_for(r.cap), 256, 0, st, r, cols, table_of(m), counters(m),
+           b.sk, b.sseq, b.vrank, b.seg_start, m->res_sq);
+    launch(OB_FAM_VOXEL_MAP, vm_advance_stamp_kernel, 1, 1, 0, st, r.cap, b.vrank, counters(m));
     return cudaGetLastError();
 }
 
@@ -823,7 +795,7 @@ cudaError_t insert_batch(ob_voxel_map* m, Rows r, unsigned cols, const AddBatch&
 // *n_dev = the number of rows selected
 cudaError_t run_emit(const ob_voxel_map* m, const uint32_t* sel, Staging& stg, cudaStream_t st, double* out,
                      size_t capacity, unsigned long long* n_dev) {
-    const unsigned cap = m->cap;
+    const unsigned cap = m->slots.cap;
     if (cap == 0) return cudaMemsetAsync(n_dev, 0, 8, st);
     auto* keys = stg.scratch<unsigned long long>(cap);
     auto* skeys = stg.scratch<unsigned long long>(cap);
@@ -904,7 +876,7 @@ ob_status ob_voxel_map_create_xd(double voxel_size, double max_distance, size_t 
     if (num_attributes > 0xffffu) return fail(OB_INVALID_ARGUMENT, "num_attributes too large");
     ob_status rs = require_device(device);
     if (rs != OB_OK) return rs;
-    ob_voxel_map* m = new ob_voxel_map{};
+    std::unique_ptr<ob_voxel_map> m(new ob_voxel_map{});
     m->device = device;
     m->voxel_size = voxel_size;
     m->max_distance = max_distance;
@@ -913,22 +885,16 @@ ob_status ob_voxel_map_create_xd(double voxel_size, double max_distance, size_t 
     m->na = num_attributes;
     m->res_sq = voxel_size * voxel_size / static_cast<double>(max_points_per_voxel);  // :38
     m->inv = 1.0 / voxel_size;                                                          // :39
-    cudaError_t e = cudaMalloc(&m->ctr, C_WORDS * 8);
-    if (e == cudaSuccess) e = cudaMemset(m->ctr, 0, C_WORDS * 8);
-    if (e != cudaSuccess) {
-        cudaFree(m->ctr);
-        delete m;
-        return fail_cuda(e, "voxel map allocation");
-    }
-    *out = m;
+    cudaError_t e = m->ctr.alloc(C_WORDS * 8);
+    if (e == cudaSuccess) e = cudaMemset(m->ctr.get(), 0, C_WORDS * 8);
+    if (e != cudaSuccess) return fail_cuda(e, "voxel map allocation");
+    *out = m.release();
     return OB_OK;
 }
 
 ob_status ob_voxel_map_destroy(ob_voxel_map* m) {
     if (!m) return OB_OK;
-    cudaSetDevice(m->device);
-    free_table(m);
-    cudaFree(m->ctr);
+    DeviceScope on(m->device);
     delete m;
     return OB_OK;
 }
@@ -939,9 +905,9 @@ ob_status ob_voxel_map_clear(ob_voxel_map* m, ob_stream* s) {
     if (rs != OB_OK) return rs;
     cudaStream_t st = stream_handle(s);
     cudaError_t e = cudaSuccess;
-    if (m->cap) e = cudaMemsetAsync(m->state, 0, m->cap * 4ull, st);
+    if (m->slots.cap) e = cudaMemsetAsync(m->slots.state.get(), 0, m->slots.cap * 4ull, st);
     // the stamp counter keeps running: creation order stays monotone across clears
-    if (e == cudaSuccess) e = cudaMemsetAsync(m->ctr + C_LIVE, 0, (C_WORDS - C_LIVE) * 8, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(counters(m) + C_LIVE, 0, (C_WORDS - C_LIVE) * 8, st);
     if (e != cudaSuccess) return fail_cuda(e, "voxel map clear");
     m->occupied_bound = 0;
     return OB_OK;
@@ -995,18 +961,18 @@ ob_status ob_voxel_map_remove_far(ob_voxel_map* m, const ob_voxel_map_cull_io* i
     CountedRows res(io->n_extracted, io->extracted ? io->capacity : CountedRows::kCountOnly, stg, st, "voxel map cull");
     const double* org = stg.in(io->origin, 3);
     if (cudaError_t e = stg.error()) return fail_cuda(e, "stage origin");
-    if (!m->cap) return res.zero();
+    if (!m->slots.cap) return res.zero();
     if (extract) {  // refused before the cull, so a refused call leaves the map as it was
         rs = res.refuse({io->extracted}, kMixedCount);
         if (rs != OB_OK) return rs;
     }
     uint32_t* removed = nullptr;
     if (extract) {
-        removed = stg.scratch<uint32_t>(m->cap);
+        removed = stg.scratch<uint32_t>(m->slots.cap);
         if (cudaError_t e = stg.error()) return fail_cuda(e, "voxel map cull");
     }
-    launch(OB_FAM_VOXEL_MAP, vm_cull_kernel, blocks_for(m->cap), 256, 0, st, table_of(m), m->ctr, org, m->inv,
-           cull_threshold(m->max_distance, m->inv), removed);
+    launch(OB_FAM_VOXEL_MAP, vm_cull_kernel, blocks_for(m->slots.cap), 256, 0, st, table_of(m), counters(m), org,
+           m->inv, cull_threshold(m->max_distance, m->inv), removed);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail_cuda(e, "voxel map cull");
     if (!extract) return OB_OK;
@@ -1021,7 +987,7 @@ ob_status ob_voxel_map_point_cloud(const ob_voxel_map* m, double* points, size_t
     Staging stg(st);
     // as ob_voxel_map_remove_far: a device count is zeroed only for an empty map or a refused call
     CountedRows res(n_out, points ? capacity : CountedRows::kCountOnly, stg, st, "voxel map point cloud");
-    if (!m->cap) return res.zero();
+    if (!m->slots.cap) return res.zero();
     rs = res.refuse({points}, kMixedCount);
     if (rs != OB_OK) return rs;
     return emit_rows(m, nullptr, stg, st, points, capacity, res, "voxel map point cloud");
@@ -1033,7 +999,7 @@ ob_status ob_voxel_map_size(const ob_voxel_map* m, size_t* voxels, size_t* point
     if (rs != OB_OK) return rs;
     cudaStream_t st = stream_handle(s);
     unsigned long long c[C_WORDS] = {};
-    cudaError_t e = cudaMemcpyAsync(c, m->ctr, sizeof(c), cudaMemcpyDeviceToHost, st);
+    cudaError_t e = cudaMemcpyAsync(c, counters(m), sizeof(c), cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail_cuda(e, "voxel map size");
     if (c[C_FULL]) return fail(OB_RUNTIME_ERROR, "voxel map table overflow");
@@ -1124,9 +1090,9 @@ ob_status ob_icp_align(const ob_voxel_map* m, const ob_icp_io* io, ob_stream* s)
     const double md2 = io->max_distance * io->max_distance;  // square(max_correspondance_distance)
     const double crit_sq = io->convergence_criterion * io->convergence_criterion;
     if (io->source.dtype == OB_F64)
-        launch(OB_FAM_ICP, icp_init_kernel<double>, nb, kAssocThreads, 0, st, r, m->ctr, src, state);
+        launch(OB_FAM_ICP, icp_init_kernel<double>, nb, kAssocThreads, 0, st, r, counters(m), src, state);
     else
-        launch(OB_FAM_ICP, icp_init_kernel<float>, nb, kAssocThreads, 0, st, r, m->ctr, src, state);
+        launch(OB_FAM_ICP, icp_init_kernel<float>, nb, kAssocThreads, 0, st, r, counters(m), src, state);
     for (int it = 0; it < io->max_num_iterations; ++it) {
         launch(OB_FAM_ICP, icp_assoc_kernel, nb, kAssocThreads, 0, st, r, t, m->inv, m->voxel_size, md2, src, tgt,
                valid, bc, state);

@@ -19,11 +19,10 @@
 struct ob_zone_monitor {
     int device;
     uint32_t h, w, n_live;
-    uint32_t* near_mm;  // n_live x h x w
-    uint32_t* far_mm;
-    void* acc;          // ZoneAcc[OB_ZONE_MAX_LIVE]
-    void* ctl;          // ZoneCtl[OB_ZONE_MAX_LIVE]
-    ob_zone_state* states;  // [OB_ZONE_MAX_LIVE]
+    ob::DeviceBlock near_mm, far_mm;  // uint32 n_live x h x w
+    ob::DeviceBlock acc;              // ZoneAcc[OB_ZONE_MAX_LIVE]
+    ob::DeviceBlock ctl;              // ZoneCtl[OB_ZONE_MAX_LIVE]
+    ob::DeviceBlock states;           // ob_zone_state[OB_ZONE_MAX_LIVE]
 };
 
 namespace ob {
@@ -446,41 +445,39 @@ ob_status ob_zone_monitor_create(int device, uint32_t n_rows, uint32_t n_cols, c
         if (npx && (!live[i].near_mm || !live[i].far_mm)) return fail(OB_INVALID_ARGUMENT, "null zone image");
     ob_status rs = require_device(device);
     if (rs != OB_OK) return rs;
-    cudaError_t e = cudaSetDevice(device);
-    ob_zone_monitor* m = new ob_zone_monitor{device, n_rows, n_cols, n_live, nullptr, nullptr, nullptr, nullptr, nullptr};
+    std::unique_ptr<ob_zone_monitor> m(new ob_zone_monitor{device, n_rows, n_cols, n_live});
     const size_t img = npx * 4;
-    if (e == cudaSuccess) e = cudaMalloc(&m->near_mm, std::max<size_t>(img * n_live, 4));
-    if (e == cudaSuccess) e = cudaMalloc(&m->far_mm, std::max<size_t>(img * n_live, 4));
-    if (e == cudaSuccess) e = cudaMalloc(&m->acc, sizeof(ZoneAcc) * OB_ZONE_MAX_LIVE);
-    if (e == cudaSuccess) e = cudaMalloc(&m->ctl, sizeof(ZoneCtl) * OB_ZONE_MAX_LIVE);
-    if (e == cudaSuccess) e = cudaMalloc(&m->states, sizeof(ob_zone_state) * OB_ZONE_MAX_LIVE);
+    cudaError_t e = m->near_mm.alloc(std::max<size_t>(img * n_live, 4));
+    if (e == cudaSuccess) e = m->far_mm.alloc(std::max<size_t>(img * n_live, 4));
+    if (e == cudaSuccess) e = m->acc.alloc(sizeof(ZoneAcc) * OB_ZONE_MAX_LIVE);
+    if (e == cudaSuccess) e = m->ctl.alloc(sizeof(ZoneCtl) * OB_ZONE_MAX_LIVE);
+    if (e == cudaSuccess) e = m->states.alloc(sizeof(ob_zone_state) * OB_ZONE_MAX_LIVE);
+    uint32_t* near_mm = m->near_mm.get<uint32_t>();
+    uint32_t* far_mm = m->far_mm.get<uint32_t>();
     ZoneCtl ctl[OB_ZONE_MAX_LIVE] = {};
     for (uint32_t i = 0; i < n_live; ++i) {
         ctl[i] = ZoneCtl{live[i].id, uint32_t(live[i].mode), live[i].point_count, live[i].frame_count,
                          live[i].triggers, live[i].alerts, 0, 0, 0};
-        if (e == cudaSuccess && img) e = cudaMemcpy(m->near_mm + i * npx, live[i].near_mm, img, cudaMemcpyDefault);
-        if (e == cudaSuccess && img) e = cudaMemcpy(m->far_mm + i * npx, live[i].far_mm, img, cudaMemcpyDefault);
+        if (e == cudaSuccess && img) e = cudaMemcpy(near_mm + i * npx, live[i].near_mm, img, cudaMemcpyDefault);
+        if (e == cudaSuccess && img) e = cudaMemcpy(far_mm + i * npx, live[i].far_mm, img, cudaMemcpyDefault);
     }
-    if (e == cudaSuccess) e = cudaMemcpy(m->ctl, ctl, sizeof(ctl), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(m->ctl.get(), ctl, sizeof(ctl), cudaMemcpyHostToDevice);
     // states before the first update: what get_packet() gives for slots that have not been computed
     ob_zone_state st0[OB_ZONE_MAX_LIVE] = {};
     for (uint32_t i = n_live; i < OB_ZONE_MAX_LIVE; ++i) st0[i].id = 255;
-    if (e == cudaSuccess) e = cudaMemcpy(m->states, st0, sizeof(st0), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(m->states.get(), st0, sizeof(st0), cudaMemcpyHostToDevice);
     if (e == cudaSuccess) {
-        launch(OB_FAM_ZONE, zone_acc_reset_kernel, 1, 32, 0, 0, static_cast<ZoneAcc*>(m->acc));
+        launch(OB_FAM_ZONE, zone_acc_reset_kernel, 1, 32, 0, 0, m->acc.get<ZoneAcc>());
         if (n_live && npx) {
             const dim3 grid(unsigned(std::min<size_t>((npx + 255) / 256, 1024)), n_live);
-            launch(OB_FAM_ZONE, zone_max_count_kernel, grid, 256, 0, 0, m->near_mm, m->far_mm, uint32_t(npx),
-                   static_cast<ZoneCtl*>(m->ctl));
+            launch(OB_FAM_ZONE, zone_max_count_kernel, grid, 256, 0, 0, near_mm, far_mm, uint32_t(npx),
+                   m->ctl.get<ZoneCtl>());
         }
         e = cudaGetLastError();
     }
     if (e == cudaSuccess) e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) {
-        ob_zone_monitor_destroy(m);
-        return fail_cuda(e, "ob_zone_monitor_create");
-    }
-    *out = m;
+    if (e != cudaSuccess) return fail_cuda(e, "ob_zone_monitor_create");
+    *out = m.release();
     return OB_OK;
 }
 
@@ -500,9 +497,10 @@ ob_status ob_zone_monitor_update(ob_zone_monitor* m, const uint32_t* range, uint
     if (cudaError_t e = stg.error()) return fail_cuda(e, "stage zone update");
     if (npx)
         launch(OB_FAM_ZONE, zone_occupancy_kernel, unsigned((npx + kOccTile - 1) / kOccTile), kOccThreads, 0, st, r,
-               m->near_mm, m->far_mm, m->n_live, uint32_t(npx), static_cast<ZoneAcc*>(m->acc), bm);
-    launch(OB_FAM_ZONE, zone_tail_kernel, 1, 32, 0, st, static_cast<ZoneAcc*>(m->acc), static_cast<ZoneCtl*>(m->ctl),
-           m->n_live, m->states);
+               m->near_mm.get<uint32_t>(), m->far_mm.get<uint32_t>(), m->n_live, uint32_t(npx), m->acc.get<ZoneAcc>(),
+               bm);
+    launch(OB_FAM_ZONE, zone_tail_kernel, 1, 32, 0, st, m->acc.get<ZoneAcc>(), m->ctl.get<ZoneCtl>(), m->n_live,
+           m->states.get<ob_zone_state>());
     stg.check(cudaGetLastError());
     cudaError_t e = stg.flush();
     if (e == cudaSuccess && (host_bm || (npx && !is_device_ptr(range)))) e = cudaStreamSynchronize(st);
@@ -516,7 +514,7 @@ ob_status ob_zone_monitor_states(const ob_zone_monitor* m, void* out, ob_stream*
     if (rs != OB_OK) return rs;
     cudaStream_t st = stream_handle(s);
     const bool dev = is_device_ptr(out);
-    cudaError_t e = cudaMemcpyAsync(out, m->states, sizeof(ob_zone_state) * OB_ZONE_MAX_LIVE,
+    cudaError_t e = cudaMemcpyAsync(out, m->states.get(), sizeof(ob_zone_state) * OB_ZONE_MAX_LIVE,
                                     dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess && !dev) e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail_cuda(e, "zone states");
@@ -530,7 +528,7 @@ ob_status ob_zone_monitor_counters(const ob_zone_monitor* m, uint32_t* triggers,
     if (rs != OB_OK) return rs;
     ZoneCtl ctl[OB_ZONE_MAX_LIVE];
     cudaStream_t st = stream_handle(s);
-    cudaError_t e = cudaMemcpyAsync(ctl, m->ctl, sizeof(ctl), cudaMemcpyDeviceToHost, st);
+    cudaError_t e = cudaMemcpyAsync(ctl, m->ctl.get(), sizeof(ctl), cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail_cuda(e, "zone counters");
     for (uint32_t i = 0; i < m->n_live; ++i) {
@@ -543,15 +541,7 @@ ob_status ob_zone_monitor_counters(const ob_zone_monitor* m, uint32_t* triggers,
 
 ob_status ob_zone_monitor_destroy(ob_zone_monitor* m) {
     if (!m) return OB_OK;
-    int prev = 0;
-    cudaGetDevice(&prev);
-    cudaSetDevice(m->device);
-    cudaFree(m->near_mm);
-    cudaFree(m->far_mm);
-    cudaFree(m->acc);
-    cudaFree(m->ctl);
-    cudaFree(m->states);
-    cudaSetDevice(prev);
+    DeviceScope on(m->device);
     delete m;
     return OB_OK;
 }
