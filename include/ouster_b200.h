@@ -1029,7 +1029,11 @@ ob_status ob_decode_frames(const ob_decoder* dec, const ob_decode_io* frames, si
 
 /* Uniformly strided batch of COMPLETE, in-order frames (identity column map): frame f of every
  * array lives `*_frame_stride` BYTES after frame f-1.  Same products as ob_decode_frames with O(1)
- * host work per call -- the form a packet ring / frame pool uses. */
+ * host work per call -- the form a packet ring / frame pool uses.
+ * Each output is written in its n_frames blocks (one frame's image or header array) and nowhere else, in host
+ * and device memory alike: the bytes between two frames' blocks keep their contents, so outputs may interleave
+ * in one allocation (K1's [frame][return] XYZ layout, or a pool that holds all outputs of a frame back to back).
+ * A host output with such gaps is decoded into dense device scratch and copied back one block per frame. */
 typedef struct ob_decode_batch {
     uint32_t n_frames;
     const uint8_t* packets; /* frame f, slot k at packets + f*packets_frame_stride + k*packet_stride */

@@ -157,7 +157,15 @@ void* Staging::stage(const void* p, size_t bytes, bool upload, bool download) {
     if (bytes == 0 || p == nullptr || is_device_ptr(p)) return const_cast<void*>(p);
     void* d = scratch_bytes(bytes);
     if (d && upload) check(cudaMemcpyAsync(d, p, bytes, cudaMemcpyHostToDevice, st_));
-    if (d && download) pending_.push_back({const_cast<void*>(p), d, bytes});
+    if (d && download) pending_.push_back({const_cast<void*>(p), d, bytes, bytes, 1});
+    return d;
+}
+
+void* Staging::out_rows(void* p, size_t row_bytes, size_t pitch, size_t rows) {
+    if (err_ != cudaSuccess) return nullptr;
+    if (row_bytes == 0 || rows == 0 || p == nullptr || is_device_ptr(p)) return p;
+    void* d = scratch_bytes(row_bytes * rows);
+    if (d) pending_.push_back({p, d, row_bytes, pitch, rows});
     return d;
 }
 
@@ -170,8 +178,12 @@ void* Staging::scratch_bytes(size_t bytes) {
 }
 
 cudaError_t Staging::flush() {
-    for (const Pending& q : pending_)
-        if (err_ == cudaSuccess) check(cudaMemcpyAsync(q.host, q.dev, q.bytes, cudaMemcpyDeviceToHost, st_));
+    for (const Pending& q : pending_) {
+        if (err_ != cudaSuccess) break;
+        check(q.rows == 1 ? cudaMemcpyAsync(q.host, q.dev, q.bytes, cudaMemcpyDeviceToHost, st_)
+                          : cudaMemcpy2DAsync(q.host, q.pitch, q.dev, q.bytes, q.bytes, q.rows,
+                                              cudaMemcpyDeviceToHost, st_));
+    }
     pending_.clear();
     return err_;
 }

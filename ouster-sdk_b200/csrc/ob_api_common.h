@@ -23,6 +23,9 @@ void reduce_shifts(const int32_t* shifts, size_t h, size_t w, int inverse, std::
 // out(): scratch now, D2H issued by flush() after the kernel.
 // inout(): as out(), but the host contents are uploaded first, so bytes the kernel leaves alone
 //          (padding between strided frames) come back unchanged.
+// out_rows(): out() for `rows` blocks of `row_bytes` that lie `pitch` bytes apart on the host.  The scratch holds
+//          them back to back and flush() copies each block to its place: host bytes between the blocks are
+//          neither read nor written.
 // scratch(): device memory for the call, freed in stream order when the Staging goes (at least 16 bytes).
 // The first CUDA error of the call is kept: error() returns it, and from then on in / out / inout / scratch return
 // null and make no CUDA call, and flush() / finish() return it.  check() records an error met outside the Staging.
@@ -47,6 +50,7 @@ class Staging {
     T* inout(T* p, size_t n) {
         return static_cast<T*>(stage(p, n * elem_bytes<T>(), true, true));
     }
+    void* out_rows(void* p, size_t row_bytes, size_t pitch, size_t rows);
     template <typename T>
     T* scratch(size_t n) {
         return static_cast<T*>(scratch_bytes(n * elem_bytes<T>()));
@@ -65,10 +69,12 @@ class Staging {
     // scratch for a host buffer, filled from it (upload) and copied back to it by flush() (download)
     void* stage(const void* p, size_t bytes, bool upload, bool download);
     void* scratch_bytes(size_t bytes);
-    struct Pending {
+    struct Pending {  // `rows` blocks of `bytes`, dense on the device, `pitch` apart on the host
         void* host;
         void* dev;
         size_t bytes;
+        size_t pitch;
+        size_t rows;
     };
     cudaStream_t st_;
     cudaError_t err_ = cudaSuccess;

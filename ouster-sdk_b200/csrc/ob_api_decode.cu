@@ -353,11 +353,22 @@ ob_status ob_decode_batch_run(const ob_decoder* dec, const ob_decode_batch* b, c
     const uint8_t* dpk =
         stg.in(b->packets, span(b->packets_frame_stride, (b->n_slots - 1) * b->packet_stride + L.packet_size));
     if (cudaError_t e = stg.error()) return fail_cuda(e, "stage packets");
-    void* dout[kOuts] = {};  // frame 0's outputs
+    void* dout[kOuts] = {};       // frame 0's outputs as the kernel writes them ...
+    size_t dstride[kOuts] = {};   // ... and the bytes from one frame's to the next's there
     for (int k = 0; k < kOuts; ++k) {
         void* user = io_out(L, *b, k);
         if (!user) continue;
-        dout[k] = stg.out(user, span(batch_stride(*b, k), out_bytes(L, c.dtype, k)));
+        const size_t fs = batch_stride(*b, k), block = out_bytes(L, c.dtype, k);
+        if (F > 1 && fs > block) {
+            // a host output with gaps between its frames is decoded into dense scratch and copied back block by
+            // block: the gaps (padding, or the frames of another output that shares the allocation) keep the
+            // caller's bytes
+            dout[k] = stg.out_rows(user, block, fs, F);
+            dstride[k] = dout[k] == user ? fs : block;
+        } else {
+            dout[k] = stg.out(user, span(fs, block));
+            dstride[k] = fs;
+        }
         if (cudaError_t e = stg.error()) return fail_cuda(e, "stage outputs");
     }
     const bool bulk_ok = al16(dpk) && b->packet_stride % 16 == 0 && L.packet_size % 16 == 0 &&
@@ -370,13 +381,16 @@ ob_status ob_decode_batch_run(const ob_decoder* dec, const ob_decode_batch* b, c
         d.packet_stride = b->packet_stride;
         d.n_slots = static_cast<uint32_t>(b->n_slots);
         for (int k = 0; k < kOuts; ++k)
-            if (dout[k]) set_out(d, k, static_cast<uint8_t*>(dout[k]) + f * batch_stride(*b, k));
+            if (dout[k]) set_out(d, k, static_cast<uint8_t*>(dout[k]) + f * dstride[k]);
         finish_frame(c, d, bulk_ok, frame_luts.empty() ? nullptr : &frame_luts[f]);
     }
     // the frames' XYZ pointers show a stride that breaks alignment only when there are two of them
-    if (c.any_xyz && b->xyz_frame_stride % 16) c.vec_ok = false;
+    const size_t xs0 = dstride[kOutReturns], xs1 = dstride[kOutReturns + 2];
+    if (c.any_xyz && (xs0 | xs1) % 16) c.vec_ok = false;
+    // the XYZ outputs as one strided batch: only when both returns are written with one frame stride
+    const bool one_xyz_stride = !dout[kOutReturns] || !dout[kOutReturns + 2] || xs0 == xs1;
     const void* xyz_base[OB_MAX_RETURNS] = {hf[0].xyz[0], hf[0].xyz[1]};
-    return run_table(c, s, hf, stg, xyz_base, b->xyz_frame_stride);
+    return run_table(c, s, hf, stg, one_xyz_stride ? xyz_base : nullptr, xs0);
 }
 
 
