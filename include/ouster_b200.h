@@ -235,6 +235,12 @@ ob_status ob_frames_interp_pose(const ob_frame_poses_item* frames, size_t n_fram
  * ceil(min_range*1e3) <= r <= floor(max_range*1e3) are emitted top to bottom as R_col*lut(r) + t_col
  * (body_to_world cast to the LUT dtype) -- the reference's order and arithmetic, without
  * materialising the full cloud first (the fusion its own note at dewarp_impl.h:27-29 asks for).
+ * Range window: ceil(min_range*1e3) and floor(max_range*1e3) are computed in double, as the reference does, and
+ * must both be finite and in [0, 4294967295] (a ceil of -0.0 counts as 0); otherwise the call fails with
+ * OB_INVALID_ARGUMENT before anything is staged, since the reference's conversion of such a bound to uint32 is
+ * undefined.  To keep every range, pass max_range = 4294967.295.  A minimum above the maximum is a valid, empty
+ * window (nothing is launched).  Frames may have at most 25600 rows (a taller one fails with OB_INVALID_ARGUMENT
+ * before anything is staged).
  * ONE kernel launch (count, decoupled look-back scan and emit fused; the count is a device-side word).
  * n_points in host memory: the call waits for the count and, when outputs are in host memory, then for their
  * points (host outputs are final on return, device outputs after ob_stream_sync); it raises
@@ -267,7 +273,9 @@ ob_status ob_dewarp_frame(const ob_lut* lut, const ob_dewarp_frame_io* io, size_
  * look-back chain of the compaction simply continues across the frames); n_points may be device memory as
  * for ob_dewarp_frame (then counts must be NULL).
  * Optional per-point provenance: frame index, column index, column timestamp (dewarp_impl.h:88-90).
- * counts[i] (optional, n_frames entries) = points of frame i.  Buffers may be host or device memory.
+ * counts[i] (optional, n_frames entries, host memory) = points of slot i; zeroed on entry and filled only by a
+ * call that succeeds.
+ * Buffers may be host or device memory.  The range window and row limit are those of ob_dewarp_frame.
  * errors: "output capacity too small", "the luts of a set must share one dtype". */
 typedef struct ob_dewarp_frames_io {
     const ob_lut* lut;           /* NULL: no frame in this slot */

@@ -373,6 +373,9 @@ def dewarp_frame(lut, rng, poses, status, timestamps=None, min_range=0.0, max_ra
     """dewarp(lidar_frame, xyzlut, min_range, max_range) (pose_util.h:456-485): project the range
     image, apply each column's body_to_world pose, keep the points with min_range <= r <= max_range
     (metres) of the columns between the first and last valid one, in column-major order.
+    The default max_range=inf is passed as 4294967.295 m, the largest window the C ABI takes; any other window whose
+    ceil(min_range * 1e3) or floor(max_range * 1e3) lies outside [0, 4294967295] mm raises ValueError, as does a
+    frame of more than 25600 rows.
     Returns points [n, 3] (LUT dtype); with provenance=True also (col_idx u32 [n], timestamps u64 [n]).
     One fused GPU launch: nothing but the surviving points is written.
     Asynchronous device form: `out` = CUDA tensor [capacity, 3] of the LUT dtype and `out_count` = CUDA int64
@@ -1016,6 +1019,7 @@ def dewarp_frames(frames, min_range=0.0, max_range=float("inf"), provenance=Fals
     `frames` is a list with one entry per slot of the set -- None for an empty slot, else a dict
     {lut, range, poses, status[, timestamps]} -- and the result is the concatenation of the frames'
     dewarped points in slot order.  provenance=True also returns (frame_idx, col_idx, timestamps).
+    The range window and row limit are dewarp_frame's (the default max_range=inf is passed as 4294967.295 m).
     One launch for the whole set."""
     from ._capi import DewarpFramesIO
     n = len(frames)

@@ -181,8 +181,7 @@ cudaError_t launch_dewarp_fused(const K3Frame* frames_dev, unsigned n_frames, un
     if (frame_end_dev) *frame_end_dev = sc.frame_end;
     cudaError_t e = cudaMemsetAsync(b, 0, k3_state_bytes(n_blocks), st);  // ticket + state words
     if (e != cudaSuccess) return e;
-    const size_t smem = static_cast<size_t>(max_slabs) * 32 * sizeof(uint32_t);
-    if (smem > 200u * 1024u) return cudaErrorInvalidValue;
+    const size_t smem = static_cast<size_t>(max_slabs) * 32 * sizeof(uint32_t);  // the caller keeps H <= kDewarpMaxRows
     if (dtype == OB_F64) {
         if (smem > 48u * 1024u) {
             e = cudaFuncSetAttribute(k3_fused_kernel<double>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));

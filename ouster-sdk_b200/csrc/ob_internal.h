@@ -104,6 +104,9 @@ struct K3Frame {
     unsigned first_block;        // logical index of the frame's first CTA (sum of n_cg of the frames before)
     unsigned index;              // the frame's index in the set (reported as frame_idx)
 };
+// tallest frame K3 takes: a CTA keeps one count per (16-row slab, column) for its 32 columns in shared memory, and
+// 1600 slabs of them are 200 KB
+constexpr size_t kDewarpMaxRows = 25600;
 size_t dewarp_scan_scratch_bytes(unsigned n_blocks, unsigned n_frames);
 // *frame_end_dev: device array [n_frames], points up to and including frame f (valid when the launch is done)
 cudaError_t launch_dewarp_fused(const K3Frame* frames_dev, unsigned n_frames, unsigned n_blocks, unsigned max_slabs,

@@ -207,6 +207,10 @@ int main() {
         CHECK(std::memcmp(set_pts.data(), world.data(), sizeof(double) * 3 * world.rows()) == 0);
         CHECK(std::memcmp(set_pts.data() + 3 * world.rows(), second.data(), sizeof(double) * 3 * second.rows()) == 0);
         CHECK(fidx.front() == 0 && fidx.back() == 2);
+        // a window the reference cannot convert to uint32 millimetres throws; 4294967.295 m keeps every range
+        expect_throw<std::invalid_argument>([&] { dewarp<double>(posed, lut, 0.0, HUGE_VAL); }, "range window");
+        expect_throw<std::invalid_argument>([&] { dewarp<double>(set, luts, -1.0, 50.0); }, "range window");
+        CHECK(dewarp<double>(posed, lut, 0.0, 4294967.295).rows() >= world.rows());
     }
 
     // ---- surface normals on the destaggered cloud (ouster/algorithm/normals.h) ----

@@ -191,12 +191,15 @@ def _lut_and_frames(h, w, n_returns, seed):
     return lut_d, off, items
 
 
-@pytest.mark.parametrize("n_returns", [1, 2])
+@pytest.mark.parametrize("n_returns,h,w,repeat", [
+    pytest.param(1, 64, 1024, 1, id="1"), pytest.param(2, 64, 1024, 1, id="2"),
+    # 12 items of 256 CTAs: a look-back chain of 3072 CTAs, more than an H100 holds at once
+    pytest.param(2, 128, 2048, 6, id="2-x6-128x2048")])
 @pytest.mark.parametrize("fields", [slice(0, 0), slice(0, 1), slice(3, 4), slice(0, 6)])
-def test_map_rows_bit_exact_against_the_exporter_step(ob, n_returns, fields):
-    h, w = 64, 1024
+def test_map_rows_bit_exact_against_the_exporter_step(ob, n_returns, h, w, repeat, fields):
     lut_d, off, items = _lut_and_frames(h, w, n_returns, 7 + n_returns)
     lut = ob.XYZLutT.from_arrays(lut_d, off, h, w)
+    items = [dict(it, range=np.roll(it["range"], 37 * k, axis=1)) for k in range(repeat) for it in items]
     its = [dict(it, fields=it["fields"][fields]) for it in items]
     want = xr.map_rows(its)
     got = ob.map_rows([dict(it, lut=lut) for it in its])

@@ -269,6 +269,33 @@ for i, (hh, ww) in enumerate(((16, 64), (24, 96))):
     want.append(orc.dewarp_frame(rg, d, o, poses, stt, tsn, 0.5, 40.0)[0])
 assert np.array_equal(ob.dewarp_frames(frames, 0.5, 40.0), np.concatenate(want))
 print("batched K3 ok")
+# K3 with later turns of the slab loop (1000 rows), more than 48 KB of shared memory (6160 rows), and a look-back
+# chain of 3072 CTAs (48 frames of 64 CTAs) with long runs of CTAs that emit nothing
+for dt in (np.float32, np.float64):
+    for hh, ww in ((1000, 33), (6160, 33)):
+        rg = random_range(hh, ww, 90, p_zero=0.3, max_range=50000)
+        d, o = random_lut(hh * ww, 91, dt)
+        poses = np.tile(np.eye(4), (ww, 1, 1))
+        poses[:, :3, 3] = np.random.default_rng(92).random((ww, 3))
+        stt = np.ones(ww, np.uint32)
+        tsn = np.arange(ww, dtype=np.uint64)
+        got = ob.dewarp_frame(ob.XYZLutT.from_arrays(d, o, hh, ww), rg, poses, stt, tsn, 0.5, 40.0, provenance=True)
+        for a, b in zip(got, orc.dewarp_frame(rg, d, o, poses, stt, tsn, 0.5, 40.0)):
+            assert np.array_equal(a, b), (hh, ww)
+hh, ww = 16, 2048
+d, o = random_lut(hh * ww, 93)
+lut = ob.XYZLutT.from_arrays(d, o, hh, ww)
+frames, want = [], []
+for i in range(48):
+    rg = random_range(hh, ww, 200 + i, p_zero=0.3, max_range=50000)
+    rg[:, (173 * i) % 1500:(173 * i) % 1500 + 400] = 0
+    poses = np.tile(np.eye(4), (ww, 1, 1))
+    poses[:, :3, 3] = np.random.default_rng(i).random((ww, 3))
+    stt = np.ones(ww, np.uint32)
+    frames.append({"lut": lut, "range": rg, "poses": poses, "status": stt})
+    want.append(orc.dewarp_frame(rg, d, o, poses, stt, np.zeros(ww, np.uint64), 0.5, 40.0)[0])
+assert np.array_equal(ob.dewarp_frames(frames, 0.5, 40.0), np.concatenate(want))
+print("K3 tall frames and 3072 CTAs ok")
 vp = np.random.default_rng(12).random((3000, 4)) * 3
 for code, name in ((orv.FIRST_N_POINT, "first_n"), (orv.AVERAGE_POINT, "average"), (orv.RANDOM, "random")):
     got, gi = ob.voxel_downsample(vp, 0.5, name, max_points_per_voxel=3, min_pts_threshold=2)
